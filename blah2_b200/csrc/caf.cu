@@ -1264,7 +1264,7 @@ static int caf_host_plan(const b200dd_caf_params *params, b200dd_caf *h) {
     cudaGetLastError();
   }
   plan_range(h);
-  if (h->log2m == 0) return geom_fail("b200dd_caf_create: nDelayBins too large for the range FFT (max ~7168)");
+  if (h->log2m == 0) return geom_fail("b200dd_caf_create: nDelayBins too large for the range FFT (max 8192)");
   int l2 = 8;
   while ((1 << l2) < 2 * (int)g.nDop - 1) l2++;
   h->log2m2 = l2;

@@ -351,7 +351,11 @@ template <class TMAP> __device__ __forceinline__ void interp_one(const InterpArg
   if (keep) {
     a.out.delay[i] = intDelay;
     a.out.doppler[i] = intDoppler;
-    a.out.snr[i] = fmax(fmax(intSnrDelay, intSnrDoppler), s);  // :86
+    // :86 std::max(std::max(intSnrDelay, intSnrDoppler), snr): (a < b) ? b : a keeps a NaN first argument, where fmax
+    // would drop it -- the NaN of a detection whose neighbours are both zero cells (10 log10 0 = -inf on each side;
+    // test_interpolate_with_all_zero_neighbours in tests/test_kernel_edges_gpu.py)
+    auto std_max = [](double a, double b) { return a < b ? b : a; };
+    a.out.snr[i] = std_max(std_max(intSnrDelay, intSnrDoppler), s);
   }
 }
 
