@@ -5,11 +5,11 @@
 //
 //   K0  caf_convert / caf_prerotate   complex128 -> complex64 (+ the dopplerMiddle != 0
 //                                     pre-rotation, Ambiguity.cpp:95-102)
-//   K1  caf_range_kernel<LOG2M>       per-batch range correlation (Ambiguity.cpp:106-149):
+//   K1  caf_range[_dit]_kernel<LOG2M> per-batch range correlation (Ambiguity.cpp:106-149):
 //                                     one CTA per batch, segmented power-of-two FFT
 //                                     cross-spectrum accumulated in registers, ONE inverse
 //                                     FFT per batch, nDelayBins lags written
-//   K2  caf_doppler_kernel<LOG2M>     DFT of odd length nDopplerBins down every delay
+//   K2  caf_doppler[_dit]_kernel<LOG2M> DFT of odd length nDopplerBins down every delay
 //                                     column (Ambiguity.cpp:152-169) as a Bluestein chirp-z
 //                                     in shared memory, fftshift folded into the store
 //
@@ -114,72 +114,20 @@ struct RangeArgs {
   long long validLo, validHi;  // elements [validLo, validHi) of x / y (relative to the pointers above) may be read
 };
 
-// ---- TMA (bulk async copy) staging of the IQ segments ---------------------------------------------
-// One elected thread per CTA issues cp.async.bulk global -> shared (SASS UBLKCP) for the NEXT segment's x
-// and y windows while the CTA computes the current one; completion is signalled on an mbarrier
-// (expect_tx / complete_tx), the other threads only spin on its phase bit.  Bulk copies need 16-byte
-// aligned addresses and sizes but float2 segments start on any 8-byte boundary (nCorr and the hop are
-// arbitrary), so the copy covers the 16-byte-aligned INTERIOR of the wanted range and the at most one
-// element on either side is read with an ordinary load -- no byte outside the caller's buffers is touched.
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                 : "=r"(done)
-                 : "r"(smem_u32(bar)), "r"(parity)
-                 : "memory");
-  } while (!done);
+// resident CTAs per SM the register allocator must leave room for: <= 128 registers per thread
+template <int LOG2M> constexpr int range_min_ctas() {
+  constexpr int NT = Plan<LOG2M>::NT;
+  return NT >= 512 ? 1 : (512 / NT > 16 ? 16 : 512 / NT);
 }
 
-// [g0, g1) wanted elements of a float2 array -> [s0, s1) the 16-byte aligned interior (may be empty)
-struct StageRange {
-  long long g0, s0, s1;
-};
-__device__ __forceinline__ StageRange stage_range(const float2 *base, long long g0, long long g1) {
-  StageRange r;
-  r.g0 = g0;
-  r.s0 = g0 + (long long)((reinterpret_cast<uintptr_t>(base + g0) >> 3) & 1);
-  r.s1 = g1 - (long long)((reinterpret_cast<uintptr_t>(base + g1) >> 3) & 1);
-  if (r.s1 < r.s0) r.s1 = r.s0;
-  return r;
-}
-
-// resident CTAs per SM the register allocator must leave room for
-template <int LOG2M, bool STAGE, int LR = 4> constexpr int range_min_ctas() {
-  constexpr int NT = Plan<LOG2M, LR>::NT;
-  if (STAGE) {  // shared memory (two FFT buffers + two staging buffers) is the limit, not registers
-    constexpr int smem = 2 * Plan<LOG2M, LR>::MP * 8 + 2 * Plan<LOG2M, LR>::M * 8 + 1024;
-    constexpr int by_smem = (227 * 1024) / smem;
-    return by_smem < 1 ? 1 : (by_smem > 8 ? 8 : by_smem);
-  }
-  return NT >= 512 ? 1 : (512 / NT > 16 ? 16 : 512 / NT);  // <= 128 regs/thread
-}
-
-// LR = log2 of the base radix: 4 (M/16 threads, three passes at M = 2048) or 3 (M/8 threads: twice the warps
-// per batch for CPIs with too few batches to fill the GPU, at the price of one more pass; B200DD_CAF_RADIX=8)
-template <int LOG2M, bool STAGE, int LR = 4>
-__global__ void __launch_bounds__(Plan<LOG2M, LR>::NT, range_min_ctas<LOG2M, STAGE, LR>()) caf_range_kernel(RangeArgs a) {
-  using P = Plan<LOG2M, LR>;
+// round-1 range kernel (fft_core.cuh, direct loads): the FFT lengths the DIT core does not cover, M = 256 and 8192
+template <int LOG2M>
+__global__ void __launch_bounds__(Plan<LOG2M>::NT, range_min_ctas<LOG2M>()) caf_range_kernel(RangeArgs a) {
+  using P = Plan<LOG2M>;
   constexpr int R = P::R;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float2 *A = reinterpret_cast<float2 *>(smem_raw);
   float2 *B = A + P::MP;
-  float2 *SX = B + P::MP;   // staging (STAGE only): x segment, then the y window
-  float2 *SY = SX + P::M;
-  __shared__ uint64_t mbar;
   const int tid = threadIdx.x;
   const int batch = a.batch0 + blockIdx.x;
   const long long boff = (long long)batch * a.nCorr;
@@ -197,69 +145,20 @@ __global__ void __launch_bounds__(Plan<LOG2M, LR>::NT, range_min_ctas<LOG2M, STA
   const int seg0 = blockIdx.y * a.segPerPart;
   const int seg1 = min(a.nSeg, seg0 + a.segPerPart);
 
-  // wanted element ranges of segment `seg`, relative to the start of the batch
-  auto seg_ranges = [&](int seg, StageRange &rx, StageRange &ry) {
-    const int n0 = seg * a.L;
-    const int len = min(a.L, a.nCorr - n0);
-    const int yoff = n0 + a.lagMin;
-    const int j0 = max(yoff, 0), j1 = max(j0, min(yoff + len + a.nDel - 1, a.nCorr));
-    rx = stage_range(xb, n0, n0 + len);
-    ry = stage_range(yb, j0, j1);
-  };
-  auto issue = [&](int seg) {  // one thread
-    StageRange rx, ry;
-    seg_ranges(seg, rx, ry);
-    const uint32_t bx = (uint32_t)(rx.s1 - rx.s0) * 8u, by = (uint32_t)(ry.s1 - ry.s0) * 8u;
-    mbar_expect_tx(&mbar, bx + by);
-    if (bx) bulk_g2s(SX, xb + rx.s0, bx, &mbar);
-    if (by) bulk_g2s(SY, yb + ry.s0, by, &mbar);
-  };
-  uint32_t phase = 0;
-  if constexpr (STAGE) {
-    if (tid == 0) {
-      mbar_init(&mbar, 1);
-      if (seg0 < seg1) issue(seg0);
-    }
-    __syncthreads();
-  }
-
   for (int seg = seg0; seg < seg1; seg++) {
     const int n0 = seg * a.L;
     const int len = min(a.L, a.nCorr - n0);
     const int ylen = len + a.nDel - 1;   // window entries that can reach a wanted lag
     const int yoff = n0 + a.lagMin;
-    auto stA = [&](int i, float2 v) { A[padr<LR>(i)] = v; };
-    auto stB = [&](int i, float2 v) { B[padr<LR>(i)] = v; };
-    StageRange rx, ry;
-    if constexpr (STAGE) seg_ranges(seg, rx, ry);
+    auto stA = [&](int i, float2 v) { A[pad(i)] = v; };
+    auto stB = [&](int i, float2 v) { B[pad(i)] = v; };
     // loaders: element m of the zero-padded x segment / of the y window masked to the batch
-    auto ldx = [&](int m) {
-      if constexpr (STAGE) {
-        const long long g = (long long)n0 + m;
-        const int idx = (int)(g - rx.s0);
-        float2 v = SX[min(max(idx, 0), P::M - 1)];
-        if (m < len && (g < rx.s0 || g >= rx.s1)) v = __ldg(xb + g);   // at most one element per side
-        return m < len ? v : zero;
-      } else {
-        return m < len ? __ldg(xb + n0 + m) : zero;
-      }
-    };
+    auto ldx = [&](int m) { return m < len ? __ldg(xb + n0 + m) : zero; };
     auto ldy = [&](int m) {
       const int j = yoff + m;
       const bool valid = m < ylen && j >= 0 && j < a.nCorr;
-      if constexpr (STAGE) {
-        const int idx = (int)((long long)j - ry.s0);
-        float2 v = SY[min(max(idx, 0), P::M - 1)];
-        if (valid && (j < ry.s0 || j >= ry.s1)) v = __ldg(yb + j);
-        return valid ? v : zero;
-      } else {
-        return valid ? __ldg(yb + j) : zero;
-      }
+      return valid ? __ldg(yb + j) : zero;
     };
-    if constexpr (STAGE) {
-      mbar_wait(&mbar, phase);
-      phase ^= 1;
-    }
     if (seg > seg0) __syncthreads();  // previous segment's last pass has finished reading A/B
     if constexpr (P::R0 == R) {
       fft_butterfly<float, R, -1, LOG2M>(tid, P::log2S(0), a.tw, ldx, stA);
@@ -272,34 +171,31 @@ __global__ void __launch_bounds__(Plan<LOG2M, LR>::NT, range_min_ctas<LOG2M, STA
       }
     }
     __syncthreads();
-    if constexpr (STAGE) {  // staging buffers are free again: fetch the next segment under the remaining passes
-      if (tid == 0 && seg + 1 < seg1) issue(seg + 1);
-    }
 #pragma unroll 1
     for (int p = 1; p < P::NP - 1; p++) {
-      smem_pass<float, LOG2M, -1, LR>(A, a.tw, p, tid);
-      smem_pass<float, LOG2M, -1, LR>(B, a.tw, p, tid);
+      smem_pass<float, LOG2M, -1>(A, a.tw, p, tid);
+      smem_pass<float, LOG2M, -1>(B, a.tw, p, tid);
       __syncthreads();
     }
     float2 vx[R], vy[R];
-    fwd_last_to_regs<float, LOG2M, LR>(A, tid, vx);
-    fwd_last_to_regs<float, LOG2M, LR>(B, tid, vy);
+    fwd_last_to_regs<float, LOG2M>(A, tid, vx);
+    fwd_last_to_regs<float, LOG2M>(B, tid, vy);
 #pragma unroll
     for (int r = 0; r < R; r++) cfmac(Z[r], vy[r], vx[r]);  // Z += Y conj(X)
   }
 
   __syncthreads();
-  inv_first_from_regs<float, LOG2M, LR>(A, tid, Z);
+  inv_first_from_regs<float, LOG2M>(A, tid, Z);
   __syncthreads();
 #pragma unroll 1
   for (int p = P::NP - 2; p >= 1; p--) {
-    smem_pass<float, LOG2M, +1, LR>(A, a.tw, p, tid);
+    smem_pass<float, LOG2M, +1>(A, a.tw, p, tid);
     __syncthreads();
   }
   // final inverse pass: natural-order lag index m = delay bin; keep m < nDel only
   const float scale = 1.0f / (float)P::M;
   float2 *__restrict__ Rrow = a.R + ((size_t)blockIdx.y * a.nDop + batch) * a.nDel;
-  auto ldA = [&](int i) { return A[padr<LR>(i)]; };
+  auto ldA = [&](int i) { return A[pad(i)]; };
   auto stR = [&](int m, float2 v) {
     if (m < a.nDel) Rrow[m] = make_float2(v.x * scale, v.y * scale);
   };
@@ -326,21 +222,6 @@ template <int LOG2M> struct RangeDit {
   static constexpr int kMinCtas = (227 * 1024) / (int)kSmem < 1 ? 1 : ((227 * 1024) / (int)kSmem > 16 ? 16 : (227 * 1024) / (int)kSmem);
 };
 
-struct TwPairF { float2 t1, t2; };
-
-template <int LOG2M, int DIR, class F>
-__device__ __forceinline__ void dit_transform_f32(float2 *A, const TwPairF &tw, int tid, float2 (&v)[16], F after_store) {
-  dit::pass0_store<float, LOG2M, DIR>(A, tid, v);
-  __syncthreads();
-  after_store();
-  dit::pass1_load<float, LOG2M>(A, tid, v);
-  dit::pass1_compute<float, LOG2M, DIR>(tw.t1, v);
-  dit::pass1_store<float, LOG2M>(A, tid, v);
-  __syncthreads();
-  dit::pass2_load<float, LOG2M>(A, tid, v);
-  dit::pass2_compute<float, LOG2M, DIR>(tw.t2, v);
-}
-
 template <int LOG2M>
 __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, (RangeDit<LOG2M>::kMinCtas * dit::Plan3<LOG2M>::NT > 512 ? 512 / dit::Plan3<LOG2M>::NT : RangeDit<LOG2M>::kMinCtas))
 caf_range_dit_kernel(RangeArgs a) {
@@ -358,9 +239,7 @@ caf_range_dit_kernel(RangeArgs a) {
   const float2 *__restrict__ xb = a.x + boff;
   const float2 *__restrict__ yb = a.y + boff;
   const float2 zero = make_float2(0.f, 0.f);
-  TwPairF tw;
-  tw.t1 = dit::pass1_twiddle<float, LOG2M>(a.tw, tid);
-  tw.t2 = dit::pass2_twiddle<float, LOG2M>(a.tw, tid);
+  const dit::TwPair<float> tw = dit::load_twiddles<float, LOG2M>(a.tw, tid);
 
   float2 Z[16];  // cross-spectrum of frequency tid + NT q in Z[q]
 #pragma unroll
@@ -438,131 +317,24 @@ caf_range_dit_kernel(RangeArgs a) {
     }
     // both staging buffers are consumed once every thread has passed the first barrier of the x transform:
     // the next segment's copies start there and have the rest of this segment to land
-    dit_transform_f32<LOG2M, -1>(A, tw, tid, vx, [&] {
+    dit::transform<float, LOG2M, -1>(A, tw, tid, vx, [&] {
       if (tid == 0 && seg + 1 < seg1) issue(seg + 1);
     });
     __syncthreads();
-    dit_transform_f32<LOG2M, -1>(A, tw, tid, vy, [] {});
+    dit::transform<float, LOG2M, -1>(A, tw, tid, vy);
 #pragma unroll
     for (int q = 0; q < 16; q++) cfmac(Z[q], vy[brev<16>(q)], vx[brev<16>(q)]);  // Z += Y conj(X)
     __syncthreads();
   }
 
   // one inverse transform per part; output sample m = tid + NT q is lag lagMin + m: keep m < nDel
-  dit_transform_f32<LOG2M, +1>(A, tw, tid, Z, [] {});
+  dit::transform<float, LOG2M, +1>(A, tw, tid, Z);
   const float scale = 1.0f / (float)P::M;
   float2 *__restrict__ Rrow = a.R + ((size_t)blockIdx.y * a.nDop + batch) * a.nDel;
 #pragma unroll
   for (int q = 0; q < 16; q++) {
     const int m = tid + NT * q;
     if (m < a.nDel) Rrow[m] = make_float2(Z[brev<16>(q)].x * scale, Z[brev<16>(q)].y * scale);
-  }
-}
-
-// ---- segment groups: several warps-groups of one CTA work on DIFFERENT segments of the same batch -----------
-// A CPI with few batches (257 at BASELINE config 1/2) cannot fill 132 SMs with one 4-warp CTA per batch: the
-// FMA pipe then idles with 2 warps per scheduler.  Splitting a batch
-// into `parts` CTAs buys occupancy but costs one more inverse FFT per part.  Here the CTA has G groups of NT
-// threads instead; group g transforms segments g, g + G, ... in its own pair of shared-memory buffers and
-// synchronises only with itself (named barrier g + 1, NT threads), the cross-spectra are accumulated in each
-// group's registers, added in group order through shared memory (deterministic) and group 0 alone runs the ONE
-// inverse transform.  Same arithmetic as G = 1 up to the order of the segment sum.
-template <int LOG2M, int G> constexpr int grouped_min_ctas() {
-  constexpr int T = Plan<LOG2M>::NT * G;
-  return T >= 512 ? 1 : 512 / T;
-}
-
-template <int LOG2M, int G>
-__global__ void __launch_bounds__(Plan<LOG2M>::NT * G, grouped_min_ctas<LOG2M, G>()) caf_range_grouped_kernel(RangeArgs a) {
-  using P = Plan<LOG2M>;
-  constexpr int R = P::R, NT = P::NT;
-  static_assert(G >= 2 && G <= 8 && NT * G <= 1024 && NT % 32 == 0, "group layout");
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int grp = threadIdx.x / NT;
-  const int tid = threadIdx.x - grp * NT;
-  float2 *A = reinterpret_cast<float2 *>(smem_raw) + (size_t)grp * 2 * P::MP;
-  float2 *B = A + P::MP;
-  auto gsync = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "n"(NT) : "memory"); };
-  const int batch = a.batch0 + blockIdx.x;
-  const long long boff = (long long)batch * a.nCorr;
-  const float2 *__restrict__ xb = a.x + boff;
-  const float2 *__restrict__ yb = a.y + boff;
-  const float2 zero = make_float2(0.f, 0.f);
-
-  float2 Z[R];
-#pragma unroll
-  for (int r = 0; r < R; r++) Z[r] = zero;
-  const int seg0 = blockIdx.y * a.segPerPart;
-  const int seg1 = min(a.nSeg, seg0 + a.segPerPart);
-
-  for (int seg = seg0 + grp; seg < seg1; seg += G) {
-    const int n0 = seg * a.L;
-    const int len = min(a.L, a.nCorr - n0);
-    const int ylen = len + a.nDel - 1;
-    const int yoff = n0 + a.lagMin;
-    auto stA = [&](int i, float2 v) { A[pad(i)] = v; };
-    auto stB = [&](int i, float2 v) { B[pad(i)] = v; };
-    auto ldx = [&](int m) { return m < len ? __ldg(xb + n0 + m) : zero; };
-    auto ldy = [&](int m) {
-      const int j = yoff + m;
-      return (m < ylen && j >= 0 && j < a.nCorr) ? __ldg(yb + j) : zero;
-    };
-    if (seg >= seg0 + G) gsync();  // this group's previous segment has finished reading A/B
-    if constexpr (P::R0 == R) {
-      fft_butterfly<float, R, -1, LOG2M>(tid, P::log2S(0), a.tw, ldx, stA);
-      fft_butterfly<float, R, -1, LOG2M>(tid, P::log2S(0), a.tw, ldy, stB);
-    } else {
-#pragma unroll 1
-      for (int b = tid; b < P::M / P::R0; b += NT) {
-        fft_butterfly<float, P::R0, -1, LOG2M>(b, P::log2S(0), a.tw, ldx, stA);
-        fft_butterfly<float, P::R0, -1, LOG2M>(b, P::log2S(0), a.tw, ldy, stB);
-      }
-    }
-    gsync();
-#pragma unroll 1
-    for (int p = 1; p < P::NP - 1; p++) {
-      smem_pass<float, LOG2M, -1>(A, a.tw, p, tid);
-      smem_pass<float, LOG2M, -1>(B, a.tw, p, tid);
-      gsync();
-    }
-    float2 vx[R], vy[R];
-    fwd_last_to_regs<float, LOG2M>(A, tid, vx);
-    fwd_last_to_regs<float, LOG2M>(B, tid, vy);
-#pragma unroll
-    for (int r = 0; r < R; r++) cfmac(Z[r], vy[r], vx[r]);  // Z += Y conj(X)
-  }
-
-  // hand the groups' cross-spectra to group 0 (each group parks its 16 values per thread in its own A)
-  gsync();
-  if (grp > 0) {
-#pragma unroll
-    for (int r = 0; r < R; r++) A[r * NT + tid] = Z[r];
-  }
-  __syncthreads();
-  if (grp > 0) return;
-#pragma unroll 1
-  for (int g = 1; g < G; g++) {
-    const float2 *Ag = A + (size_t)g * 2 * P::MP;
-#pragma unroll
-    for (int r = 0; r < R; r++) Z[r] = cadd(Z[r], Ag[r * NT + tid]);
-  }
-  inv_first_from_regs<float, LOG2M>(A, tid, Z);
-  gsync();
-#pragma unroll 1
-  for (int p = P::NP - 2; p >= 1; p--) {
-    smem_pass<float, LOG2M, +1>(A, a.tw, p, tid);
-    gsync();
-  }
-  const float scale = 1.0f / (float)P::M;
-  float2 *__restrict__ Rrow = a.R + ((size_t)blockIdx.y * a.nDop + batch) * a.nDel;
-  auto ldA = [&](int i) { return A[pad(i)]; };
-  auto stR = [&](int m, float2 v) {
-    if (m < a.nDel) Rrow[m] = make_float2(v.x * scale, v.y * scale);
-  };
-  constexpr int S0 = 1 << P::log2S(0);
-#pragma unroll 1
-  for (int b = tid; b < P::M / P::R0; b += NT) {
-    if ((b & (S0 - 1)) < a.nDel) fft_butterfly<float, P::R0, +1, LOG2M>(b, P::log2S(0), a.tw, ldA, stR);
   }
 }
 
@@ -709,9 +481,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT) caf_doppler_dit_kernel(
   const int col = a.col0 + blockIdx.x;
   const float2 zero = make_float2(0.f, 0.f);
   const size_t plane = (size_t)a.nDop * a.nDel;
-  TwPairF tw;
-  tw.t1 = dit::pass1_twiddle<float, LOG2M>(a.tw, tid);
-  tw.t2 = dit::pass2_twiddle<float, LOG2M>(a.tw, tid);
+  const dit::TwPair<float> tw = dit::load_twiddles<float, LOG2M>(a.tw, tid);
   float2 v[16], ch[16];
 #pragma unroll
   for (int k = 0; k < 16; k++) {
@@ -728,7 +498,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT) caf_doppler_dit_kernel(
   }
 #pragma unroll
   for (int k = 0; k < 16; k++) v[k] = tid + NT * k < a.nDop ? cmul(v[k], ch[k]) : zero;
-  dit_transform_f32<LOG2M, -1>(A, tw, tid, v, [] {});
+  dit::transform<float, LOG2M, -1>(A, tw, tid, v);
   float2 z[16];
 #pragma unroll
   for (int q = 0; q < 16; q++) z[q] = cmul(v[brev<16>(q)], __ldg(a.bhat + q * NT + tid));
@@ -736,7 +506,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT) caf_doppler_dit_kernel(
 #pragma unroll
   for (int q = 0; q < 16; q++) ch[q] = __ldg(a.chirp + min(tid + NT * q, a.nDop - 1));
   __syncthreads();
-  dit_transform_f32<LOG2M, +1>(A, tw, tid, z, [] {});
+  dit::transform<float, LOG2M, +1>(A, tw, tid, z);
   const float scale = 1.0f / (float)P::M;
   const int shift = a.nDop / 2 + 1;
 #pragma unroll
@@ -759,13 +529,11 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT) fft_forward_dit_kernel(
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float2 *A = reinterpret_cast<float2 *>(smem_raw);
   const int tid = threadIdx.x;
-  TwPairF t;
-  t.t1 = dit::pass1_twiddle<float, LOG2M>(tw, tid);
-  t.t2 = dit::pass2_twiddle<float, LOG2M>(tw, tid);
+  const dit::TwPair<float> t = dit::load_twiddles<float, LOG2M>(tw, tid);
   float2 v[16];
 #pragma unroll
   for (int k = 0; k < 16; k++) v[k] = in[tid + NT * k];
-  dit_transform_f32<LOG2M, -1>(A, t, tid, v, [] {});
+  dit::transform<float, LOG2M, -1>(A, t, tid, v);
 #pragma unroll
   for (int q = 0; q < 16; q++) out[q * NT + tid] = v[brev<16>(q)];
 }
@@ -857,37 +625,17 @@ __global__ void caf_widen_kernel(const float2 *__restrict__ in, double2 *__restr
 
 // ------------------------------------------------------------------ launch dispatch
 
-template <int LOG2M, bool STAGE, int LR = 4> int launch_range_impl(const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
-  using P = Plan<LOG2M, LR>;
-  const size_t smem = 2 * (size_t)P::MP * sizeof(float2) + (STAGE ? 2 * (size_t)P::M * sizeof(float2) : 0);
-  static bool attr_done[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!attr_done[dev & 63]) {
-    B2_CUDA(cudaFuncSetAttribute(caf_range_kernel<LOG2M, STAGE, LR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_done[dev & 63] = true;
-  }
-  caf_range_kernel<LOG2M, STAGE, LR><<<dim3(nDop, nParts), P::NT, smem, st>>>(a);
-  B2_LAUNCH_CHECK();
-  return B200DD_OK;
-}
-
-// TMA staging needs 2 more M-element buffers (fits up to M = 4096).  It measured no faster than direct
-// loads at config 1/2 and slower at config 3/4, so it is opt-in:
-// B200DD_CAF_TMA=1.  B200DD_CAF_RADIX=8 selects the radix-8 plan (M/8 threads per CTA).
-template <int LOG2M> int launch_range(const RangeArgs &a, int nDop, int nParts, cudaStream_t st);
-
-template <int LOG2M, int G> int launch_range_grouped(const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
+template <int LOG2M> int launch_range(const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
   using P = Plan<LOG2M>;
-  const size_t smem = (size_t)G * 2 * P::MP * sizeof(float2);
+  const size_t smem = 2 * (size_t)P::MP * sizeof(float2);
   static bool attr_done[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr_done[dev & 63]) {
-    B2_CUDA(cudaFuncSetAttribute(caf_range_grouped_kernel<LOG2M, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    B2_CUDA(cudaFuncSetAttribute(caf_range_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done[dev & 63] = true;
   }
-  caf_range_grouped_kernel<LOG2M, G><<<dim3(nDop, nParts), P::NT * G, smem, st>>>(a);
+  caf_range_kernel<LOG2M><<<dim3(nDop, nParts), P::NT, smem, st>>>(a);
   B2_LAUNCH_CHECK();
   return B200DD_OK;
 }
@@ -901,33 +649,6 @@ template <int LOG2M> int launch_range_dit(const RangeArgs &a, int nDop, int nPar
 template <int LOG2M> int prepare_range_dit() {
   B2_CUDA(cudaFuncSetAttribute(caf_range_dit_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RangeDit<LOG2M>::kSmem));
   return B200DD_OK;
-}
-
-// groups > 1: the grouped kernel (direct loads, radix 16) for the FFT lengths small CPIs use
-template <int LOG2M> int launch_range(const RangeArgs &a, int nDop, int nParts, int groups, cudaStream_t st) {
-  const char *e = getenv("B200DD_CAF_TMA"), *r = getenv("B200DD_CAF_RADIX");  // per call, like launch_range below
-  if ((e && atoi(e) == 1) || (r && atoi(r) == 8)) groups = 1;                  // those variants are ungrouped
-  if constexpr (LOG2M >= 10 && LOG2M <= 12) {
-    if constexpr (LOG2M <= 11) {  // 3+ groups of M = 4096 leave < 128 registers per thread (spills)
-      if (groups == 3) return launch_range_grouped<LOG2M, 3>(a, nDop, nParts, st);
-      if (groups >= 4) return launch_range_grouped<LOG2M, 4>(a, nDop, nParts, st);
-    }
-    if (groups >= 2) return launch_range_grouped<LOG2M, 2>(a, nDop, nParts, st);
-  }
-  return launch_range<LOG2M>(a, nDop, nParts, st);
-}
-
-template <int LOG2M> int launch_range(const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
-  const char *e = getenv("B200DD_CAF_TMA");  // read per call: the parity tests toggle it
-  const int env = e ? atoi(e) : 0;
-  const char *r = getenv("B200DD_CAF_RADIX");
-  if constexpr (LOG2M >= 9 && LOG2M <= 12) {
-    if (r && atoi(r) == 8) return launch_range_impl<LOG2M, false, 3>(a, nDop, nParts, st);
-  }
-  if constexpr (LOG2M <= 12) {
-    if (env == 1) return launch_range_impl<LOG2M, true>(a, nDop, nParts, st);
-  }
-  return launch_range_impl<LOG2M, false>(a, nDop, nParts, st);
 }
 
 template <int LOG2M> int launch_doppler(const DopplerArgs &a, cudaStream_t st) {
@@ -970,76 +691,50 @@ template <int LOG2M> int launch_fft_forward(const float2 *in, float2 *out, const
   return B200DD_OK;
 }
 
-int dispatch_range_dit(int log2m, const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
+// The FFT length picks the kernel: the DIT core (fft_dit.cuh) covers 512 .. 4096, the round-1 core (fft_core.cuh)
+// the other lengths.
+int dispatch_range(int log2m, const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
   switch (log2m) {
+    case 8: return launch_range<8>(a, nDop, nParts, st);
     case 9: return launch_range_dit<9>(a, nDop, nParts, st);
     case 10: return launch_range_dit<10>(a, nDop, nParts, st);
     case 11: return launch_range_dit<11>(a, nDop, nParts, st);
     case 12: return launch_range_dit<12>(a, nDop, nParts, st);
+    case 13: return launch_range<13>(a, nDop, nParts, st);
   }
   return geom_fail("range FFT length out of range");
 }
-int prepare_range_dit(int log2m) {
+// the DIT range kernels get their shared-memory limit once, at handle creation; the round-1 ones at their first launch
+int prepare_range(int log2m) {
   switch (log2m) {
     case 9: return prepare_range_dit<9>();
     case 10: return prepare_range_dit<10>();
     case 11: return prepare_range_dit<11>();
     case 12: return prepare_range_dit<12>();
   }
-  return geom_fail("range FFT length out of range");
-}
-
-int dispatch_range(int log2m, const RangeArgs &a, int nDop, int nParts, int groups, cudaStream_t st) {
-  switch (log2m) {
-    case 8: return launch_range<8>(a, nDop, nParts, st);
-    case 9: return launch_range<9>(a, nDop, nParts, st);
-    case 10: return launch_range<10>(a, nDop, nParts, groups, st);
-    case 11: return launch_range<11>(a, nDop, nParts, groups, st);
-    case 12: return launch_range<12>(a, nDop, nParts, groups, st);
-    case 13: return launch_range<13>(a, nDop, nParts, st);
-  }
-  return geom_fail("range FFT length out of range");
+  return B200DD_OK;
 }
 
 int dispatch_doppler(int log2m, const DopplerArgs &a, cudaStream_t st) {
   switch (log2m) {
     case 8: return launch_doppler<8>(a, st);
-    case 9: return launch_doppler<9>(a, st);
-    case 10: return launch_doppler<10>(a, st);
-    case 11: return launch_doppler<11>(a, st);
-    case 12: return launch_doppler<12>(a, st);
+    case 9: return launch_doppler_dit<9>(a, st);
+    case 10: return launch_doppler_dit<10>(a, st);
+    case 11: return launch_doppler_dit<11>(a, st);
+    case 12: return launch_doppler_dit<12>(a, st);
     case 13: return launch_doppler<13>(a, st);
     case 14: return launch_doppler<14>(a, st);
   }
   return geom_fail("Doppler FFT length out of range");
 }
 
-int dispatch_doppler_dit(int log2m, const DopplerArgs &a, cudaStream_t st) {
+int dispatch_fft_forward(int log2m, const float2 *in, float2 *out, const float2 *tw, cudaStream_t st) {
   switch (log2m) {
-    case 9: return launch_doppler_dit<9>(a, st);
-    case 10: return launch_doppler_dit<10>(a, st);
-    case 11: return launch_doppler_dit<11>(a, st);
-    case 12: return launch_doppler_dit<12>(a, st);
-  }
-  return geom_fail("Doppler FFT length out of range");
-}
-int dispatch_fft_forward_dit(int log2m, const float2 *in, float2 *out, const float2 *tw, cudaStream_t st) {
-  switch (log2m) {
+    case 8: return launch_fft_forward<8>(in, out, tw, st);
     case 9: return launch_fft_forward_dit<9>(in, out, tw, st);
     case 10: return launch_fft_forward_dit<10>(in, out, tw, st);
     case 11: return launch_fft_forward_dit<11>(in, out, tw, st);
     case 12: return launch_fft_forward_dit<12>(in, out, tw, st);
-  }
-  return geom_fail("FFT length out of range");
-}
-
-int dispatch_fft_forward(int log2m, const float2 *in, float2 *out, const float2 *tw, cudaStream_t st) {
-  switch (log2m) {
-    case 8: return launch_fft_forward<8>(in, out, tw, st);
-    case 9: return launch_fft_forward<9>(in, out, tw, st);
-    case 10: return launch_fft_forward<10>(in, out, tw, st);
-    case 11: return launch_fft_forward<11>(in, out, tw, st);
-    case 12: return launch_fft_forward<12>(in, out, tw, st);
     case 13: return launch_fft_forward<13>(in, out, tw, st);
     case 14: return launch_fft_forward<14>(in, out, tw, st);
   }
@@ -1066,9 +761,7 @@ struct b200dd_caf {
   int device = 0;
   cudaStream_t stream = nullptr;
   // range stage plan
-  int log2m = 12, nSeg = 1, L = 0, nParts = 1, segPerPart = 1, nGroups = 1;
-  bool dit_doppler = false;  // second-generation Doppler kernel: Bluestein lengths 512 .. 4096
-  bool dit_range = false;  // second-generation range kernel (fft_dit.cuh + TMA staging): FFT lengths 512 .. 4096
+  int log2m = 12, nSeg = 1, L = 0, nParts = 1, segPerPart = 1;
   int num_sms = 132;
   // doppler stage plan
   int log2m2 = 10;
@@ -1110,33 +803,19 @@ void plan_range(b200dd_caf *h) {
     if (h->nSeg < 1) h->nSeg = 1;
     h->L = (nCorr + h->nSeg - 1) / h->nSeg;
     h->nSeg = (nCorr + h->L - 1) / h->L;
-    // occupancy for CPIs with few batches (257 at BASELINE config 1/2 against 132 SMs): first give the CTA of a
-    // batch several segment GROUPS (caf_range_grouped_kernel: more warps per batch, still ONE inverse FFT),
-    // then, if that is still fewer than ~3 segment streams per SM, split the batch into parts (one more inverse
-    // FFT and one more partial range matrix each).  B200DD_CAF_GROUPS / B200DD_CAF_PARTS override.
+    // occupancy for CPIs with few batches (257 at BASELINE config 1/2 against 132 SMs): split a batch into parts,
+    // each with its own inverse FFT and partial range matrix, until there are ~3 CTAs per SM.  The DIT kernel
+    // (M = 512 .. 4096) keeps 4-5 CTAs resident per SM and stops once those are filled; the round-1 kernel does not
+    // split CPIs that already give every SM a batch.  B200DD_CAF_PARTS overrides.
     const int nDop = (int)h->g.nDop;
-    int want = nDop >= 3 * h->num_sms ? 1 : (3 * h->num_sms + nDop - 1) / nDop;  // segment streams per batch
-    // B200DD_CAF_KERNEL=legacy selects the round-1 kernels (and their TMA / radix-8 / group variants)
-    const char *kenv = getenv("B200DD_CAF_KERNEL");
-    const bool legacy = (kenv && strcmp(kenv, "legacy") == 0) || getenv("B200DD_CAF_TMA") || getenv("B200DD_CAF_RADIX") || getenv("B200DD_CAF_GROUPS");
-    h->dit_range = !legacy && best_l >= 9 && best_l <= 12;
-    int gmax = best_l == 12 ? 2 : 4;
-    if (best_l < 10 || best_l > 12 || h->dit_range) gmax = 1;
-    if (const char *r = getenv("B200DD_CAF_RADIX")) { if (atoi(r) == 8) gmax = 1; }
-    if (const char *t = getenv("B200DD_CAF_TMA")) { if (atoi(t) == 1) gmax = 1; }
-    int groups = want < gmax ? want : gmax;
-    if (const char *e = getenv("B200DD_CAF_GROUPS")) groups = atoi(e);
-    if (groups > gmax) groups = gmax;
-    if (groups > h->nSeg) groups = h->nSeg;
-    if (groups < 1) groups = 1;
-    h->nGroups = groups;
-    int parts = (want + groups - 1) / groups;
-    if (nDop >= h->num_sms && !h->dit_range) parts = 1;
-    // second-generation kernel: 4-5 CTAs are resident per SM; split batches into parts until they are filled once
-    if (h->dit_range && nDop * parts > 5 * h->num_sms) parts = (5 * h->num_sms) / nDop < 1 ? 1 : (5 * h->num_sms) / nDop;
+    int parts = nDop >= 3 * h->num_sms ? 1 : (3 * h->num_sms + nDop - 1) / nDop;
+    if (best_l >= 9 && best_l <= 12) {
+      if (nDop * parts > 5 * h->num_sms) parts = (5 * h->num_sms) / nDop < 1 ? 1 : (5 * h->num_sms) / nDop;
+    } else if (nDop >= h->num_sms) {
+      parts = 1;
+    }
     if (const char *e = getenv("B200DD_CAF_PARTS")) parts = atoi(e);
-    if (parts < 1) parts = 1;
-    if (parts * groups > h->nSeg) parts = h->nSeg / groups;
+    if (parts > h->nSeg) parts = h->nSeg;
     if (parts < 1) parts = 1;
     h->segPerPart = (h->nSeg + parts - 1) / parts;
     h->nParts = (h->nSeg + h->segPerPart - 1) / h->segPerPart;
@@ -1170,19 +849,12 @@ int caf_setup_device(b200dd_caf *h) {
   B2_CUDA(cudaMalloc(&d_bw, sizeof(float2) * M2));
   B2_CUDA(cudaMalloc(&h->d_bhat, sizeof(float2) * M2));
   B2_CUDA(cudaMemcpy(d_bw, bw.data(), sizeof(float2) * M2, cudaMemcpyHostToDevice));
-  {
-    const char *kenv = getenv("B200DD_CAF_KERNEL");
-    h->dit_doppler = !(kenv && strcmp(kenv, "legacy") == 0) && h->log2m2 >= 9 && h->log2m2 <= 12;
-  }
-  int rc = h->dit_doppler ? dispatch_fft_forward_dit(h->log2m2, d_bw, h->d_bhat, h->d_tw2, h->stream)
-                          : dispatch_fft_forward(h->log2m2, d_bw, h->d_bhat, h->d_tw2, h->stream);
+  int rc = dispatch_fft_forward(h->log2m2, d_bw, h->d_bhat, h->d_tw2, h->stream);
   if (rc != B200DD_OK) { cudaFree(d_bw); return rc; }
   B2_CUDA(cudaStreamSynchronize(h->stream));
   cudaFree(d_bw);
-  if (h->dit_range) {
-    rc = prepare_range_dit(h->log2m);
-    if (rc != B200DD_OK) return rc;
-  }
+  rc = prepare_range(h->log2m);
+  if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaMalloc(&h->d_R, sizeof(float2) * (size_t)h->nParts * g.nDop * g.nDel));
   B2_CUDA(cudaMalloc(&h->d_map, sizeof(float2) * (size_t)g.nDop * g.nDel));
   return B200DD_OK;
@@ -1207,8 +879,7 @@ int caf_run_device(b200dd_caf *h, const float2 *d_x, const float2 *d_y, float2 *
   ra.validLo = 0;
   ra.validHi = (long long)g.nDop * g.nCorr;
   if (ev) B2_CUDA(cudaEventRecord(ev[0], st));
-  int rc = h->dit_range ? dispatch_range_dit(h->log2m, ra, (int)g.nDop, h->nParts, st)
-                        : dispatch_range(h->log2m, ra, (int)g.nDop, h->nParts, h->nGroups, st);
+  int rc = dispatch_range(h->log2m, ra, (int)g.nDop, h->nParts, st);
   if (rc != B200DD_OK) return rc;
   if (ev) B2_CUDA(cudaEventRecord(ev[1], st));
   DopplerArgs da;
@@ -1223,7 +894,7 @@ int caf_run_device(b200dd_caf *h, const float2 *d_x, const float2 *d_y, float2 *
   da.col0 = 0;
   da.nCols = (int)g.nDel;
   da.ldOut = (int)g.nDel;
-  rc = h->dit_doppler ? dispatch_doppler_dit(h->log2m2, da, st) : dispatch_doppler(h->log2m2, da, st);
+  rc = dispatch_doppler(h->log2m2, da, st);
   if (rc != B200DD_OK) return rc;
   if (ev) B2_CUDA(cudaEventRecord(ev[2], st));
   return B200DD_OK;
@@ -1342,7 +1013,7 @@ int b200dd_caf_get_geometry(const b200dd_caf *h, b200dd_caf_geometry *out) {
   out->range_segments = (uint32_t)h->nSeg;
   out->range_hop = (uint32_t)h->L;
   out->range_parts = (uint32_t)h->nParts;
-  out->range_groups = (uint32_t)h->nGroups;
+  out->range_groups = 1;
   out->doppler_fft_len = 1u << h->log2m2;
   return B200DD_OK;
 }
@@ -1439,8 +1110,7 @@ int b200dd_caf_range_device(b200dd_caf *h, const void *d_x, const void *d_y, uin
   ra.segPerPart = h->segPerPart; ra.nDop = (int)g.nDop; ra.batch0 = (int)batch0;
   ra.validLo = (long long)batch0 * g.nCorr;
   ra.validHi = (long long)(batch0 + n_batches) * g.nCorr;
-  int rc = h->dit_range ? dispatch_range_dit(h->log2m, ra, (int)n_batches, h->nParts, st)
-                        : dispatch_range(h->log2m, ra, (int)n_batches, h->nParts, h->nGroups, st);
+  int rc = dispatch_range(h->log2m, ra, (int)n_batches, h->nParts, st);
   if (rc != B200DD_OK) return rc;
   const size_t plane = (size_t)g.nDop * g.nDel, first = (size_t)batch0 * g.nDel, count = (size_t)n_batches * g.nDel;
   caf_sum_parts_kernel<<<grid_for((uint32_t)count), 256, 0, st>>>(h->d_R, h->nParts, plane, first, count, (float2 *)d_R);
@@ -1459,7 +1129,7 @@ int b200dd_caf_doppler_device(b200dd_caf *h, const void *d_R, uint32_t col0, uin
   da.R = (const float2 *)d_R; da.nParts = 1; da.out = (float2 *)d_map_tile; da.chirp = h->d_chirp; da.bhat = h->d_bhat;
   da.tw = h->d_tw2; da.nDop = (int)g.nDop; da.nDel = (int)g.nDel; da.col0 = (int)col0; da.nCols = (int)n_cols;
   da.ldOut = (int)n_cols;
-  return h->dit_doppler ? dispatch_doppler_dit(h->log2m2, da, st) : dispatch_doppler(h->log2m2, da, st);
+  return dispatch_doppler(h->log2m2, da, st);
 }
 
 int b200dd_caf_place_tile_device(b200dd_caf *h, const void *d_tile, uint32_t col0, uint32_t n_cols, void *d_map, void *stream) {

@@ -117,9 +117,8 @@ B2_HD float2 csqr(float2 a) {
 template <class C> B2_HD C cconj(C a) { a.y = -a.y; return a; }
 template <class C, class T> B2_HD C cscale(C a, T s) { a.x *= s; a.y *= s; return a; }
 
-// padded shared-memory index: one pad element per base-radix group (LR = log2 of the base radix)
-template <int LR> B2_HD int padr(int i) { return i + (i >> LR); }
-B2_HD int pad(int i) { return padr<4>(i); }
+// padded shared-memory index: one pad element per 16
+B2_HD int pad(int i) { return i + (i >> 4); }
 B2_HD constexpr int padded_size(int m) { return m + (m >> 4); }
 
 // bit reversal of q within R = 2^k (compile-time folded when q is a constant)
@@ -224,19 +223,16 @@ template <class T, int R, int DIR> B2_HD void dft_reg(cpx<T> (&v)[R]) { Dif<T, R
 // ---------------------------------------------------------------------------------
 // Plan
 // ---------------------------------------------------------------------------------
-// LR = log2 of the base radix: 4 (radix-16 passes, M/16 threads; the FP32 kernels) or 3 (radix-8 passes,
-// M/8 threads: twice the warps per FFT and half the registers per thread; the FP64 kernels).
-template <int LOG2M, int LR = 4> struct Plan {
+template <int LOG2M> struct Plan {
   static_assert(LOG2M >= 8 && LOG2M <= 16, "supported FFT sizes: 256 .. 65536");
-  static_assert(LR == 3 || LR == 4, "base radix 8 or 16");
-  static constexpr int R = 1 << LR;
+  static constexpr int R = 16;
   static constexpr int M = 1 << LOG2M;
   static constexpr int NT = M / R;
-  static constexpr int NP = (LOG2M + LR - 1) / LR;
-  static constexpr int LOG2R0 = LOG2M - LR * (NP - 1);
+  static constexpr int NP = (LOG2M + 3) / 4;
+  static constexpr int LOG2R0 = LOG2M - 4 * (NP - 1);
   static constexpr int R0 = 1 << LOG2R0;
-  static constexpr int MP = M + (M >> LR);
-  B2_HD static constexpr int log2S(int p) { return LOG2M - LOG2R0 - LR * p; }  // stride of pass p
+  static constexpr int MP = M + (M >> 4);
+  B2_HD static constexpr int log2S(int p) { return LOG2M - LOG2R0 - 4 * p; }  // stride of pass p
 };
 
 // ---------------------------------------------------------------------------------
@@ -300,11 +296,11 @@ B2_HD void fft_butterfly(int b, int log2S, const cpx<T> *__restrict__ tw, LD ld,
 }
 
 // In-place shared-memory pass p of the plan (all butterflies owned by thread tid).
-template <class T, int LOG2M, int DIR, int LR = 4>
+template <class T, int LOG2M, int DIR>
 B2_HD void smem_pass(cpx<T> *s, const cpx<T> *__restrict__ tw, int p, int tid) {
-  using P = Plan<LOG2M, LR>;
-  auto ld = [&](int i) { return s[padr<LR>(i)]; };
-  auto st = [&](int i, cpx<T> v) { s[padr<LR>(i)] = v; };
+  using P = Plan<LOG2M>;
+  auto ld = [&](int i) { return s[pad(i)]; };
+  auto st = [&](int i, cpx<T> v) { s[pad(i)] = v; };
   if (p == 0) {
     if constexpr (P::R0 == P::R) {
       fft_butterfly<T, P::R, DIR, LOG2M>(tid, P::log2S(0), tw, ld, st);
@@ -319,22 +315,22 @@ B2_HD void smem_pass(cpx<T> *s, const cpx<T> *__restrict__ tw, int p, int tid) {
 
 // Last forward pass (stride 1): thread tid's R contiguous elements -> registers.
 // Register r holds the element whose digit-reversed POSITION is R*tid + brev<R>(r).
-template <class T, int LOG2M, int LR = 4> B2_HD void fwd_last_to_regs(const cpx<T> *s, int tid, cpx<T> (&v)[1 << LR]) {
-  constexpr int R = 1 << LR;
+template <class T, int LOG2M> B2_HD void fwd_last_to_regs(const cpx<T> *s, int tid, cpx<T> (&v)[16]) {
+  constexpr int R = 16;
 #pragma unroll
-  for (int k = 0; k < R; k++) v[k] = s[padr<LR>(R * tid + k)];
+  for (int k = 0; k < R; k++) v[k] = s[pad(R * tid + k)];
   dft_reg<T, R, -1>(v);
 }
 
 // First inverse pass (stride 1) from registers laid out as fwd_last_to_regs leaves them.
-template <class T, int LOG2M, int LR = 4> B2_HD void inv_first_from_regs(cpx<T> *s, int tid, const cpx<T> (&z)[1 << LR]) {
-  constexpr int R = 1 << LR;
+template <class T, int LOG2M> B2_HD void inv_first_from_regs(cpx<T> *s, int tid, const cpx<T> (&z)[16]) {
+  constexpr int R = 16;
   cpx<T> v[R];
 #pragma unroll
   for (int q = 0; q < R; q++) v[q] = z[brev<R>(q)];
   dft_reg<T, R, +1>(v);
 #pragma unroll
-  for (int k = 0; k < R; k++) s[padr<LR>(R * tid + k)] = v[brev<R>(k)];
+  for (int k = 0; k < R; k++) s[pad(R * tid + k)] = v[brev<R>(k)];
 }
 
 }  // namespace b2

@@ -276,5 +276,35 @@ template <class T, int LOG2M, int DIR> B2_HD void pass2_compute(const cpx<T> *__
   dft_tw<T, DIR, 16>(v, tw[tid]);
 }
 
+// ---- whole transform (device only: CTA barriers) -------------------------------------------------------------
+// the two twiddle bases of a thread, loaded once per kernel
+template <class T> struct TwPair { cpx<T> t1, t2; };
+template <class T, int LOG2M> __device__ __forceinline__ TwPair<T> load_twiddles(const cpx<T> *__restrict__ tw, int tid) {
+  TwPair<T> t;
+  t.t1 = pass1_twiddle<T, LOG2M>(tw, tid);
+  t.t2 = pass2_twiddle<T, LOG2M>(tw, tid);
+  return t;
+}
+
+// v (the thread's 16 inputs m = tid + NT k) -> its 16 outputs X[tid + NT q], left in v[brev16(q)].
+// Two CTA barriers inside; the caller adds one before the buffer is written again.  AFTER_STORE runs between the
+// first barrier and the middle pass: every thread has consumed its inputs by then, so that is where the NEXT
+// window's staging copy is started.
+template <class T, int LOG2M, int DIR, class F>
+__device__ __forceinline__ void transform(cpx<T> *A, const TwPair<T> &tw, int tid, cpx<T> (&v)[16], F after_store) {
+  pass0_store<T, LOG2M, DIR>(A, tid, v);
+  __syncthreads();
+  after_store();
+  pass1_load<T, LOG2M>(A, tid, v);
+  pass1_compute<T, LOG2M, DIR>(tw.t1, v);
+  pass1_store<T, LOG2M>(A, tid, v);
+  __syncthreads();
+  pass2_load<T, LOG2M>(A, tid, v);
+  pass2_compute<T, LOG2M, DIR>(tw.t2, v);
+}
+template <class T, int LOG2M, int DIR> __device__ __forceinline__ void transform(cpx<T> *A, const TwPair<T> &tw, int tid, cpx<T> (&v)[16]) {
+  transform<T, LOG2M, DIR>(A, tw, tid, v, [] {});
+}
+
 }  // namespace dit
 }  // namespace b2

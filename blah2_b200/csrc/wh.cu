@@ -100,44 +100,16 @@ struct CorrArgs {
   int nBins, L, nSegTotal, segPerCta;
 };
 
-// twiddle bases of a thread, loaded once per kernel (fft_dit.cuh pass1_twiddle / pass2_twiddle)
-struct TwPair { double2 t1, t2; };
-template <int LOG2M> __device__ __forceinline__ TwPair load_twiddles(const double2 *__restrict__ tw, int tid) {
-  TwPair t;
-  t.t1 = dit::pass1_twiddle<double, LOG2M>(tw, tid);
-  t.t2 = dit::pass2_twiddle<double, LOG2M>(tw, tid);
-  return t;
-}
-
-// v (the thread's 16 window elements m = tid + NT k) -> its 16 spectrum values X[tid + NT q], left in v[brev16(q)].
-// Two CTA barriers inside; the caller adds one before the buffer is written again.  AFTER_STORE runs between the
-// first barrier and the middle pass: every thread has consumed its inputs by then, so that is where the NEXT
-// window's staging copy is started.
-template <int LOG2M, int DIR, class F>
-__device__ __forceinline__ void dit_transform(double2 *A, const TwPair &tw, int tid, double2 (&v)[16], F after_store) {
-  dit::pass0_store<double, LOG2M, DIR>(A, tid, v);
-  __syncthreads();
-  after_store();
-  dit::pass1_load<double, LOG2M>(A, tid, v);
-  dit::pass1_compute<double, LOG2M, DIR>(tw.t1, v);
-  dit::pass1_store<double, LOG2M>(A, tid, v);
-  __syncthreads();
-  dit::pass2_load<double, LOG2M>(A, tid, v);
-  dit::pass2_compute<double, LOG2M, DIR>(tw.t2, v);
-}
-template <int LOG2M, int DIR> __device__ __forceinline__ void dit_transform(double2 *A, const TwPair &tw, int tid, double2 (&v)[16]) {
-  dit_transform<LOG2M, DIR>(A, tw, tid, v, [] {});
-}
-// Variant for kernels at the 128-register bound (two CTAs per SM): the two twiddle bases are requested at the top of
-// the transform -- the twiddle-free first pass covers their latency -- instead of living in registers across the
-// whole kernel.
+// Variant of dit::transform for kernels at the 128-register bound (two CTAs per SM): the two twiddle bases are
+// requested at the top of the transform -- the twiddle-free first pass covers their latency -- instead of living in
+// registers across the whole kernel.
 template <int LOG2M, int DIR, class F>
 __device__ __forceinline__ void dit_transform_ld(double2 *A, const double2 *__restrict__ twtab, int tid, double2 (&v)[16], F after_store) {
   const double2 *p1 = twtab + (tid & 15) * (dit::Plan3<LOG2M>::M / (16 * dit::Plan3<LOG2M>::RM)), *p2 = twtab + tid;
-  TwPair tw;
+  dit::TwPair<double> tw;
   asm volatile("ld.global.nc.v2.f64 {%0, %1}, [%2];" : "=d"(tw.t1.x), "=d"(tw.t1.y) : "l"(p1));
   asm volatile("ld.global.nc.v2.f64 {%0, %1}, [%2];" : "=d"(tw.t2.x), "=d"(tw.t2.y) : "l"(p2));
-  dit_transform<LOG2M, DIR>(A, tw, tid, v, after_store);
+  dit::transform<double, LOG2M, DIR>(A, tw, tid, v, after_store);
 }
 
 // One window of a channel: `lim` valid elements starting at circular index `start` of p (element m lives at
@@ -176,7 +148,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
   const TIN *__restrict__ x = reinterpret_cast<const TIN *>(a.x);
   const TIN *__restrict__ y = reinterpret_cast<const TIN *>(a.y);
   const double2 zero = make_double2(0.0, 0.0);
-  const TwPair tw = load_twiddles<LOG2M>(a.tw, tid);
+  const dit::TwPair<double> tw = dit::load_twiddles<double, LOG2M>(a.tw, tid);
 #pragma unroll
   for (int q = 0; q < 16; q++) {
     Za[q * NT + tid] = zero;
@@ -269,7 +241,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
       // next window (of this or the next segment): staged while this one is transformed
       const bool more = t < 2 || s + 1 < s1;
       const int ns = t < 2 ? s : s + 1, nt = t < 2 ? t + 1 : 0;
-      dit_transform<LOG2M, -1>(A, tw, tid, v, [&] {
+      dit::transform<double, LOG2M, -1>(A, tw, tid, v, [&] {
         if (more) {
           const WinDesc<TIN> dn = describe(ns, nt);
           if constexpr (kStage) {
@@ -307,7 +279,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
     double2 z[16];
 #pragma unroll
     for (int q = 0; q < 16; q++) z[q] = c == 0 ? za[q] : Z[q * NT + tid];
-    dit_transform<LOG2M, +1>(A, tw, tid, z);
+    dit::transform<double, LOG2M, +1>(A, tw, tid, z);
 #pragma unroll
     for (int q = 0; q < 16; q++) {
       const int m = tid + NT * q;
@@ -947,14 +919,14 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_wspec_kernel(cons
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2 *A = reinterpret_cast<double2 *>(smem_raw);
   const int tid = threadIdx.x;
-  const TwPair t = load_twiddles<LOG2M>(tw, tid);
+  const dit::TwPair<double> t = dit::load_twiddles<double, LOG2M>(tw, tid);
   double2 v[16];
 #pragma unroll
   for (int k = 0; k < 16; k++) {
     const int m = tid + NT * k;
     v[k] = m < nBins ? w[m] : make_double2(0.0, 0.0);
   }
-  dit_transform<LOG2M, -1>(A, t, tid, v);
+  dit::transform<double, LOG2M, -1>(A, t, tid, v);
 #pragma unroll
   for (int q = 0; q < 16; q++) what[q * NT + tid] = v[brev<16>(q)];
   if (tid == 0) *next_block = first_free;  // the filter kernel's work queue: blocks [0, grid) are taken by blockIdx

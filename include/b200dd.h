@@ -40,8 +40,6 @@
  *
  * Environment (all optional; default plans use the device's SM count, other heuristics not re-tuned on H100):
  *   B200DD_CAF_LOG2M / B200DD_CAF_PARTS      range-correlation FFT length (2^k) / CTAs per batch
- *   B200DD_CAF_GROUPS                        warp groups per range CTA, each on its own segments (1..4)
- *   B200DD_CAF_TMA=1                         stage IQ segments through shared memory with bulk async copies
  *   B200DD_WH_LOG2M, B200DD_WH_CORR_LOG2M, B200DD_WH_APPLY_LOG2M   WienerHopf FFT plans
  *   B200DD_WH_SOLVE_SPLIT=0                  one-barrier-per-step Toeplitz solve kernel also for <= 448 taps
  *   B200DD_WH_SOLVE_SHORT=0                  generic Toeplitz solve kernel also for <= 992 taps
@@ -113,7 +111,8 @@ typedef struct {
   uint32_t range_hop;       /* new samples per segment */
   uint32_t doppler_fft_len; /* Bluestein length M2 */
   uint32_t range_parts;     /* CTAs per batch (partial range matrices summed by the Doppler kernel) */
-  uint32_t range_groups;    /* warp groups per range CTA, each transforming its own segments of the batch */
+  uint32_t range_groups;    /* always 1 (one warp group per range CTA); kept so that the layout and the readers
+                               of this struct (bench.py) stay unchanged */
 } b200dd_caf_geometry;
 
 B200DD_API int b200dd_caf_create(const b200dd_caf_params *params, b200dd_caf **out);

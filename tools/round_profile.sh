@@ -20,7 +20,6 @@ timeout 200 ncu --set full --clock-control none --import-source on -k "$KF" --la
 timeout 200 ncu --set full --clock-control none --import-source on -k "regex:caf_range|caf_doppler" --launch-skip 4 -c 2 -f -o $O/${TAG}_full_cfg3 \
     python tools/profile_target.py cfg3 3 > $O/${TAG}_ncu_cfg3.log 2>&1
 timeout 100 python tools/time_caf.py cfg1 cfg3 cfg4 > $O/${TAG}_time_caf.log 2>&1
-B200DD_CAF_KERNEL=legacy timeout 100 python tools/time_caf.py cfg1 cfg3 cfg4 > $O/${TAG}_time_caf_legacy.log 2>&1
 timeout 60 python tools/wh_times.py > $O/${TAG}_wh_times.log 2>&1
 timeout 100 python tools/bench_cfg5.py 5 2>/dev/null | tail -1 > $O/${TAG}_cfg5_n1.log
 timeout 100 python tools/bench_cfg5.py 5 --no-filter 2>/dev/null | tail -1 >> $O/${TAG}_cfg5_n1.log

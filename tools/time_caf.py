@@ -21,9 +21,7 @@ def _peak():
 
 PEAK = _peak()
 
-def run(name, log2m=None, parts=None, iters=20, nbuf=8, groups=None):
-    if groups: os.environ["B200DD_CAF_GROUPS"] = str(groups)
-    else: os.environ.pop("B200DD_CAF_GROUPS", None)
+def run(name, log2m=None, parts=None, iters=20, nbuf=8):
     if log2m: os.environ["B200DD_CAF_LOG2M"] = str(log2m)
     else: os.environ.pop("B200DD_CAF_LOG2M", None)
     if parts: os.environ["B200DD_CAF_PARTS"] = str(parts)
@@ -56,20 +54,13 @@ def run(name, log2m=None, parts=None, iters=20, nbuf=8, groups=None):
     k_range = sum(a for a, _ in kr[2:]) / len(kr[2:])
     k_dop = sum(b for _, b in kr[2:]) / len(kr[2:])
     byts = 16 * g.n_used + 8 * g.n_doppler_bins * g.n_delay_bins
-    print(json.dumps(dict(cfg=name, groups=groups, range_ms=round(k_range, 5), doppler_ms=round(k_dop, 5), log2m=g.range_fft_len, nseg=g.range_segments, parts=g.range_parts, hop=g.range_hop, m2=g.doppler_fft_len,
+    print(json.dumps(dict(cfg=name, range_ms=round(k_range, 5), doppler_ms=round(k_dop, 5), log2m=g.range_fft_len, nseg=g.range_segments, parts=g.range_parts, hop=g.range_hop, m2=g.doppler_fft_len,
                           ms=round(ms, 4), maps_per_s=round(1e3 / ms, 1), msamples_per_s=round(n / ms / 1e3, 1),
                           gbs=round(byts / ms / 1e6, 1), frac=round(byts / (ms * 1e-3) / PEAK, 4))), flush=True)
     amb.close()
 
 if __name__ == "__main__":
     sweep = "--sweep" in sys.argv
-    if "--groups" in sys.argv:
-        for name in [a for a in sys.argv[1:] if not a.startswith("--")]:
-            for gr in (1, 2, 3, 4):
-                run(name, groups=gr)
-            run(name, groups=1, parts=2)
-            run(name, groups=2, parts=2)
-        sys.exit(0)
     for name in [a for a in sys.argv[1:] if not a.startswith("--")] or ["cfg1", "cfg3"]:
         run(name)
         if sweep:

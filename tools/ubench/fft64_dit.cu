@@ -20,7 +20,7 @@ using namespace b2;
 
 constexpr int LOG2M = 12;
 using PD = dit::Plan3<LOG2M>;
-using PO = Plan<LOG2M, 4>;
+using PO = Plan<LOG2M>;
 
 __global__ void __launch_bounds__(256, 1) k_old(const double2 *__restrict__ tw, int reps, double2 *sink) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -32,21 +32,21 @@ __global__ void __launch_bounds__(256, 1) k_old(const double2 *__restrict__ tw, 
   for (int it = 0; it < reps; it++) {
 #pragma unroll 1
     for (int p = 0; p < PO::NP - 1; p++) {
-      smem_pass<double, LOG2M, -1, 4>(A, tw, p, tid);
+      smem_pass<double, LOG2M, -1>(A, tw, p, tid);
       __syncthreads();
     }
     double2 v[16];
-    fwd_last_to_regs<double, LOG2M, 4>(A, tid, v);
+    fwd_last_to_regs<double, LOG2M>(A, tid, v);
     const double s = 1.0 / (double)PO::M;
 #pragma unroll
     for (int r = 0; r < 16; r++) { v[r].x *= s; v[r].y *= s; }
     acc.x += v[3].x; acc.y += v[5].y;
     __syncthreads();
-    inv_first_from_regs<double, LOG2M, 4>(A, tid, v);
+    inv_first_from_regs<double, LOG2M>(A, tid, v);
     __syncthreads();
 #pragma unroll 1
     for (int p = PO::NP - 2; p >= 0; p--) {
-      smem_pass<double, LOG2M, +1, 4>(A, tw, p, tid);
+      smem_pass<double, LOG2M, +1>(A, tw, p, tid);
       __syncthreads();
     }
   }

@@ -6,8 +6,8 @@
 //        tools/ubench/fft64_rates.cu && tools/ubench/fft64_rates
 //
 // Each CTA runs `reps` forward+inverse FFT pairs of M = 2^LOG2M complex doubles that never leave shared memory /
-// registers (inputs synthesised once), for the base radix 16 (M/16 threads) and 8 (M/8 threads), with one or two
-// CTAs per SM where shared memory allows.  Output: us per FFT per SM and the implied FP64 rate
+// registers (inputs synthesised once), radix 16 (M/16 threads), with one or more CTAs per SM where shared memory
+// allows.  Output: us per FFT per SM and the implied FP64 rate
 // (5 M log2 M flop per FFT) against 34 TFLOP/s / 132 SMs (H100 SXM data sheet).
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -17,14 +17,14 @@
 
 using namespace b2;
 
-template <int LOG2M, int LR>
-__global__ void __launch_bounds__(Plan<LOG2M, LR>::NT) k_fft(const double2 *__restrict__ tw, int reps, double2 *sink) {
-  using P = Plan<LOG2M, LR>;
+template <int LOG2M>
+__global__ void __launch_bounds__(Plan<LOG2M>::NT) k_fft(const double2 *__restrict__ tw, int reps, double2 *sink) {
+  using P = Plan<LOG2M>;
   constexpr int R = P::R;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2 *A = reinterpret_cast<double2 *>(smem_raw);
   const int tid = threadIdx.x;
-  for (int i = tid; i < P::M; i += P::NT) A[padr<LR>(i)] = make_double2(1e-3 * (i % 97) - 0.05, 2e-3 * (i % 89) - 0.08);
+  for (int i = tid; i < P::M; i += P::NT) A[pad(i)] = make_double2(1e-3 * (i % 97) - 0.05, 2e-3 * (i % 89) - 0.08);
   __syncthreads();
   double2 acc[R];
 #pragma unroll
@@ -33,25 +33,25 @@ __global__ void __launch_bounds__(Plan<LOG2M, LR>::NT) k_fft(const double2 *__re
     // forward: all passes in shared memory, last pass to registers
 #pragma unroll 1
     for (int p = 0; p < P::NP - 1; p++) {
-      smem_pass<double, LOG2M, -1, LR>(A, tw, p, tid);
+      smem_pass<double, LOG2M, -1>(A, tw, p, tid);
       __syncthreads();
     }
     double2 v[R];
-    fwd_last_to_regs<double, LOG2M, LR>(A, tid, v);
+    fwd_last_to_regs<double, LOG2M>(A, tid, v);
 #pragma unroll
     for (int r = 0; r < R; r++) { acc[r].x += v[r].x * 1e-9; acc[r].y += v[r].y * 1e-9; }
     __syncthreads();
     // inverse: from registers back to natural order in shared memory
-    inv_first_from_regs<double, LOG2M, LR>(A, tid, v);
+    inv_first_from_regs<double, LOG2M>(A, tid, v);
     __syncthreads();
 #pragma unroll 1
     for (int p = P::NP - 2; p >= 0; p--) {
-      smem_pass<double, LOG2M, +1, LR>(A, tw, p, tid);
+      smem_pass<double, LOG2M, +1>(A, tw, p, tid);
       __syncthreads();
     }
     // keep magnitudes bounded: the pair scales by M
     const double s = 1.0 / (double)P::M;
-    for (int i = tid; i < P::M; i += P::NT) { A[padr<LR>(i)].x *= s; A[padr<LR>(i)].y *= s; }
+    for (int i = tid; i < P::M; i += P::NT) { A[pad(i)].x *= s; A[pad(i)].y *= s; }
     __syncthreads();
   }
   double2 t = make_double2(0.0, 0.0);
@@ -60,8 +60,8 @@ __global__ void __launch_bounds__(Plan<LOG2M, LR>::NT) k_fft(const double2 *__re
   sink[blockIdx.x * P::NT + tid] = t;
 }
 
-template <int LOG2M, int LR> void run(int ctas_per_sm, int reps) {
-  using P = Plan<LOG2M, LR>;
+template <int LOG2M> void run(int ctas_per_sm, int reps) {
+  using P = Plan<LOG2M>;
   const int M = P::M;
   std::vector<double2> tw(M);
   for (int j = 0; j < M; j++) {
@@ -76,9 +76,9 @@ template <int LOG2M, int LR> void run(int ctas_per_sm, int reps) {
   const int grid = sms * ctas_per_sm;
   cudaMalloc(&d_sink, sizeof(double2) * grid * P::NT);
   const size_t smem = sizeof(double2) * P::MP;
-  cudaFuncSetAttribute(k_fft<LOG2M, LR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaFuncSetAttribute(k_fft<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_fft<LOG2M, LR>, P::NT, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_fft<LOG2M>, P::NT, smem);
   if (occ < ctas_per_sm) {
     printf("M=%5d radix %2d: %d CTAs/SM not resident (max %d), skipped\n", M, P::R, ctas_per_sm, occ);
     cudaFree(d_tw); cudaFree(d_sink);
@@ -86,10 +86,10 @@ template <int LOG2M, int LR> void run(int ctas_per_sm, int reps) {
   }
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
-  k_fft<LOG2M, LR><<<grid, P::NT, smem>>>(d_tw, 2, d_sink);
+  k_fft<LOG2M><<<grid, P::NT, smem>>>(d_tw, 2, d_sink);
   cudaDeviceSynchronize();
   cudaEventRecord(e0);
-  k_fft<LOG2M, LR><<<grid, P::NT, smem>>>(d_tw, reps, d_sink);
+  k_fft<LOG2M><<<grid, P::NT, smem>>>(d_tw, reps, d_sink);
   cudaEventRecord(e1);
   cudaEventSynchronize(e1);
   float ms = 0.f;
@@ -104,10 +104,8 @@ template <int LOG2M, int LR> void run(int ctas_per_sm, int reps) {
 
 int main() {
   const int reps = 200;
-  run<12, 4>(1, reps); run<12, 4>(2, reps); run<12, 4>(3, reps);
-  run<12, 3>(1, reps); run<12, 3>(2, reps);
-  run<11, 4>(2, reps); run<11, 4>(4, reps); run<11, 4>(6, reps);
-  run<11, 3>(2, reps); run<11, 3>(4, reps);
-  run<10, 4>(4, reps); run<10, 4>(8, reps);
+  run<12>(1, reps); run<12>(2, reps); run<12>(3, reps);
+  run<11>(2, reps); run<11>(4, reps); run<11>(6, reps);
+  run<10>(4, reps); run<10>(8, reps);
   return 0;
 }
