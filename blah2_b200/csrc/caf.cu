@@ -625,120 +625,73 @@ __global__ void caf_widen_kernel(const float2 *__restrict__ in, double2 *__restr
 
 // ------------------------------------------------------------------ launch dispatch
 
-template <int LOG2M> int launch_range(const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
-  using P = Plan<LOG2M>;
-  const size_t smem = 2 * (size_t)P::MP * sizeof(float2);
-  static bool attr_done[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!attr_done[dev & 63]) {
-    B2_CUDA(cudaFuncSetAttribute(caf_range_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_done[dev & 63] = true;
+// One kernel of a handle's plan: entry point, threads per CTA and dynamic shared memory.  Its shared-memory limit is
+// set once, when the handle is created.
+template <class... Args> struct Kernel {
+  void (*fn)(Args...) = nullptr;
+  int nt = 0;
+  size_t smem = 0;
+  int set_smem_limit() const {
+    B2_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    return B200DD_OK;
   }
-  caf_range_kernel<LOG2M><<<dim3(nDop, nParts), P::NT, smem, st>>>(a);
-  B2_LAUNCH_CHECK();
-  return B200DD_OK;
-}
-
-template <int LOG2M> int launch_range_dit(const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
-  using P = dit::Plan3<LOG2M>;
-  caf_range_dit_kernel<LOG2M><<<dim3(nDop, nParts), P::NT, RangeDit<LOG2M>::kSmem, st>>>(a);
-  B2_LAUNCH_CHECK();
-  return B200DD_OK;
-}
-template <int LOG2M> int prepare_range_dit() {
-  B2_CUDA(cudaFuncSetAttribute(caf_range_dit_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RangeDit<LOG2M>::kSmem));
-  return B200DD_OK;
-}
-
-template <int LOG2M> int launch_doppler(const DopplerArgs &a, cudaStream_t st) {
-  using P = Plan<LOG2M>;
-  const size_t smem = (size_t)P::MP * sizeof(float2);
-  static bool attr_done[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!attr_done[dev & 63]) {
-    B2_CUDA(cudaFuncSetAttribute(caf_doppler_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_done[dev & 63] = true;
+  int launch(dim3 grid, cudaStream_t st, Args... args) const {
+    fn<<<grid, nt, smem, st>>>(args...);
+    B2_LAUNCH_CHECK();
+    return B200DD_OK;
   }
-  caf_doppler_kernel<LOG2M><<<a.nCols, P::NT, smem, st>>>(a);
-  B2_LAUNCH_CHECK();
-  return B200DD_OK;
-}
+};
+using RangeKernel = Kernel<RangeArgs>;
+using DopplerKernel = Kernel<DopplerArgs>;
+using FftKernel = Kernel<const float2 *, float2 *, const float2 *>;
+// the Doppler stage at one length: the Doppler kernel, and the forward FFT of the Bluestein filter
+struct DopplerKernels {
+  DopplerKernel doppler;
+  FftKernel fft_forward;
+};
 
-template <int LOG2M> int launch_doppler_dit(const DopplerArgs &a, cudaStream_t st) {
-  using P = dit::Plan3<LOG2M>;
-  caf_doppler_dit_kernel<LOG2M><<<a.nCols, P::NT, (size_t)P::MP * sizeof(float2), st>>>(a);
-  B2_LAUNCH_CHECK();
-  return B200DD_OK;
+template <int LOG2M> RangeKernel range_r1() {
+  return {caf_range_kernel<LOG2M>, Plan<LOG2M>::NT, 2 * (size_t)Plan<LOG2M>::MP * sizeof(float2)};
 }
-template <int LOG2M> int launch_fft_forward_dit(const float2 *in, float2 *out, const float2 *tw, cudaStream_t st) {
-  using P = dit::Plan3<LOG2M>;
-  const size_t smem = (size_t)P::MP * sizeof(float2);
-  B2_CUDA(cudaFuncSetAttribute(fft_forward_dit_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  B2_CUDA(cudaFuncSetAttribute(caf_doppler_dit_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  fft_forward_dit_kernel<LOG2M><<<1, P::NT, smem, st>>>(in, out, tw);
-  B2_LAUNCH_CHECK();
-  return B200DD_OK;
+template <int LOG2M> RangeKernel range_dit() {
+  return {caf_range_dit_kernel<LOG2M>, dit::Plan3<LOG2M>::NT, RangeDit<LOG2M>::kSmem};
 }
-
-template <int LOG2M> int launch_fft_forward(const float2 *in, float2 *out, const float2 *tw, cudaStream_t st) {
+template <int LOG2M> DopplerKernels doppler_r1() {
   using P = Plan<LOG2M>;
-  const size_t smem = (size_t)P::MP * sizeof(float2);
-  B2_CUDA(cudaFuncSetAttribute(fft_forward_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  fft_forward_kernel<LOG2M><<<1, P::NT, smem, st>>>(in, out, tw);
-  B2_LAUNCH_CHECK();
-  return B200DD_OK;
+  return {{caf_doppler_kernel<LOG2M>, P::NT, (size_t)P::MP * sizeof(float2)},
+          {fft_forward_kernel<LOG2M>, P::NT, (size_t)P::MP * sizeof(float2)}};
+}
+template <int LOG2M> DopplerKernels doppler_dit() {
+  using P = dit::Plan3<LOG2M>;
+  return {{caf_doppler_dit_kernel<LOG2M>, P::NT, (size_t)P::MP * sizeof(float2)},
+          {fft_forward_dit_kernel<LOG2M>, P::NT, (size_t)P::MP * sizeof(float2)}};
 }
 
 // The FFT length picks the kernel: the DIT core (fft_dit.cuh) covers 512 .. 4096, the round-1 core (fft_core.cuh)
-// the other lengths.
-int dispatch_range(int log2m, const RangeArgs &a, int nDop, int nParts, cudaStream_t st) {
+// the other lengths.  A null entry point: no kernel for this length.
+RangeKernel range_kernel(int log2m) {
   switch (log2m) {
-    case 8: return launch_range<8>(a, nDop, nParts, st);
-    case 9: return launch_range_dit<9>(a, nDop, nParts, st);
-    case 10: return launch_range_dit<10>(a, nDop, nParts, st);
-    case 11: return launch_range_dit<11>(a, nDop, nParts, st);
-    case 12: return launch_range_dit<12>(a, nDop, nParts, st);
-    case 13: return launch_range<13>(a, nDop, nParts, st);
+    case 8: return range_r1<8>();
+    case 9: return range_dit<9>();
+    case 10: return range_dit<10>();
+    case 11: return range_dit<11>();
+    case 12: return range_dit<12>();
+    case 13: return range_r1<13>();
   }
-  return geom_fail("range FFT length out of range");
-}
-// the DIT range kernels get their shared-memory limit once, at handle creation; the round-1 ones at their first launch
-int prepare_range(int log2m) {
-  switch (log2m) {
-    case 9: return prepare_range_dit<9>();
-    case 10: return prepare_range_dit<10>();
-    case 11: return prepare_range_dit<11>();
-    case 12: return prepare_range_dit<12>();
-  }
-  return B200DD_OK;
+  return {};
 }
 
-int dispatch_doppler(int log2m, const DopplerArgs &a, cudaStream_t st) {
+DopplerKernels doppler_kernels(int log2m) {
   switch (log2m) {
-    case 8: return launch_doppler<8>(a, st);
-    case 9: return launch_doppler_dit<9>(a, st);
-    case 10: return launch_doppler_dit<10>(a, st);
-    case 11: return launch_doppler_dit<11>(a, st);
-    case 12: return launch_doppler_dit<12>(a, st);
-    case 13: return launch_doppler<13>(a, st);
-    case 14: return launch_doppler<14>(a, st);
+    case 8: return doppler_r1<8>();
+    case 9: return doppler_dit<9>();
+    case 10: return doppler_dit<10>();
+    case 11: return doppler_dit<11>();
+    case 12: return doppler_dit<12>();
+    case 13: return doppler_r1<13>();
+    case 14: return doppler_r1<14>();
   }
-  return geom_fail("Doppler FFT length out of range");
-}
-
-int dispatch_fft_forward(int log2m, const float2 *in, float2 *out, const float2 *tw, cudaStream_t st) {
-  switch (log2m) {
-    case 8: return launch_fft_forward<8>(in, out, tw, st);
-    case 9: return launch_fft_forward_dit<9>(in, out, tw, st);
-    case 10: return launch_fft_forward_dit<10>(in, out, tw, st);
-    case 11: return launch_fft_forward_dit<11>(in, out, tw, st);
-    case 12: return launch_fft_forward_dit<12>(in, out, tw, st);
-    case 13: return launch_fft_forward<13>(in, out, tw, st);
-    case 14: return launch_fft_forward<14>(in, out, tw, st);
-  }
-  return geom_fail("FFT length out of range");
+  return {};
 }
 
 std::vector<float2> twiddle_table_f32(int M) {
@@ -765,6 +718,8 @@ struct b200dd_caf {
   int num_sms = 132;
   // doppler stage plan
   int log2m2 = 10;
+  RangeKernel range;  // the kernels of (log2m, log2m2)
+  DopplerKernels dop;
   float2 *d_tw1 = nullptr, *d_tw2 = nullptr, *d_chirp = nullptr, *d_bhat = nullptr;
   float2 *d_R = nullptr, *d_map = nullptr;
   float2 *d_xrot = nullptr;                      // device path, dopplerMiddle != 0
@@ -824,6 +779,13 @@ void plan_range(b200dd_caf *h) {
 
 int caf_setup_device(b200dd_caf *h) {
   const HostGeom &g = h->g;
+  h->range = range_kernel(h->log2m);
+  h->dop = doppler_kernels(h->log2m2);
+  if (!h->range.fn || !h->dop.doppler.fn) return geom_fail("FFT length out of range");
+  int rc = h->range.set_smem_limit();
+  if (rc == B200DD_OK) rc = h->dop.doppler.set_smem_limit();
+  if (rc == B200DD_OK) rc = h->dop.fft_forward.set_smem_limit();
+  if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   const int M1 = 1 << h->log2m, M2 = 1 << h->log2m2;
   auto tw1 = twiddle_table_f32(M1), tw2 = twiddle_table_f32(M2);
@@ -849,12 +811,10 @@ int caf_setup_device(b200dd_caf *h) {
   B2_CUDA(cudaMalloc(&d_bw, sizeof(float2) * M2));
   B2_CUDA(cudaMalloc(&h->d_bhat, sizeof(float2) * M2));
   B2_CUDA(cudaMemcpy(d_bw, bw.data(), sizeof(float2) * M2, cudaMemcpyHostToDevice));
-  int rc = dispatch_fft_forward(h->log2m2, d_bw, h->d_bhat, h->d_tw2, h->stream);
+  rc = h->dop.fft_forward.launch(1, h->stream, d_bw, h->d_bhat, h->d_tw2);
   if (rc != B200DD_OK) { cudaFree(d_bw); return rc; }
   B2_CUDA(cudaStreamSynchronize(h->stream));
   cudaFree(d_bw);
-  rc = prepare_range(h->log2m);
-  if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaMalloc(&h->d_R, sizeof(float2) * (size_t)h->nParts * g.nDop * g.nDel));
   B2_CUDA(cudaMalloc(&h->d_map, sizeof(float2) * (size_t)g.nDop * g.nDel));
   return B200DD_OK;
@@ -879,7 +839,7 @@ int caf_run_device(b200dd_caf *h, const float2 *d_x, const float2 *d_y, float2 *
   ra.validLo = 0;
   ra.validHi = (long long)g.nDop * g.nCorr;
   if (ev) B2_CUDA(cudaEventRecord(ev[0], st));
-  int rc = dispatch_range(h->log2m, ra, (int)g.nDop, h->nParts, st);
+  int rc = h->range.launch(dim3(g.nDop, h->nParts), st, ra);
   if (rc != B200DD_OK) return rc;
   if (ev) B2_CUDA(cudaEventRecord(ev[1], st));
   DopplerArgs da;
@@ -894,7 +854,7 @@ int caf_run_device(b200dd_caf *h, const float2 *d_x, const float2 *d_y, float2 *
   da.col0 = 0;
   da.nCols = (int)g.nDel;
   da.ldOut = (int)g.nDel;
-  rc = dispatch_doppler(h->log2m2, da, st);
+  rc = h->dop.doppler.launch(da.nCols, st, da);
   if (rc != B200DD_OK) return rc;
   if (ev) B2_CUDA(cudaEventRecord(ev[2], st));
   return B200DD_OK;
@@ -1110,7 +1070,7 @@ int b200dd_caf_range_device(b200dd_caf *h, const void *d_x, const void *d_y, uin
   ra.segPerPart = h->segPerPart; ra.nDop = (int)g.nDop; ra.batch0 = (int)batch0;
   ra.validLo = (long long)batch0 * g.nCorr;
   ra.validHi = (long long)(batch0 + n_batches) * g.nCorr;
-  int rc = dispatch_range(h->log2m, ra, (int)n_batches, h->nParts, st);
+  int rc = h->range.launch(dim3(n_batches, h->nParts), st, ra);
   if (rc != B200DD_OK) return rc;
   const size_t plane = (size_t)g.nDop * g.nDel, first = (size_t)batch0 * g.nDel, count = (size_t)n_batches * g.nDel;
   caf_sum_parts_kernel<<<grid_for((uint32_t)count), 256, 0, st>>>(h->d_R, h->nParts, plane, first, count, (float2 *)d_R);
@@ -1129,7 +1089,7 @@ int b200dd_caf_doppler_device(b200dd_caf *h, const void *d_R, uint32_t col0, uin
   da.R = (const float2 *)d_R; da.nParts = 1; da.out = (float2 *)d_map_tile; da.chirp = h->d_chirp; da.bhat = h->d_bhat;
   da.tw = h->d_tw2; da.nDop = (int)g.nDop; da.nDel = (int)g.nDel; da.col0 = (int)col0; da.nCols = (int)n_cols;
   da.ldOut = (int)n_cols;
-  return dispatch_doppler(h->log2m2, da, st);
+  return h->dop.doppler.launch(da.nCols, st, da);
 }
 
 int b200dd_caf_place_tile_device(b200dd_caf *h, const void *d_tile, uint32_t col0, uint32_t n_cols, void *d_map, void *stream) {

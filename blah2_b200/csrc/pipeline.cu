@@ -4,7 +4,6 @@
 // defined here are the complex128 <-> complex64 conversions of the host entry point.
 #include "common.cuh"
 
-#include <cstdlib>
 #include <new>
 #include <vector>
 
@@ -64,8 +63,8 @@ struct b200dd_pipeline {
   float2 *d_map = nullptr;
   short4 *d_iq16 = nullptr;  // int16 ingest staging
   bool last_had_filter = false;
-  // CUDA-graph replay of the device chain (b200dd_pipeline_submit_device): one instantiated graph per distinct
-  // (d_x, d_y, d_map) triple, captured from the ordinary enqueue code the SECOND time a triple is seen
+  // CUDA-graph replay of the device chain (b200dd_pipeline_submit_device): one instantiated graph per
+  // (d_x, d_y, d_map) triple given to b200dd_pipeline_prepare_device
   struct GraphEntry {
     const void *x = nullptr, *y = nullptr;
     void *map = nullptr;
@@ -73,9 +72,7 @@ struct b200dd_pipeline {
     cudaGraphExec_t exec = nullptr;
   };
   std::vector<GraphEntry> graphs;
-  // 2 (default): replay only triples recorded by b200dd_pipeline_prepare_device; 1 (B200DD_PIPELINE_GRAPH=1): also
-  // record any triple on its second use; 0 (B200DD_PIPELINE_GRAPH=0): every submit eager, prepare is a no-op
-  int graph_mode = 2;
+  bool eager_only = false;  // the chain could not be captured: every submit eager, prepare is a no-op
 };
 
 extern "C" {
@@ -88,7 +85,6 @@ int b200dd_pipeline_create(const b200dd_pipeline_params *params, b200dd_pipeline
   b200dd_pipeline *h = new (std::nothrow) b200dd_pipeline();
   if (!h) return arg_fail("b200dd_pipeline_create: out of host memory");
   h->p = *params;
-  if (const char *e = getenv("B200DD_PIPELINE_GRAPH")) h->graph_mode = atoi(e) != 0 ? 1 : 0;
   auto fail = [&](int rc) { b200dd_pipeline_destroy(h); return rc; };
   int dev = params->caf.device;
   if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
@@ -190,76 +186,59 @@ static void pipeline_drop_graphs(b200dd_pipeline *h) {
   h->graphs.clear();
 }
 
+static const b200dd_pipeline::GraphEntry *pipeline_find_graph(const b200dd_pipeline *h, const void *d_x, const void *d_y,
+                                                              uint32_t n, const void *d_map) {
+  for (auto &e : h->graphs)
+    if (e.x == d_x && e.y == d_y && e.map == d_map && e.n == n) return &e;
+  return nullptr;
+}
+
 // A CPI is 12+ kernel launches on the single submitting thread.  The chain's arguments only depend on the caller's
 // three device pointers, so a triple can be recorded by stream capture (everything below runs on `st`; no
 // allocation, attribute call or host copy after the first eager run) and replayed with ONE cudaGraphLaunch.
 // Replay pays off in a submit -> fetch -> submit loop; in a deep queue of CPIs enqueued ahead eager launches can be
-// faster, so replay is opt-in per triple (b200dd_pipeline_prepare_device), or for every triple with B200DD_PIPELINE_GRAPH=1.
+// faster, so replay is opt-in per triple (b200dd_pipeline_prepare_device).
 int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
                                   void *stream) {
   if (!h || !d_x || !d_y) return arg_fail("b200dd_pipeline_submit_device: null argument");
   if (h->wh && n != h->p.caf.n_samples) return arg_fail("b200dd_pipeline_submit_device: the clutter filter needs exactly n_samples");
   DeviceGuard guard(h->device);
   void *st = stream ? stream : (void *)h->stream;
-  if (!h->graph_mode) return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
-  b200dd_pipeline::GraphEntry *hit = nullptr;
-  for (auto &e : h->graphs)
-    if (e.x == d_x && e.y == d_y && e.map == d_map && e.n == n) { hit = &e; break; }
-  if (!hit) {  // first sight: eager (sets function attributes, uploads the axes, sizes scratch buffers)
-    if (h->graph_mode == 1 && h->graphs.size() < 64) {
-      b200dd_pipeline::GraphEntry e;
-      e.x = d_x; e.y = d_y; e.map = d_map; e.n = n;
-      h->graphs.push_back(e);
-    }
-    return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
-  }
-  if (!hit->exec) {  // second sight: record
-    cudaGraph_t graph = nullptr;
-    if (cudaStreamBeginCapture((cudaStream_t)st, cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
-      cudaGetLastError();
-      return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
-    }
-    const int rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
-    const cudaError_t ce = cudaStreamEndCapture((cudaStream_t)st, &graph);
-    if (rc != B200DD_OK || ce != cudaSuccess || !graph) {
-      if (graph) cudaGraphDestroy(graph);
-      cudaGetLastError();
-      h->graph_mode = 0;  // something in the chain is not capturable here: stay eager from now on
-      return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);  // (a genuine error shows up again here)
-    }
-    cudaGraphExec_t exec = nullptr;
-    const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ie != cudaSuccess || !exec) {
-      cudaGetLastError();
-      h->graph_mode = 0;
-      return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
-    }
-    hit->exec = exec;
-  }
+  const b200dd_pipeline::GraphEntry *g = pipeline_find_graph(h, d_x, d_y, n, d_map);
+  if (!g) return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
   h->last_had_filter = h->wh != nullptr;
-  B2_CUDA(cudaGraphLaunch(hit->exec, (cudaStream_t)st));
+  B2_CUDA(cudaGraphLaunch(g->exec, (cudaStream_t)st));
   return B200DD_OK;
 }
 
 int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
                                    void *stream) {
   if (!h || !d_x || !d_y) return arg_fail("b200dd_pipeline_prepare_device: null argument");
-  if (!h->graph_mode) return B200DD_OK;
+  if (h->eager_only) return B200DD_OK;
+  if (h->wh && n != h->p.caf.n_samples) return arg_fail("b200dd_pipeline_prepare_device: the clutter filter needs exactly n_samples");
   DeviceGuard guard(h->device);
   void *st = stream ? stream : (void *)h->stream;
-  const int mode = h->graph_mode;
-  h->graph_mode = 1;  // record on second sight, for the two submits below
-  int rc = B200DD_OK;
-  for (int pass = 0; pass < 2 && rc == B200DD_OK; pass++) {  // first sight runs the chain eagerly, second sight records it
-    bool ready = false;
-    for (auto &e : h->graphs)
-      if (e.x == d_x && e.y == d_y && e.map == d_map && e.n == n && e.exec) ready = true;
-    if (ready) break;
-    rc = b200dd_pipeline_submit_device(h, d_x, d_y, n, d_map, st);
+  if (!pipeline_find_graph(h, d_x, d_y, n, d_map)) {
+    // the eager run sets up what a capture must not do (uploads the axes, sizes scratch buffers)
+    int rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
+    if (rc != B200DD_OK) return rc;
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    if (cudaStreamBeginCapture((cudaStream_t)st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+      rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
+      const cudaError_t ce = cudaStreamEndCapture((cudaStream_t)st, &graph);
+      if (rc == B200DD_OK && ce == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) != cudaSuccess) exec = nullptr;
+      if (graph) cudaGraphDestroy(graph);
+    }
+    if (exec) {
+      b200dd_pipeline::GraphEntry e;
+      e.x = d_x; e.y = d_y; e.map = d_map; e.n = n; e.exec = exec;
+      h->graphs.push_back(e);
+    } else {
+      cudaGetLastError();
+      h->eager_only = true;  // something in the chain is not capturable here: stay eager from now on
+    }
   }
-  if (h->graph_mode != 0) h->graph_mode = mode;  // (0 = the chain turned out not to be capturable: stay eager)
-  if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaStreamSynchronize((cudaStream_t)st));
   return B200DD_OK;
 }

@@ -1106,6 +1106,15 @@ std::vector<double2> twiddle_table_f64(int M) {
   return t;
 }
 
+// The samples a handle's kernels walk.  A whole signal: [0, N) through the reference's circular index map.  A chunk:
+// x and y are virtual pointers indexed by the GLOBAL sample number and the halos carry the circular wrap.
+struct Span {
+  uint32_t N;                    // modulus of the index map (2^31 for a chunk: no wrap)
+  uint32_t begin, end;           // the samples [begin, end)
+  XsMap xs;
+  long long xLo, xHi, yLo, yHi;  // readable element ranges of x / y relative to the pointers
+};
+
 }  // namespace
 
 struct b200dd_wh {
@@ -1116,20 +1125,20 @@ struct b200dd_wh {
   cudaStream_t stream = nullptr;
   int log2m_c = 12, log2m_a = 12;  // FFT lengths of the correlation / filter stages
   int L = 0, nSeg = 0, segPerCta = 1, gridCorr = 1;  // correlation stage
-  int Lout = 0, gridApply = 1;                       // filter stage
+  int Lout = 0, gridApply = 1, ctasApply = 1;       // filter stage: blocks, persistent CTAs
+  void (*solve)(SolveArgs) = nullptr;                // the solve kernel of the tap count
+  int solveThreads = 0;
+  Span span;
   double2 *d_tw_c = nullptr, *d_tw_a = nullptr, *d_partial = nullptr, *d_a = nullptr, *d_b = nullptr, *d_w = nullptr, *d_what = nullptr;
   int *d_status = nullptr;
   int *d_next_block = nullptr;  // work queue of the persistent filter CTAs
   double2 *d_xd = nullptr, *d_yd = nullptr;  // host path staging (complex128)
   int num_sms = 132;
-  bool solve_short = true;  // B200DD_WH_SOLVE_SHORT, read once at create
-  bool solve_split = true;  // B200DD_WH_SOLVE_SPLIT, read once at create
   // chunk mode (one CPI split over several GPUs): this handle filters the samples [c0, c0 + nc) of an N-sample signal
   bool chunked = false;
   uint32_t c0 = 0, nc = 0;
   int haloXL = 0, haloXR = 0, haloYR = 0;
   double2 *d_ab = nullptr;  // [2][nBins] this chunk's correlation sums (reduced over its CTAs)
-  bool attr_corr_f32 = false, attr_corr_f64 = false, attr_apply_f32 = false, attr_apply_f64 = false, attr_solve = false;
 };
 
 namespace {
@@ -1142,116 +1151,63 @@ template <int LOG2M> size_t fft_smem() { return (size_t)dit::Plan3<LOG2M>::MP * 
 // FFT buffer + TMA staging of one window (M + 2 float2) + mbarrier
 template <int LOG2M> size_t apply_smem() { return fft_smem<LOG2M>() + (size_t)(dit::Plan3<LOG2M>::M + 2) * sizeof(float2) + 16; }
 
-template <class TIN> constexpr bool is_f32() { return sizeof(TIN) == sizeof(float2); }
+// Calls f(std::integral_constant<int, LOG2M>) for the FFT length 2^log2m of a stage (512 .. 4096)
+template <class F> int with_log2m(int log2m, F &&f) {
+  switch (log2m) {
+    case 9: return f(std::integral_constant<int, 9>());
+    case 10: return f(std::integral_constant<int, 10>());
+    case 11: return f(std::integral_constant<int, 11>());
+    case 12: return f(std::integral_constant<int, 12>());
+  }
+  return geom_fail("WienerHopf FFT length out of range");
+}
 
 template <int LOG2M, class TIN> int wh_launch_corr(b200dd_wh *h, const void *x, const void *y, cudaStream_t st) {
-  using P = dit::Plan3<LOG2M>;
-  bool &done = is_f32<TIN>() ? h->attr_corr_f32 : h->attr_corr_f64;
-  if (!done) {
-    B2_CUDA(cudaFuncSetAttribute(wh_corr_kernel<LOG2M, TIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)corr_smem<LOG2M>()));
-    done = true;
-  }
+  const Span &s = h->span;
   CorrArgs ca;
   ca.x = x; ca.y = y; ca.partial = h->d_partial; ca.tw = h->d_tw_c;
-  if (h->chunked) {  // x, y are virtual pointers indexed by GLOBAL sample number; the halos carry the circular wrap
-    ca.N = 1u << 31; ca.nBegin = h->c0; ca.nEnd = h->c0 + h->nc;
-    ca.xs.N = 1u << 31; ca.xs.thr = 0; ca.xs.add1 = (uint32_t)(-h->delayMin); ca.xs.add2 = 0;
-    ca.xLo = (long long)h->c0 - h->haloXL; ca.xHi = (long long)h->c0 + h->nc + h->haloXR;
-    ca.yLo = (long long)h->c0; ca.yHi = (long long)h->c0 + h->nc + h->haloYR;
-  } else {
-    ca.N = h->N; ca.nBegin = 0; ca.nEnd = h->N; ca.xs = make_xs_map(h->N, h->delayMin);
-    ca.xLo = ca.yLo = 0; ca.xHi = ca.yHi = (long long)h->N;
-  }
+  ca.N = s.N; ca.nBegin = s.begin; ca.nEnd = s.end; ca.xs = s.xs;
+  ca.xLo = s.xLo; ca.xHi = s.xHi; ca.yLo = s.yLo; ca.yHi = s.yHi;
   ca.nBins = h->nBins; ca.L = h->L; ca.nSegTotal = h->nSeg; ca.segPerCta = h->segPerCta;
-  wh_corr_kernel<LOG2M, TIN><<<h->gridCorr, P::NT, corr_smem<LOG2M>(), st>>>(ca);
+  wh_corr_kernel<LOG2M, TIN><<<h->gridCorr, dit::Plan3<LOG2M>::NT, corr_smem<LOG2M>(), st>>>(ca);
   B2_LAUNCH_CHECK();
   return B200DD_OK;
 }
 
 template <int LOG2M, class TIN> int wh_launch_apply(b200dd_wh *h, const void *x, const void *y, void *y_out, cudaStream_t st) {
   using P = dit::Plan3<LOG2M>;
-  bool &done = is_f32<TIN>() ? h->attr_apply_f32 : h->attr_apply_f64;
-  if (!done) {
-    B2_CUDA(cudaFuncSetAttribute(wh_apply_kernel<LOG2M, TIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)apply_smem<LOG2M>()));
-    B2_CUDA(cudaFuncSetAttribute(wh_wspec_kernel<LOG2M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fft_smem<LOG2M>()));
-    done = true;
-  }
-  // persistent CTAs: as many as are resident at once (shared memory and the 128-register bound decide)
-  int per_sm = (int)((227 * 1024) / apply_smem<LOG2M>());
-  if (per_sm > wh_min_ctas<LOG2M>()) per_sm = wh_min_ctas<LOG2M>();
-  if (per_sm < 1) per_sm = 1;
-  int grid = h->num_sms * per_sm;
-  if (grid > h->gridApply) grid = h->gridApply;
-  wh_wspec_kernel<LOG2M><<<1, P::NT, fft_smem<LOG2M>(), st>>>(h->d_w, h->nBins, h->d_what, h->d_tw_a, h->d_next_block, grid);
+  wh_wspec_kernel<LOG2M><<<1, P::NT, fft_smem<LOG2M>(), st>>>(h->d_w, h->nBins, h->d_what, h->d_tw_a, h->d_next_block, h->ctasApply);
   B2_LAUNCH_CHECK();
+  const Span &s = h->span;
   ApplyArgs aa;
   aa.x = x; aa.y = y; aa.y_out = y_out; aa.what = h->d_what; aa.tw = h->d_tw_a; aa.status = h->d_status;
-  if (h->chunked) {
-    aa.N = 1u << 31; aa.iBegin = h->c0; aa.iEnd = h->c0 + h->nc;
-    aa.xs.N = 1u << 31; aa.xs.thr = 0; aa.xs.add1 = (uint32_t)(-h->delayMin); aa.xs.add2 = 0;
-    aa.xLo = (long long)h->c0 - h->haloXL; aa.xHi = (long long)h->c0 + h->nc + h->haloXR;
-  } else {
-    aa.N = h->N; aa.iBegin = 0; aa.iEnd = h->N; aa.xs = make_xs_map(h->N, h->delayMin);
-    aa.xLo = 0; aa.xHi = (long long)h->N;
-  }
+  aa.N = s.N; aa.iBegin = s.begin; aa.iEnd = s.end; aa.xs = s.xs; aa.xLo = s.xLo; aa.xHi = s.xHi;
   aa.nBins = h->nBins; aa.Lout = h->Lout; aa.nBlocks = h->gridApply; aa.next_block = h->d_next_block;
-  wh_apply_kernel<LOG2M, TIN><<<grid, P::NT, apply_smem<LOG2M>(), st>>>(aa);
+  wh_apply_kernel<LOG2M, TIN><<<h->ctasApply, P::NT, apply_smem<LOG2M>(), st>>>(aa);
   B2_LAUNCH_CHECK();
   return B200DD_OK;
 }
 
 int wh_launch_solve(b200dd_wh *h, cudaStream_t st) {
-  const size_t solve_smem = ((size_t)h->nBins * 6 + 16) * sizeof(double2);
-  const size_t solve_smem_max = ((size_t)kMaxBins * 6 + 16) * sizeof(double2);  // attribute is per function, not per handle
-  if (!h->attr_solve) {
-    B2_CUDA(cudaFuncSetAttribute(wh_solve_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem_max));
-    B2_CUDA(cudaFuncSetAttribute(wh_solve_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem_max));
-    B2_CUDA(cudaFuncSetAttribute(wh_solve_short_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem_max));
-    B2_CUDA(cudaFuncSetAttribute(wh_solve_short_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem_max));
-    B2_CUDA(cudaFuncSetAttribute(wh_solve_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem_max));
-    h->attr_solve = true;
-  }
   SolveArgs sa;
   sa.partial = h->chunked ? h->d_ab : h->d_partial; sa.nPartial = h->chunked ? 1 : h->gridCorr; sa.nBins = h->nBins;
   sa.a_out = h->d_a; sa.b_out = h->d_b; sa.w_out = h->d_w; sa.status = h->d_status;
-  const int threads = ((h->nBins + 31) / 32) * 32;
-  if (h->solve_split && 2 * threads + 96 <= 1024) {  // includes the reference's configuration (410 taps)
-    wh_solve_split_kernel<<<1, 2 * threads + 96, solve_smem, st>>>(sa);
-  } else if (h->solve_short && threads + 32 <= 1024) {
-    if (threads + 32 <= 512) wh_solve_short_kernel<512><<<1, threads + 32, solve_smem, st>>>(sa);
-    else wh_solve_short_kernel<1024><<<1, threads + 32, solve_smem, st>>>(sa);
-  } else if (h->nBins <= 1024) {
-    wh_solve_kernel<1><<<1, threads, solve_smem, st>>>(sa);
-  } else {
-    wh_solve_kernel<2><<<1, 1024, solve_smem, st>>>(sa);
-  }
+  h->solve<<<1, h->solveThreads, ((size_t)h->nBins * 6 + 16) * sizeof(double2), st>>>(sa);
   B2_LAUNCH_CHECK();
   return B200DD_OK;
 }
 
 template <class TIN> int wh_dispatch(b200dd_wh *h, const void *x, const void *y, void *y_out, cudaStream_t st,
                                      cudaEvent_t *ev = nullptr) {
-  int rc = B200DD_ERR_GEOMETRY;
   if (ev) B2_CUDA(cudaEventRecord(ev[0], st));
-  switch (h->log2m_c) {
-    case 9: rc = wh_launch_corr<9, TIN>(h, x, y, st); break;
-    case 10: rc = wh_launch_corr<10, TIN>(h, x, y, st); break;
-    case 11: rc = wh_launch_corr<11, TIN>(h, x, y, st); break;
-    case 12: rc = wh_launch_corr<12, TIN>(h, x, y, st); break;
-  }
-  if (rc != B200DD_OK) return rc == B200DD_ERR_GEOMETRY ? geom_fail("WienerHopf FFT length out of range") : rc;
+  int rc = with_log2m(h->log2m_c, [&](auto l) { return wh_launch_corr<decltype(l)::value, TIN>(h, x, y, st); });
+  if (rc != B200DD_OK) return rc;
   if (ev) B2_CUDA(cudaEventRecord(ev[1], st));
   rc = wh_launch_solve(h, st);
   if (rc != B200DD_OK) return rc;
   if (ev) B2_CUDA(cudaEventRecord(ev[2], st));
-  rc = B200DD_ERR_GEOMETRY;
-  switch (h->log2m_a) {
-    case 9: rc = wh_launch_apply<9, TIN>(h, x, y, y_out, st); break;
-    case 10: rc = wh_launch_apply<10, TIN>(h, x, y, y_out, st); break;
-    case 11: rc = wh_launch_apply<11, TIN>(h, x, y, y_out, st); break;
-    case 12: rc = wh_launch_apply<12, TIN>(h, x, y, y_out, st); break;
-  }
-  if (rc != B200DD_OK) return rc == B200DD_ERR_GEOMETRY ? geom_fail("WienerHopf FFT length out of range") : rc;
+  rc = with_log2m(h->log2m_a, [&](auto l) { return wh_launch_apply<decltype(l)::value, TIN>(h, x, y, y_out, st); });
+  if (rc != B200DD_OK) return rc;
   if (ev) B2_CUDA(cudaEventRecord(ev[3], st));
   return B200DD_OK;
 }
@@ -1279,14 +1235,22 @@ int wh_pick_log2m(const b200dd_wh *h, const char *env1, const char *env2, bool f
 }
 
 void wh_plan(b200dd_wh *h) {
-  if (const char *e = getenv("B200DD_WH_SOLVE_SHORT")) h->solve_short = atoi(e) != 0;
-  if (const char *e = getenv("B200DD_WH_SOLVE_SPLIT")) h->solve_split = atoi(e) != 0;
   h->log2m_c = wh_pick_log2m(h, "B200DD_WH_LOG2M", "B200DD_WH_CORR_LOG2M", false);
   h->log2m_a = wh_pick_log2m(h, "B200DD_WH_LOG2M", "B200DD_WH_APPLY_LOG2M", true);
   if (!h->log2m_c || !h->log2m_a) return;
+  Span &s = h->span;
+  if (h->chunked) {
+    s.N = 1u << 31; s.begin = h->c0; s.end = h->c0 + h->nc;
+    s.xs.N = 1u << 31; s.xs.thr = 0; s.xs.add1 = (uint32_t)(-h->delayMin); s.xs.add2 = 0;
+    s.xLo = (long long)h->c0 - h->haloXL; s.xHi = (long long)h->c0 + h->nc + h->haloXR;
+    s.yLo = (long long)h->c0; s.yHi = (long long)h->c0 + h->nc + h->haloYR;
+  } else {
+    s.N = h->N; s.begin = 0; s.end = h->N; s.xs = make_xs_map(h->N, h->delayMin);
+    s.xLo = s.yLo = 0; s.xHi = s.yHi = (long long)h->N;
+  }
+  const uint64_t span = s.end - s.begin;
   const int M = 1 << h->log2m_c;
   h->L = M - h->nBins + 1;
-  const uint64_t span = h->chunked ? h->nc : h->N;  // samples this handle's kernels walk
   h->nSeg = (int)((span + h->L - 1) / h->L);
   // CTAs resident at once: shared memory allows 1 (M=4096) or 2 (smaller) per SM
   const size_t smem = (size_t)(M + M / 16 + 2 * M) * sizeof(double2);
@@ -1300,6 +1264,45 @@ void wh_plan(b200dd_wh *h) {
   const int Ma = 1 << h->log2m_a;
   h->Lout = Ma - h->nBins + 1;
   h->gridApply = (int)((span + h->Lout - 1) / h->Lout);
+  // persistent filter CTAs: as many as are resident at once (shared memory and the 128-register bound decide)
+  h->ctasApply = with_log2m(h->log2m_a, [&](auto l) {
+    constexpr int LOG2M = decltype(l)::value;
+    int resident = (int)((227 * 1024) / apply_smem<LOG2M>());
+    if (resident > wh_min_ctas<LOG2M>()) resident = wh_min_ctas<LOG2M>();
+    if (resident < 1) resident = 1;
+    return h->num_sms * resident < h->gridApply ? h->num_sms * resident : h->gridApply;
+  });
+  // the tap count picks the solve kernel: 1-448 split (includes the reference's 410 taps), 449-480 short<512>,
+  // 481-992 short<1024>, 993-1024 generic<1>, 1025-2048 generic<2>
+  const int threads = ((h->nBins + 31) / 32) * 32;
+  if (2 * threads + 96 <= 1024) { h->solve = wh_solve_split_kernel; h->solveThreads = 2 * threads + 96; }
+  else if (threads + 32 <= 512) { h->solve = wh_solve_short_kernel<512>; h->solveThreads = threads + 32; }
+  else if (threads + 32 <= 1024) { h->solve = wh_solve_short_kernel<1024>; h->solveThreads = threads + 32; }
+  else if (h->nBins <= 1024) { h->solve = wh_solve_kernel<1>; h->solveThreads = threads; }
+  else { h->solve = wh_solve_kernel<2>; h->solveThreads = 1024; }
+}
+
+// Shared-memory limits of the kernels the plan launches.  A limit belongs to the function (per device), not to the
+// handle, so the solve kernel gets the largest any tap count needs.
+int wh_set_smem_limits(const b200dd_wh *h) {
+  constexpr cudaFuncAttribute kLimit = cudaFuncAttributeMaxDynamicSharedMemorySize;
+  int rc = with_log2m(h->log2m_c, [](auto l) {
+    constexpr int LOG2M = decltype(l)::value;
+    B2_CUDA(cudaFuncSetAttribute(wh_corr_kernel<LOG2M, float2>, kLimit, (int)corr_smem<LOG2M>()));
+    B2_CUDA(cudaFuncSetAttribute(wh_corr_kernel<LOG2M, double2>, kLimit, (int)corr_smem<LOG2M>()));
+    return B200DD_OK;
+  });
+  if (rc != B200DD_OK) return rc;
+  rc = with_log2m(h->log2m_a, [](auto l) {
+    constexpr int LOG2M = decltype(l)::value;
+    B2_CUDA(cudaFuncSetAttribute(wh_apply_kernel<LOG2M, float2>, kLimit, (int)apply_smem<LOG2M>()));
+    B2_CUDA(cudaFuncSetAttribute(wh_apply_kernel<LOG2M, double2>, kLimit, (int)apply_smem<LOG2M>()));
+    B2_CUDA(cudaFuncSetAttribute(wh_wspec_kernel<LOG2M>, kLimit, (int)fft_smem<LOG2M>()));
+    return B200DD_OK;
+  });
+  if (rc != B200DD_OK) return rc;
+  B2_CUDA(cudaFuncSetAttribute(h->solve, kLimit, (int)(((size_t)kMaxBins * 6 + 16) * sizeof(double2))));
+  return B200DD_OK;
 }
 
 }  // namespace
@@ -1359,6 +1362,8 @@ static int wh_create_impl(int32_t delay_min, int32_t delay_max, uint32_t n_sampl
   wh_plan(h);
   if (!h->log2m_c || !h->log2m_a) return fail(geom_fail("b200dd_wh_create: no FFT plan (needs nSamples >= 512 and nBins <= 2048)"));
   auto body = [&]() -> int {
+    const int rc = wh_set_smem_limits(h);
+    if (rc != B200DD_OK) return rc;
     B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     const int Mc = 1 << h->log2m_c, M = 1 << h->log2m_a;
     auto twc = twiddle_table_f64(Mc), twa = twiddle_table_f64(M);
@@ -1435,13 +1440,7 @@ int b200dd_wh_chunk_corr_device(b200dd_wh *h, const void *d_x_loc, const void *d
   // virtual pointers indexed by the GLOBAL sample number
   const float2 *xv = (const float2 *)d_x_loc - ((long long)h->c0 - h->haloXL);
   const float2 *yv = (const float2 *)d_y_loc - (long long)h->c0;
-  int rc = B200DD_ERR_GEOMETRY;
-  switch (h->log2m_c) {
-    case 9: rc = wh_launch_corr<9, float2>(h, xv, yv, st); break;
-    case 10: rc = wh_launch_corr<10, float2>(h, xv, yv, st); break;
-    case 11: rc = wh_launch_corr<11, float2>(h, xv, yv, st); break;
-    case 12: rc = wh_launch_corr<12, float2>(h, xv, yv, st); break;
-  }
+  const int rc = with_log2m(h->log2m_c, [&](auto l) { return wh_launch_corr<decltype(l)::value, float2>(h, xv, yv, st); });
   if (rc != B200DD_OK) return rc;
   const int n2 = 2 * h->nBins;
   wh_reduce_partials_kernel<<<(n2 + 255) / 256, 256, 0, st>>>(h->d_partial, h->gridCorr, n2, (double2 *)d_ab);
@@ -1462,14 +1461,7 @@ int b200dd_wh_chunk_filter_device(b200dd_wh *h, const void *d_ab, const void *d_
   const float2 *xv = (const float2 *)d_x_loc - ((long long)h->c0 - h->haloXL);
   const float2 *yv = (const float2 *)d_y_loc - (long long)h->c0;
   float2 *yo = (float2 *)d_y_out - (long long)h->c0;
-  rc = B200DD_ERR_GEOMETRY;
-  switch (h->log2m_a) {
-    case 9: rc = wh_launch_apply<9, float2>(h, xv, yv, yo, st); break;
-    case 10: rc = wh_launch_apply<10, float2>(h, xv, yv, yo, st); break;
-    case 11: rc = wh_launch_apply<11, float2>(h, xv, yv, yo, st); break;
-    case 12: rc = wh_launch_apply<12, float2>(h, xv, yv, yo, st); break;
-  }
-  return rc;
+  return with_log2m(h->log2m_a, [&](auto l) { return wh_launch_apply<decltype(l)::value, float2>(h, xv, yv, yo, st); });
 }
 
 int b200dd_wh_profile_device(b200dd_wh *h, const void *d_x, const void *d_y, void *d_y_out, void *stream,

@@ -41,10 +41,7 @@
  * Environment (all optional; default plans use the device's SM count, other heuristics not re-tuned on H100):
  *   B200DD_CAF_LOG2M / B200DD_CAF_PARTS      range-correlation FFT length (2^k) / CTAs per batch
  *   B200DD_WH_LOG2M, B200DD_WH_CORR_LOG2M, B200DD_WH_APPLY_LOG2M   WienerHopf FFT plans
- *   B200DD_WH_SOLVE_SPLIT=0                  one-barrier-per-step Toeplitz solve kernel also for <= 448 taps
- *   B200DD_WH_SOLVE_SHORT=0                  generic Toeplitz solve kernel also for <= 992 taps
- *   B200DD_PIPELINE_GRAPH=1 / 0              CUDA-graph replay of the device chain for every buffer triple / never
- *                                            (default: only triples given to b200dd_pipeline_prepare_device)
+ * They are read when a handle is created; the plan made then alone picks every kernel the handle launches.
  * None of them changes results beyond the rounding of a different FFT factorisation.
  */
 #ifndef B200DD_H
@@ -416,8 +413,8 @@ B200DD_API int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x
  * graph -- it runs the chain once on the buffers' current contents, captures and instantiates it and synchronises
  * the stream -- after which b200dd_pipeline_submit_device on the same triple is ONE cudaGraphLaunch.  Results are
  * identical either way.  Worth it for submit -> fetch -> submit loops over a fixed ring of buffers;
- * with many CPIs enqueued ahead eager launches can be faster, hence opt-in.  B200DD_PIPELINE_GRAPH=1 records
- * every triple on its second use without this call, B200DD_PIPELINE_GRAPH=0 turns replay off altogether. */
+ * with many CPIs enqueued ahead eager launches can be faster, hence opt-in: a triple that was never prepared is
+ * enqueued eagerly.  Where the chain cannot be captured, the pipeline stays eager and this call does nothing. */
 B200DD_API int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n,
                                               void *d_map, void *stream);
 B200DD_API int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double *o_delay,

@@ -154,11 +154,11 @@ def test_rspduo_int16_ingest_matches_complex128_entry(relerr):
     assert np.max(np.abs(dev["detections"].delay - host["detections"].delay)) < 1e-3
 
 
-def test_graph_replay_of_the_device_chain_is_bit_identical(monkeypatch):
-    """With B200DD_PIPELINE_GRAPH=1 b200dd_pipeline_submit_device records the chain for a (d_x, d_y, d_map) triple on
-    its second use and replays the CUDA graph afterwards: eager (B200DD_PIPELINE_GRAPH=0), first, recorded and replayed submissions must give
-    bit-identical maps, detections and metrics -- also when two input sets alternate, when the CONTENT of a buffer
-    changes between replays, and for a CPI whose filter fails (status word read after the replay)."""
+def test_graph_replay_of_the_device_chain_is_bit_identical():
+    """After b200dd_pipeline_prepare_device a (d_x, d_y, d_map) triple is replayed as one CUDA graph: replayed
+    submissions must give the maps, detections and metrics of a pipeline that never prepares (eager) bit for bit --
+    also when two prepared triples alternate, when the CONTENT of a buffer changes between replays, and for a CPI
+    whose filter fails (status word read after the replay)."""
     import torch
     d, geom, det, sc = _chain_fixture()
     clutter = tuple(int(v) for v in d["clutter"])
@@ -170,15 +170,15 @@ def test_graph_replay_of_the_device_chain_is_bit_identical(monkeypatch):
         r = pipe.fetch()
         return dmap.cpu().numpy().copy(), r
 
-    monkeypatch.setenv("B200DD_PIPELINE_GRAPH", "0")
     eager = Pipeline(*geom[:6], roundHamming=True, clutter=clutter, detection=det)
-    monkeypatch.setenv("B200DD_PIPELINE_GRAPH", "1")
     pipe = Pipeline(*geom[:6], roundHamming=True, clutter=clutter, detection=det)
     shape = (pipe.geometry.n_doppler_bins, pipe.geometry.n_delay_bins)
     em = torch.empty(shape, dtype=torch.complex64, device="cuda")
     gm = [torch.empty(shape, dtype=torch.complex64, device="cuda") for _ in range(2)]
     ref = [run(eager, k, em) for k in range(2)]
-    for rep in range(4):          # rep 0 eager, rep 1 records, rep 2.. replay; the two triples alternate
+    for k in range(2):
+        pipe.prepare_device(dx[k], dy[k], gm[k])
+    for rep in range(3):          # every submission a replay; the two triples alternate
         for k in range(2):
             m, r = run(pipe, k, gm[k])
             assert np.array_equal(m, ref[k][0]), (rep, k)
@@ -198,38 +198,33 @@ def test_graph_replay_of_the_device_chain_is_bit_identical(monkeypatch):
     assert r2["skipped"] and np.array_equal(m, m2)
 
 
-def test_prepare_device_records_the_graph_up_front(monkeypatch):
+def test_prepare_device_records_the_graph_up_front():
     """b200dd_pipeline_prepare_device = plan creation: afterwards the FIRST submit of the triple is already a replay and
-    gives the eager result bit for bit -- in the default mode (replay only for prepared triples) and with
-    B200DD_PIPELINE_GRAPH=1; with B200DD_PIPELINE_GRAPH=0 it is a no-op.  In the default mode a triple that was never
-    prepared stays eager however often it is submitted."""
+    gives the result of a pipeline that never prepares (eager) bit for bit, spectrum included.  A triple that was
+    never prepared stays eager however often it is submitted."""
     import torch
     d, geom, det, sc = _chain_fixture()
     clutter = tuple(int(v) for v in d["clutter"])
     dx = torch.from_numpy(sc.x.astype(np.complex64)).cuda()
     dy = torch.from_numpy(sc.y.astype(np.complex64)).cuda()
     outs = {}
-    for mode in ("0", "1", None):
-        if mode is None:
-            monkeypatch.delenv("B200DD_PIPELINE_GRAPH", raising=False)
-        else:
-            monkeypatch.setenv("B200DD_PIPELINE_GRAPH", mode)
+    for prepared in (False, True):
         pipe = Pipeline(*geom[:6], roundHamming=True, clutter=clutter, detection=det, spectrum_bandwidth=2000.0)
         dmap = torch.zeros((pipe.geometry.n_doppler_bins, pipe.geometry.n_delay_bins), dtype=torch.complex64, device="cuda")
         scratch = dx.clone()
-        pipe.prepare_device(scratch, dy, dmap)      # runs on whatever the buffers hold now ...
-        scratch.copy_(dx)                           # (same values here; the replay reads the buffers when it runs)
-        dmap.zero_()
+        if prepared:
+            pipe.prepare_device(scratch, dy, dmap)  # runs on whatever the buffers hold now ...
+            scratch.copy_(dx)                       # (same values here; the replay reads the buffers when it runs)
+            dmap.zero_()
         pipe.submit_device(scratch, dy, dmap)
         r = pipe.fetch()
-        outs[mode] = (dmap.cpu().numpy().copy(), r["noisePower"], r["detections"].delay.copy(), pipe.fetch_spectrum())
-        if mode is None:                            # an unprepared triple: eager, three times over
+        outs[prepared] = (dmap.cpu().numpy().copy(), r["noisePower"], r["detections"].delay.copy(), pipe.fetch_spectrum())
+        if prepared:                                # an unprepared triple: eager, three times over
             other = torch.zeros_like(dmap)
             for _ in range(3):
                 pipe.submit_device(dx, dy, other)
                 pipe.fetch()
-            assert np.array_equal(other.cpu().numpy(), outs[mode][0])
-    assert np.abs(outs["0"][0]).max() > 0
-    for mode in ("1", None):
-        assert np.array_equal(outs["0"][0], outs[mode][0]) and outs["0"][1] == outs[mode][1]
-        assert np.array_equal(outs["0"][2], outs[mode][2]) and np.array_equal(outs["0"][3], outs[mode][3])
+            assert np.array_equal(other.cpu().numpy(), outs[prepared][0])
+    assert np.abs(outs[False][0]).max() > 0
+    assert np.array_equal(outs[False][0], outs[True][0]) and outs[False][1] == outs[True][1]
+    assert np.array_equal(outs[False][2], outs[True][2]) and np.array_equal(outs[False][3], outs[True][3])

@@ -139,25 +139,24 @@ def test_every_fft_plan_gives_the_same_filter(log2m, relerr, monkeypatch):
     assert e[0] < 1e-9 and e[1] < 1e-9, f"radix {radix} M=2^{log2m}: {e}"
 
 
+# (n, delayMin, delayMax, seed): one tap, 33, 50, 410 (the reference's), 448 and 510 taps, then every solve kernel at both
+# ends of the tap range that picks it
 @pytest.mark.parametrize("case", [(20011, -10, 40, 2), (200000, -10, 400, 4), (150000, 0, 1, 5), (150000, -3, 30, 6),
-                                  (200000, -10, 438, 7), (200000, -10, 500, 8)])
-def test_all_solve_kernels_give_the_same_weights(case, relerr, monkeypatch):
-    """Three kernels run the same Schur + Levinson recursion: the split producer / consumer kernel (default up to 448
-    taps), the one-barrier-per-step short kernel (B200DD_WH_SOLVE_SPLIT=0; default up to 992 taps) and the generic
-    kernel (B200DD_WH_SOLVE_SHORT=0 as well).  Sizes: one tap, one warp, 410 (the reference's), the largest split
-    system (448 taps) and one beyond it (510: falls back to the short kernel)."""
+                                  (200000, -10, 438, 7), (200000, -10, 500, 8)]
+                         + [(100000, -10, nb - 10, nb) for nb in (449, 480, 481, 992, 993, 1024, 1025, 2048)])
+def test_all_solve_kernels_give_the_same_weights(case, relerr):
+    """The tap count picks the solve kernel: split producer / consumer (1-448 taps), one-barrier-per-step short kernel
+    with a 512- (449-480) or 1024-thread bound (481-992), generic kernel with one (993-1024) or two rows per thread
+    (1025-2048).  On the correlation sums of a scene every kernel gives the weights LAPACK gives for the kernel's own
+    Toeplitz system toeplitz(conj(a), a) w = b."""
+    import scipy.linalg as sla
     n, dm, dM, seed = case
     sc = _scene(n, seed)
-    ws = {}
-    for mode in (("1", "1"), ("0", "1"), ("0", "0")):
-        monkeypatch.setenv("B200DD_WH_SOLVE_SPLIT", mode[0])
-        monkeypatch.setenv("B200DD_WH_SOLVE_SHORT", mode[1])
-        wh = WienerHopf(dm, dM, n)
-        ok, _ = wh.process(sc.x, sc.y)
-        assert ok
-        ws[mode] = wh.debug_weights()[0]
-    assert relerr(ws[("1", "1")], ws[("0", "0")])[0] < 1e-11
-    assert relerr(ws[("0", "1")], ws[("0", "0")])[0] < 1e-11
+    wh = WienerHopf(dm, dM, n)
+    ok, _ = wh.process(sc.x, sc.y)
+    assert ok
+    w, a, b = wh.debug_weights()
+    assert relerr(w, np.linalg.solve(sla.toeplitz(np.conj(a), a), b))[0] < 1e-10
 
 
 def _ar_sequence(nb, seed, pole=0.9):
@@ -171,21 +170,29 @@ def _ar_sequence(nb, seed, pole=0.9):
     return a
 
 
+# every solve kernel at both ends of its tap range (1-448, 449-480, 481-992, 993-1024, 1025-2048), each with a
+# first-pivot, early, mid-recursion and last-pivot failure
+_SOLVE_ENDS = [(nb, bad) for nb in (449, 480, 481, 992, 993, 1024, 1025, 2048)
+               for bad in (None, 0, 1, nb // 2, nb - 1) if (nb, bad) not in ((480, None), (480, 479))]
+
+
 @pytest.mark.parametrize("nb,bad_at", [(1, None), (1, 0), (32, None), (33, None), (33, 1), (33, 20), (64, None), (65, 33),
                                        (410, None), (410, 1), (410, 30), (410, 31), (410, 215), (410, 409),
-                                       (448, None), (448, 447), (480, None), (480, 479), (496, None), (496, 495), (600, 300)])
-@pytest.mark.parametrize("mode", [("1", "1"), ("0", "1"), ("0", "0")])
-def test_solve_kernels_on_given_toeplitz_systems(nb, bad_at, mode, relerr, monkeypatch):
-    """The solve kernels on correlation sums handed in through the chunk API (b200dd_wh_chunk_filter_device): weights
-    against LAPACK on the matrix the reference builds (WienerHopf.cpp:85-97), and the 'not positive definite' verdict
-    -- WienerHopf.cpp:111-117: chol() fails -> process() returns false, y untouched -- when the leading minor of
-    order bad_at + 1 is the first indefinite one (first pivot / early / mid-recursion / last pivot)."""
+                                       (448, None), (448, 0), (448, 1), (448, 224), (448, 447), (480, None), (480, 479),
+                                       (496, None), (496, 495), (600, 300), (710, None), (1210, None)] + _SOLVE_ENDS)
+@pytest.mark.parametrize("mode", [(40000, 0), (120000, 0), (120000, 80000)])
+def test_solve_kernels_on_given_toeplitz_systems(nb, bad_at, mode, relerr):
+    """The solve kernel the tap count picks, on correlation sums handed in through the chunk API
+    (b200dd_wh_chunk_filter_device): weights against LAPACK on the matrix the reference builds (WienerHopf.cpp:85-97),
+    and the 'not positive definite' verdict -- WienerHopf.cpp:111-117: chol() fails -> process() returns false, y
+    untouched -- when the leading minor of order bad_at + 1 is the first indefinite one (first pivot / early /
+    mid-recursion / last pivot).  mode = (signal length, first sample) of the handle's 40000-sample chunk: the whole
+    signal, its first or its last chunk (the pass-through of a failed CPI writes the chunk's own samples)."""
     import scipy.linalg as sla
     import torch
     from blah2_b200.process import WienerHopfChunk
-    monkeypatch.setenv("B200DD_WH_SOLVE_SPLIT", mode[0])
-    monkeypatch.setenv("B200DD_WH_SOLVE_SHORT", mode[1])
     n = 40000
+    n_total, c0 = mode
     a = _ar_sequence(nb, nb)
     rng = np.random.default_rng(nb + 1)
     b = rng.standard_normal(nb) + 1j * rng.standard_normal(nb)
@@ -202,7 +209,7 @@ def test_solve_kernels_on_given_toeplitz_systems(nb, bad_at, mode, relerr, monke
     assert expect_ok == (bad_at is None)
     if bad_at:
         np.linalg.cholesky(A[:bad_at, :bad_at])          # ... and it is the FIRST bad minor
-    ch = WienerHopfChunk(0, nb, n, 0, n)
+    ch = WienerHopfChunk(0, nb, n_total, c0, n)
     xl, xr, yr = ch.halos()
     g = torch.Generator(device="cuda").manual_seed(5)
     x_loc = torch.view_as_complex(torch.randn((xl + n + xr, 2), device="cuda", generator=g))

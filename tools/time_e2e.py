@@ -4,7 +4,8 @@
 
 For CPIs in flight = 1, 2, 4, 8: ms per CPI of Pipeline.submit_host (complex128) and submit_host_rspduo (int16),
 beside the bare H2D copy of the same bytes from pinned memory and the device-resident chain, so that what bounds the
-end-to-end number (PCIe, the kernels, or the host loop) can be read off one table.
+end-to-end number (PCIe, the kernels, or the host loop) can be read off one table.  The device chain is timed eager
+and replayed as a CUDA graph (prepare_device); the host-fed legs run eager, as bench.py's e2e_rspduo_int16 does.
 """
 import json
 import os
@@ -70,13 +71,10 @@ def main(steps=24):
     torch.cuda.synchronize()
     out["h2d_c128_64MB"] = round((time.perf_counter() - t0) / 10 * 1e3, 4)
     for npipe in (1, 2, 4, 6, 8):
-        os.environ["B200DD_PIPELINE_GRAPH"] = "0"
         pipes = [Pipeline(**bench.GEOM, clutter=bench.CLUTTER, detection=bench.DET, device=0) for _ in range(npipe)]
         out[f"device_eager_x{npipe}"] = round(loop(pipes, lambda p, i: p.submit_device(dx, dy), steps), 4)
         for p in pipes:
-            p.close()
-        os.environ["B200DD_PIPELINE_GRAPH"] = "1"   # record every triple on its second use (the warm-up of loop())
-        pipes = [Pipeline(**bench.GEOM, clutter=bench.CLUTTER, detection=bench.DET, device=0) for _ in range(npipe)]
+            p.prepare_device(dx, dy)
         g = pipes[0].geometry
         hmaps = [torch.empty((g.n_doppler_bins, g.n_delay_bins), dtype=torch.complex128).pin_memory() for _ in range(npipe)]
         idx = {id(p): k for k, p in enumerate(pipes)}
