@@ -19,6 +19,7 @@ ERR_ARG = 1
 ERR_GEOMETRY = 2
 ERR_CUDA = 3
 ERR_CAPACITY = 4
+ERR_NONFINITE = 5
 FILTER_FAILED = 10
 
 DET_CFAR = 1
@@ -152,6 +153,19 @@ SIGNATURES = [
     ("b200dd_pipeline_stream", _VP, [_VP]),
     ("b200dd_pipeline_enable_spectrum", C.c_int, [_VP, C.c_double, C.POINTER(C.c_uint32)]),
     ("b200dd_pipeline_fetch_spectrum", C.c_int, [_VP, _VP, C.c_uint32]),
+    ("b200dd_pipeline_enable_map_json", C.c_int, [_VP, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_map_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
+    ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),
+    ("b200dd_mapjson_destroy", None, [_VP]),
+    ("b200dd_mapjson_render_device", C.c_int, [_VP, _VP, C.c_int, C.c_double, C.c_double, _VP]),
+    ("b200dd_mapjson_fetch", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
+    ("b200dd_mapjson_render_host", C.c_int, [_VP, _VP, C.c_double, C.c_double, C.c_uint64, _VP, C.c_size_t,
+                                             C.POINTER(C.c_size_t)]),
+    ("b200dd_mapjson_format_doubles_host", C.c_int, [_VP, C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_mapjson_format_doubles_device", C.c_int, [_VP, C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t),
+                                                       C.c_int32]),
+    ("b200dd_mapjson_debug_cell_values", C.c_int, [_VP, _VP, C.c_int, C.c_double, _VP, _VP]),
     ("b200dd_comm_get_unique_id", C.c_int, [_VP]),
     ("b200dd_comm_create", C.c_int, [C.c_int32, C.c_int32, _VP, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_comm_destroy", None, [_VP]),
@@ -235,6 +249,20 @@ def spectrum_plan(n, bandwidth):
     f = np.empty(g.n_frequency, dtype=np.float64)
     check(lib.b200dd_spectrum_plan(int(n), float(bandwidth), C.byref(g), ptr(f), f.shape[0]))
     return g, f
+
+
+def format_doubles(values, device=None) -> list:
+    """The text a map client receives for each double (written at two decimals, read back, written again), as
+    the formatter computes it on the host (device=None) or in a kernel on `device`; "" where a value has none."""
+    lib = load()
+    v = np.ascontiguousarray(np.asarray(values, dtype=np.float64).ravel())
+    n = C.c_size_t()
+    out = np.empty(v.size * 25 + 1, dtype=np.uint8)
+    if device is None:
+        check(lib.b200dd_mapjson_format_doubles_host(ptr(v), v.size, ptr(out), out.size, C.byref(n)))
+    else:
+        check(lib.b200dd_mapjson_format_doubles_device(ptr(v), v.size, ptr(out), out.size, C.byref(n), int(device)))
+    return out[:n.value].tobytes().decode("ascii").split(",") if v.size else []
 
 
 def device_count() -> int:

@@ -60,4 +60,11 @@ template <class T> inline void free_dev(T *&p) {
   p = nullptr;
 }
 
+// Hooks between translation units that the C ABI does not expose.
+// det.cu: device address of {noisePower, maxPower} as the async chain's set_metrics leaves them.
+const double *det_device_metrics(b200dd_det *h);
+// mapjson.cu: enqueue the body render of a float2 map whose noisePower is read from d_metrics[0] at run time and
+// whose header values are read back from d_metrics[0..1] by b200dd_mapjson_fetch.
+int mapjson_enqueue_with_metrics(b200dd_mapjson *h, const void *d_map, const double *d_metrics, cudaStream_t st);
+
 }  // namespace b2

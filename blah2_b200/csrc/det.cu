@@ -22,6 +22,7 @@
 // stays at the CFAR snr.  Fenced (undefined behaviour in the reference): a detection whose
 // neighbour cells fall outside the map is dropped instead of read out of bounds.
 #include "common.cuh"
+#include "scan.cuh"
 
 #include <cmath>
 #include <cstring>
@@ -42,36 +43,6 @@ template <class TMAP> __device__ __forceinline__ double2 ld_cell(const TMAP *m, 
 
 // 10 log10 |z|  (Map.cpp:198, CfarDetector1D.cpp:48, Interpolate.cpp:50)
 __device__ __forceinline__ double db_abs(double2 z) { return 10.0 * log10(hypot(z.x, z.y)); }
-
-// exclusive prefix sum of v over a block of BS threads; total = block sum.  wsum: BS/32 + 1 words.
-template <int BS> __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *wsum, uint32_t &total) {
-  constexpr int NW = BS / 32;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint32_t inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  if (lane == 31) wsum[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    const uint32_t w = lane < NW ? wsum[lane] : 0;
-    uint32_t winc = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, winc, o);
-      if (lane >= o) winc += t;
-    }
-    if (lane < NW) wsum[lane] = winc - w;
-    if (lane == 31) wsum[NW] = winc;
-  }
-  __syncthreads();
-  const uint32_t r = wsum[warp] + inc - v;
-  total = wsum[NW];
-  __syncthreads();
-  return r;
-}
 
 // ------------------------------------------------------------------ set_metrics
 template <class TMAP>
@@ -179,21 +150,6 @@ template <class TMAP> __global__ void __launch_bounds__(kBlock) cfar_flag_kernel
   if ((tid & 31) == 0 && my) atomicAdd(&row_count, my);
   __syncthreads();
   if (tid == 0) a.cnt[i] = row_count;
-}
-
-// exclusive scan of cnt[0..n) into off[0..n], off[n] = total; single block of 1024
-__global__ void __launch_bounds__(1024) scan_kernel(const uint32_t *cnt, uint32_t *off, int n, uint32_t *total) {
-  __shared__ uint32_t wsum[33];
-  uint32_t carry = 0;
-  for (int base = 0; base < n; base += 1024) {
-    const int i = base + threadIdx.x;
-    const uint32_t v = i < n ? cnt[i] : 0;
-    uint32_t tot;
-    const uint32_t ex = block_excl_scan<1024>(v, wsum, tot);
-    if (i < n) off[i] = carry + ex;
-    carry += tot;
-  }
-  if (threadIdx.x == 0) { off[n] = carry; *total = carry; }
 }
 
 struct DetList {
@@ -819,3 +775,6 @@ int b200dd_det_interpolate_host(b200dd_det *h, const double *delay, const double
 }
 
 }  // extern "C"
+
+// the device word pair {noisePower, maxPower} that the async chain's set_metrics writes (for the map-JSON stage)
+const double *b2::det_device_metrics(b200dd_det *h) { return h->d_metrics; }

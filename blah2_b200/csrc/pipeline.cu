@@ -1,6 +1,6 @@
 // pipeline.cu -- one CPI through WienerHopf -> Ambiguity -> set_metrics -> detection with all
 // intermediates resident in HBM (the body of the reference's process thread, src/blah2.cpp:268-287).
-// Composes the per-class handles of caf.cu / wh.cu / det.cu through their C ABI; the only kernels
+// Composes the per-class handles of caf.cu / wh.cu / det.cu / mapjson.cu through their C ABI; the only kernels
 // defined here are the complex128 <-> complex64 conversions of the host entry point.
 #include "common.cuh"
 
@@ -52,6 +52,8 @@ struct b200dd_pipeline {
   b200dd_wh *wh = nullptr;
   b200dd_det *det = nullptr;
   b200dd_spectrum *spec = nullptr;  // optional first stage (blah2.cpp:263-265)
+  b200dd_mapjson *mj = nullptr;     // optional last stage: the map document (blah2.cpp:303-304)
+  void *mj_stream = nullptr;        // stream of the last submit, where its document was rendered
   uint32_t spec_bins = 0, spec_nfft = 0;
   b200dd_caf_geometry g;
   std::vector<int32_t> delay;
@@ -129,6 +131,7 @@ void b200dd_pipeline_destroy(b200dd_pipeline *h) {
     pipeline_drop_graphs(h);
     b200dd_det_destroy(h->det);
     b200dd_spectrum_destroy(h->spec);
+    b200dd_mapjson_destroy(h->mj);
     free_dev(h->d_yf);
     free_dev(h->d_xd);
     free_dev(h->d_yd);
@@ -175,8 +178,11 @@ static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const vo
   if (rc != B200DD_OK) return rc;
   // Map::set_metrics runs after every Ambiguity::process, detection or not (blah2.cpp:278-279): stage 0 = metrics only
   const int last = h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0;
-  return b200dd_det_chain_device_async(h->det, last, map, h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(),
-                                       h->doppler.data(), st);
+  rc = b200dd_det_chain_device_async(h->det, last, map, h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(),
+                                     h->doppler.data(), st);
+  if (rc != B200DD_OK || !h->mj) return rc;
+  h->mj_stream = st;
+  return mapjson_enqueue_with_metrics(h->mj, map, det_device_metrics(h->det), (cudaStream_t)st);
 }
 
 
@@ -207,6 +213,7 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   const b200dd_pipeline::GraphEntry *g = pipeline_find_graph(h, d_x, d_y, n, d_map);
   if (!g) return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
   h->last_had_filter = h->wh != nullptr;
+  h->mj_stream = st;
   B2_CUDA(cudaGraphLaunch(g->exec, (cudaStream_t)st));
   return B200DD_OK;
 }
@@ -313,6 +320,11 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   rc = b200dd_det_chain_device_async(h->det, h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0, h->d_map,
                                      h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(), st);
   if (rc != B200DD_OK) return rc;
+  if (h->mj) {
+    h->mj_stream = st;
+    rc = mapjson_enqueue_with_metrics(h->mj, h->d_map, det_device_metrics(h->det), st);
+    if (rc != B200DD_OK) return rc;
+  }
   if (map_out) {
     const uint32_t cells = h->g.n_doppler_bins * h->g.n_delay_bins;
     pl_widen_kernel<<<grid_for(cells), 256, 0, st>>>(h->d_map, h->d_mapd, cells);
@@ -380,6 +392,40 @@ int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectrum_out, uin
   if (!h->spec) return arg_fail("b200dd_pipeline_fetch_spectrum: the spectrum stage is not enabled");
   if (cap < h->spec_bins) return arg_fail("b200dd_pipeline_fetch_spectrum: capacity too small");
   return b200dd_spectrum_fetch(h->spec, spectrum_out, h->stream);
+}
+
+int b200dd_pipeline_enable_map_json(b200dd_pipeline *h, size_t *max_bytes) {
+  if (!h) return arg_fail("b200dd_pipeline_enable_map_json: null handle");
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  pipeline_drop_graphs(h);  // the chain changes
+  b200dd_mapjson_destroy(h->mj);
+  h->mj = nullptr;
+  h->mj_stream = nullptr;
+  const int rc = b200dd_mapjson_create(h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(),
+                                       h->p.caf.fs, h->device, &h->mj);
+  if (rc != B200DD_OK) return rc;
+  if (max_bytes) *max_bytes = b200dd_mapjson_max_bytes(h->mj);
+  return B200DD_OK;
+}
+
+int b200dd_pipeline_fetch_map_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_map_json: null argument");
+  if (!h->mj) return arg_fail("b200dd_pipeline_fetch_map_json: the map JSON stage is not enabled");
+  if (!h->mj_stream) return arg_fail("b200dd_pipeline_fetch_map_json: no CPI submitted since the stage was enabled");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = (cudaStream_t)h->mj_stream;
+  if (h->last_had_filter) {
+    int fs = 0;
+    B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaStreamSynchronize(st));
+    if (fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273): no map is sent
+      set_last_error("b200dd_pipeline_fetch_map_json: the CPI's clutter-filter solve failed; it has no map");
+      return B200DD_FILTER_FAILED;
+    }
+  }
+  return b200dd_mapjson_fetch(h->mj, timestamp, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out,

@@ -34,6 +34,15 @@ class Map:
     def get_nCols(self):
         return self.data.shape[1]
 
+    def to_json_km(self, timestamp, fs, device=-1) -> bytes:
+        """delay_bin_to_km(to_json(timestamp), fs) (src/data/Map.cpp:116-185): the document blah2 sends on its map
+        socket, rendered on the device from this map, its axes and its noisePower / maxPower."""
+        mj = MapJson(self.delay, self.doppler, fs, device=device)
+        try:
+            return mj.render_host(self.data, self.noisePower, self.maxPower, timestamp)
+        finally:
+            mj.close()
+
 
 @dataclass
 class Detection:
@@ -478,13 +487,74 @@ def set_metrics(m: Map) -> Map:
     return m
 
 
+class MapJson:
+    """The map document of blah2.cpp:303-304 for maps of one shape: ``render_host`` for a complex128 host map,
+    ``render_device`` + ``fetch`` for a device map (float2 / complex64, or complex128).  Raises B200ddError with
+    code ERR_NONFINITE for a map cell with |z| = 0, inf or NaN, which has no JSON text."""
+
+    def __init__(self, delay, doppler, fs, device=-1):
+        lib = capi.load()
+        self.delay = np.ascontiguousarray(np.asarray(delay, dtype=np.int32))
+        self.doppler = np.ascontiguousarray(np.asarray(doppler, dtype=np.float64))
+        h = C.c_void_p()
+        capi.check(lib.b200dd_mapjson_create(self.doppler.size, self.delay.size, capi.ptr(self.delay),
+                                             capi.ptr(self.doppler), int(fs), int(device), C.byref(h)))
+        self._lib, self._h = lib, h
+        self.max_bytes = int(lib.b200dd_mapjson_max_bytes(h))
+        self._out = np.empty(self.max_bytes, dtype=np.uint8)
+
+    def render_host(self, data, noisePower, maxPower, timestamp) -> bytes:
+        data = _c128(data)
+        if data.shape != (self.doppler.size, self.delay.size):
+            raise ValueError(f"map shape {data.shape} != {(self.doppler.size, self.delay.size)}")
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_mapjson_render_host(self._h, capi.ptr(data), float(noisePower), float(maxPower),
+                                                        int(timestamp), capi.ptr(self._out), self._out.size,
+                                                        C.byref(n)))
+        return self._out[:n.value].tobytes()
+
+    def render_device(self, d_map, noisePower, maxPower, stream=None):
+        """Asynchronous: d_map is a torch tensor [nDop, nDel] of complex64 / complex128 (or a float view of it)."""
+        import torch
+        f64 = d_map.dtype in (torch.complex128, torch.float64)
+        capi.check(self._lib.b200dd_mapjson_render_device(self._h, capi.ptr(d_map), int(f64), float(noisePower),
+                                                          float(maxPower), capi.ptr(stream) if stream else None))
+
+    def fetch(self, timestamp, stream=None) -> bytes:
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_mapjson_fetch(self._h, int(timestamp), capi.ptr(self._out), self._out.size,
+                                                  C.byref(n), capi.ptr(stream) if stream else None))
+        return self._out[:n.value].tobytes()
+
+    def cell_values(self, d_map, noisePower):
+        """The double of every cell as the render computes it (10 log10|z| - noisePower), float64 [nDop, nDel]."""
+        import torch
+        f64 = d_map.dtype in (torch.complex128, torch.float64)
+        out = torch.empty((self.doppler.size, self.delay.size), dtype=torch.float64, device=d_map.device)
+        capi.check(self._lib.b200dd_mapjson_debug_cell_values(self._h, capi.ptr(d_map), int(f64), float(noisePower),
+                                                              capi.ptr(out), None))
+        torch.cuda.synchronize(d_map.device)
+        return out.cpu().numpy()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.b200dd_mapjson_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Pipeline:
     """One CPI through the body of the reference's process thread (src/blah2.cpp:268-287):
     [WienerHopf] -> Ambiguity -> Map::set_metrics -> [CfarDetector1D -> Centroid -> Interpolate],
     intermediates resident on the device.  Parameters are named like config/config.yml."""
 
     def __init__(self, delayMin, delayMax, dopplerMin, dopplerMax, fs, nSamples, roundHamming=True, clutter=None,
-                 detection=None, device=-1, max_detections=4096, spectrum_bandwidth=None):
+                 detection=None, device=-1, max_detections=4096, spectrum_bandwidth=None, map_json=False):
         lib = capi.load()
         p = capi.PipelineParams()
         p.caf = capi.CafParams(int(delayMin), int(delayMax), int(dopplerMin), int(dopplerMax), int(fs),
@@ -515,6 +585,20 @@ class Pipeline:
             ns = C.c_uint32()
             capi.check(lib.b200dd_pipeline_enable_spectrum(h, float(spectrum_bandwidth), C.byref(ns)))
             self.n_spectrum = int(ns.value)
+        self.map_json_max_bytes = 0
+        if map_json:  # map->to_json + delay_bin_to_km for every CPI, blah2.cpp:303-304
+            mb = C.c_size_t()
+            capi.check(lib.b200dd_pipeline_enable_map_json(h, C.byref(mb)))
+            self.map_json_max_bytes = int(mb.value)
+        self._json = np.empty(max(self.map_json_max_bytes, 1), dtype=np.uint8)
+
+    def fetch_map_json(self, timestamp) -> bytes:
+        """The map document of the last fetched CPI (call after fetch()).  Raises B200ddError with code
+        FILTER_FAILED when that CPI's clutter-filter solve failed: the reference sends no map then."""
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_fetch_map_json(self._h, int(timestamp), capi.ptr(self._json),
+                                                            self._json.size, C.byref(n)))
+        return self._json[:n.value].tobytes()
 
     def fetch_spectrum(self):
         """Spectrum of the reference channel of the last submitted CPI (complex128, nSpectrum bins)."""

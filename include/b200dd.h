@@ -19,6 +19,7 @@
  *   b200dd_spectrum_*   SpectrumAnalyser::SpectrumAnalyser / SpectrumAnalyser::process
  *                    src/process/spectrum/SpectrumAnalyser.h:48-57, SpectrumAnalyser.cpp:9-74
  *   b200dd_next_hamming   next_hamming, src/process/meta/HammingNumber.h:36
+ *   b200dd_mapjson_*    Map::to_json + Map::delay_bin_to_km, src/data/Map.cpp:116-185 (blah2.cpp:303-304)
  *
  * Data conventions
  *   host IQ      interleaved complex128 (re, im doubles) -- what IqData holds
@@ -64,7 +65,8 @@ extern "C" {
 #define B200DD_ERR_ARG 1         /* null pointer / size mismatch */
 #define B200DD_ERR_GEOMETRY 2    /* geometry outside the supported range (see DESIGN.md "limits") */
 #define B200DD_ERR_CUDA 3        /* CUDA runtime error; b200dd_last_error() has the text */
-#define B200DD_ERR_CAPACITY 4    /* output capacity too small (detections) */
+#define B200DD_ERR_CAPACITY 4    /* output capacity too small (detections, map JSON) */
+#define B200DD_ERR_NONFINITE 5   /* map JSON: a value rapidjson cannot write (a map cell with |z| = 0, inf or NaN) */
 #define B200DD_FILTER_FAILED 10  /* WienerHopf: matrix not positive definite -> y left untouched
                                     (reference returns false, WienerHopf.cpp:111-122) */
 
@@ -352,6 +354,51 @@ B200DD_API int b200dd_spectrum_profile_device(b200dd_spectrum *h, const void *d_
                                               float *ms_fold, float *ms_rest);
 B200DD_API void *b200dd_spectrum_stream(b200dd_spectrum *h);
 
+/* ------------------------------------------------------------------ map JSON
+ *
+ * The document blah2 sends on its map socket for every CPI: the std::string returned by
+ * map->delay_bin_to_km(map->to_json(timestamp), fs) (src/blah2.cpp:303-304, src/data/Map.cpp:116-185), byte for
+ * byte.  Members without whitespace in the order timestamp, nRows, nCols, noisePower, maxPower, delay (km),
+ * doppler (Hz), data; data[k][j] = 10 log10|map[k][j]| - noisePower.  Doubles are rapidjson's Writer text at two
+ * decimal places (shortest Grisu2 digits, TRUNCATED to two fraction digits); noisePower, maxPower, doppler and
+ * the cells are that text read back by rapidjson's default Reader and written again, as delay_bin_to_km does.
+ * The data body is rendered on the device (blah2_b200/csrc/mapjson.cu); the header is composed on the host.
+ *
+ * A map cell with |z| = 0, inf or NaN has no JSON number: rapidjson's Writer stops mid-document and blah2 then
+ * fails parsing the truncated text.  Here the render reports B200DD_ERR_NONFINITE and writes no bytes.
+ */
+typedef struct b200dd_mapjson b200dd_mapjson;
+
+/* Axes as Map holds them: delay[n_del] bins, doppler[n_dop] Hz; fs in Hz (delay km = delay c / fs / 1000). */
+B200DD_API int b200dd_mapjson_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, const double *doppler,
+                                     uint32_t fs, int32_t device, b200dd_mapjson **out);
+/* Exact upper bound of a document's size in bytes for this handle, for any map and metrics (every double's text
+ * is at most 24 bytes). */
+B200DD_API size_t b200dd_mapjson_max_bytes(const b200dd_mapjson *h);
+B200DD_API void b200dd_mapjson_destroy(b200dd_mapjson *h);
+/* Renders the data body of d_map ([n_dop][n_del] float2, or double2 when is_f64) with the given metrics,
+ * asynchronously on `stream` (NULL = the handle's stream).  d_map may be reused once the stream has passed it. */
+B200DD_API int b200dd_mapjson_render_device(b200dd_mapjson *h, const void *d_map, int is_f64, double noise_power,
+                                            double max_power, void *stream);
+/* Composes the header with `timestamp` and copies the body straight behind it into out (pinned memory for a fast
+ * copy); *n_bytes = document length (no terminating NUL).  Synchronises `stream` (the render's stream).
+ * B200DD_ERR_NONFINITE: a value has no JSON text, nothing written.  B200DD_ERR_CAPACITY: cap < *n_bytes. */
+B200DD_API int b200dd_mapjson_fetch(b200dd_mapjson *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
+                                    void *stream);
+/* Both steps for a HOST complex128 map (what Map<complex<double>>::data holds).  Synchronous. */
+B200DD_API int b200dd_mapjson_render_host(b200dd_mapjson *h, const double *map, double noise_power, double max_power,
+                                          uint64_t timestamp, char *out, size_t cap, size_t *n_bytes);
+/* Test entry points: the text a client receives for each of n doubles (written, read back, written again),
+ * comma-separated, an empty field for a value that has none (not finite, or its text reads back above DBL_MAX).
+ * _host runs the formatter on the CPU (no device needed), _device runs it in a kernel. */
+B200DD_API int b200dd_mapjson_format_doubles_host(const double *v, uint32_t n, char *out, size_t cap, size_t *n_bytes);
+B200DD_API int b200dd_mapjson_format_doubles_device(const double *v, uint32_t n, char *out, size_t cap,
+                                                    size_t *n_bytes, int32_t device);
+/* Test entry point: the double of every cell, 10 log10|z| - noise_power as the render computes it, into
+ * d_out[n_dop * n_del] (device memory).  Asynchronous on `stream`. */
+B200DD_API int b200dd_mapjson_debug_cell_values(b200dd_mapjson *h, const void *d_map, int is_f64, double noise_power,
+                                                void *d_out, void *stream);
+
 /* ------------------------------------------------------------------ whole CPI pipeline
  *
  * One coherent-processing interval through the body of the reference's process thread
@@ -428,6 +475,16 @@ B200DD_API void *b200dd_pipeline_stream(b200dd_pipeline *h);
  * synchronises the pipeline's stream itself). */
 B200DD_API int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32_t *n_spectrum);
 B200DD_API int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectrum_out, uint32_t cap);
+
+/* Optional last stage (src/blah2.cpp:303-304): renders the map document (see b200dd_mapjson_*) of every CPI
+ * submitted afterwards, right after set_metrics, with the noisePower set_metrics left on the device (no host round
+ * trip); works in recorded graphs.  Drops the graphs recorded so far.  *max_bytes (nullable) = the document size
+ * bound.  b200dd_pipeline_fetch_map_json, called after b200dd_pipeline_fetch, writes the last CPI's document;
+ * it returns B200DD_FILTER_FAILED and writes nothing when that CPI's clutter-filter solve failed (the reference
+ * skips the CPI and sends no map, blah2.cpp:270-273). */
+B200DD_API int b200dd_pipeline_enable_map_json(b200dd_pipeline *h, size_t *max_bytes);
+B200DD_API int b200dd_pipeline_fetch_map_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
+                                              size_t *n_bytes);
 
 /* ------------------------------------------------------------------------------------------------
  * Inter-GPU exchanges (one process per GPU, NCCL over NVLink / NVSwitch).  The reference has no
