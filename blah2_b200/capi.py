@@ -155,6 +155,8 @@ SIGNATURES = [
     ("b200dd_pipeline_fetch_spectrum", C.c_int, [_VP, _VP, C.c_uint32]),
     ("b200dd_pipeline_enable_map_json", C.c_int, [_VP, C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_map_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_enable_maxhold", C.c_int, [_VP, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_maxhold", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),
     ("b200dd_mapjson_destroy", None, [_VP]),
@@ -166,6 +168,14 @@ SIGNATURES = [
     ("b200dd_mapjson_format_doubles_device", C.c_int, [_VP, C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t),
                                                        C.c_int32]),
     ("b200dd_mapjson_debug_cell_values", C.c_int, [_VP, _VP, C.c_int, C.c_double, _VP, _VP]),
+    ("b200dd_maxhold_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
+    ("b200dd_maxhold_max_bytes", C.c_size_t, [_VP]),
+    ("b200dd_maxhold_destroy", None, [_VP]),
+    ("b200dd_maxhold_push_device", C.c_int, [_VP, _VP, C.c_int, C.c_double, C.c_double, _VP]),
+    ("b200dd_maxhold_fetch", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
+    ("b200dd_maxhold_format_doubles_host", C.c_int, [_VP, C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_maxhold_format_doubles_device", C.c_int, [_VP, C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t),
+                                                       C.c_int32]),
     ("b200dd_comm_get_unique_id", C.c_int, [_VP]),
     ("b200dd_comm_create", C.c_int, [C.c_int32, C.c_int32, _VP, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_comm_destroy", None, [_VP]),
@@ -262,6 +272,21 @@ def format_doubles(values, device=None) -> list:
         check(lib.b200dd_mapjson_format_doubles_host(ptr(v), v.size, ptr(out), out.size, C.byref(n)))
     else:
         check(lib.b200dd_mapjson_format_doubles_device(ptr(v), v.size, ptr(out), out.size, C.byref(n), int(device)))
+    return out[:n.value].tobytes().decode("ascii").split(",") if v.size else []
+
+
+def format_maxhold_doubles(values, device=None) -> list:
+    """The /stash/map text of a max-hold cell whose only held value is each double (its map-document text parsed
+    and re-printed by Number::toString), on the host (device=None) or in a kernel on `device`; "" where a value has
+    no map-document text or its hundredths lie outside int32."""
+    lib = load()
+    v = np.ascontiguousarray(np.asarray(values, dtype=np.float64).ravel())
+    n = C.c_size_t()
+    out = np.empty(v.size * 13 + 1, dtype=np.uint8)
+    if device is None:
+        check(lib.b200dd_maxhold_format_doubles_host(ptr(v), v.size, ptr(out), out.size, C.byref(n)))
+    else:
+        check(lib.b200dd_maxhold_format_doubles_device(ptr(v), v.size, ptr(out), out.size, C.byref(n), int(device)))
     return out[:n.value].tobytes().decode("ascii").split(",") if v.size else []
 
 

@@ -66,5 +66,9 @@ const double *det_device_metrics(b200dd_det *h);
 // mapjson.cu: enqueue the body render of a float2 map whose noisePower is read from d_metrics[0] at run time and
 // whose header values are read back from d_metrics[0..1] by b200dd_mapjson_fetch.
 int mapjson_enqueue_with_metrics(b200dd_mapjson *h, const void *d_map, const double *d_metrics, cudaStream_t st);
+// maxhold.cu: enqueue the push of a float2 map whose noisePower / maxPower are read from d_metrics[0..1] at run
+// time; the CPI is rejected with B200DD_FILTER_FAILED when *d_filter_status (nullable) is non-zero.
+int maxhold_enqueue_with_metrics(b200dd_maxhold *h, const void *d_map, const double *d_metrics,
+                                 const int *d_filter_status, cudaStream_t st);
 
 }  // namespace b2

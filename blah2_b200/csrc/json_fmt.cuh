@@ -497,4 +497,67 @@ JF_HD double cell_db(double re, double im, double noise) {
 #endif
 }
 
+// ---- the max-hold view of a cell (blah2's api/stash/maxhold.js), which parses the map document
+//
+// A cell's text from fmt_double_twice is always k/100 for an integer k: at most two fraction digits, or "0.0" /
+// "-0.0" below 0.01, or an exponent form at 10^21 and more.  k is the cell's SENT HUNDREDTHS.  JSON.parse rounds
+// correctly and is therefore monotonic, so the maximum of parsed cells is the parse of max k / 100, and the max can
+// be taken on the integers.
+
+// longest text fmt_hundredths() can produce: "-21474836.48"
+constexpr int kMaxHundredthsText = 12;
+
+// The sent hundredths of v: parses the text fmt_double_twice gives (no floating-point step of its own).  False when
+// v has no text (not finite, or not readable back) or k lies outside int32 (an exponent form included).
+JF_HD bool hundredths(double v, int32_t *k) {
+  char t[kMaxText];
+  const int n = fmt_double_twice(v, t);
+  if (n < 0) return false;
+  int p = t[0] == '-' ? 1 : 0;
+  const bool minus = p == 1;
+  int64_t a = 0;
+  for (; p < n && t[p] != '.'; p++) {
+    if (t[p] < '0' || t[p] > '9' || a > 21474836) return false;  // 'e', or already beyond int32 / 100
+    a = a * 10 + (t[p] - '0');
+  }
+  int frac = 0;
+  for (int d = 0; d < 2; d++) {  // "x.5" -> 50, "x.05" -> 5, "x.0" -> 0
+    frac *= 10;
+    if (p + 1 + d < n) {
+      const char c = t[p + 1 + d];
+      if (c < '0' || c > '9') return false;
+      frac += c - '0';
+    }
+  }
+  if (p + 3 < n) return false;  // more than two fraction digits (or an exponent after them): not produced
+  a = a * 100 + frac;
+  if (a > 2147483647) return false;
+  *k = (int32_t)(minus ? -a : a);
+  return true;
+}
+
+// ECMAScript Number::toString of the double nearest k/100: the canonical decimal of k/100 (sign, integer part,
+// 0-2 fraction digits with trailing zeros dropped; "0" for k = 0).  A decimal of at most 15 significant digits is
+// the shortest round-trip text of its own nearest double, and |k| < 2^31 has at most 10 digits.  Returns the length.
+JF_HD int fmt_hundredths(int32_t k, char *out) {
+  int n = 0;
+  uint32_t a = k < 0 ? 0u - (uint32_t)k : (uint32_t)k;
+  if (k < 0) out[n++] = '-';
+  const uint32_t ip = a / 100u, fp = a % 100u;
+  char d[10];
+  int nd = 0;
+  uint32_t q = ip;
+  do {
+    d[nd++] = (char)('0' + q % 10u);
+    q /= 10u;
+  } while (q);
+  while (nd) out[n++] = d[--nd];
+  if (fp) {
+    out[n++] = '.';
+    out[n++] = (char)('0' + fp / 10u);
+    if (fp % 10u) out[n++] = (char)('0' + fp % 10u);
+  }
+  return n;
+}
+
 }  // namespace jf

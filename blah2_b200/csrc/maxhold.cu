@@ -1,0 +1,488 @@
+// maxhold.cu -- the max-hold map document blah2's API serves at /stash/map, kept and rendered on the device.
+//
+// blah2's Node API (api/stash/maxhold.js) parses every new map document with JSON.parse, keeps the `data` arrays of
+// the last nCpi = 20 documents (:3, :54-59), and replaces the latest document's `data` with the per-cell Math.max
+// over them (:18-35); /stash/map sends JSON.stringify of that object (api/server.js:96-97, res.send(object)).  So a
+// client receives the latest document's header and, per cell, the maximum over the last 20 CPIs, every number
+// re-printed by ECMAScript's Number::toString.
+//
+// Each cell of a map document is k/100 for an integer k (json_fmt.cuh: jf::hundredths), so the window is a ring of
+// int32 hundredths.  Per CPI, mh_push_kernel writes the CPI's hundredths into ring slot `head` and mh_commit_kernel
+// (one thread) accepts or rejects the CPI.  The ring has kDepth + 1 slots: the slot a push writes is never one of
+// the held ones, so a rejected CPI leaves the window intact without a copy.  head, count and the held header live
+// on the device, so a push works inside a recorded graph.  At fetch time mh_len_kernel takes the max over the held
+// slots and counts each tile's bytes, scan_kernel places the tiles, and mh_write_kernel writes the text with the
+// staged, aligned stores of mapjson.cu.  The header is composed on the host.
+#include "common.cuh"
+#include "json_fmt.cuh"
+#include "scan.cuh"
+
+#include <math.h>
+#include <stdio.h>
+#include <stdlib.h>
+
+#include <cstring>
+#include <new>
+#include <string>
+#include <vector>
+
+using namespace b2;
+
+namespace {
+
+constexpr uint32_t kDepth = 20;         // nCpi, api/stash/maxhold.js:3
+constexpr uint32_t kSlots = kDepth + 1;  // + the slot being written
+constexpr int kThreads = 256;
+constexpr int kRounds = 4;
+constexpr int kTile = kThreads * kRounds;
+constexpr int kCellMax = jf::kMaxHundredthsText + 3;  // ",[" before the value, "]" after it
+constexpr uint32_t kC = 299792458u;                   // Constants::c, as in mapjson.cu
+constexpr double kNoiseBound = 1e7;  // |noisePower| <= 1e7 dB keeps every finite double cell inside int32 hundredths
+
+// ring state, one device copy per handle
+struct MhState {
+  uint32_t head;   // slot the next push writes
+  uint32_t count;  // slots held, <= kDepth
+  uint32_t bad;    // set by a push: a cell has no value
+  int32_t status;  // the last push's verdict: B200DD_OK, B200DD_FILTER_FAILED or B200DD_ERR_NONFINITE
+  double noise, maxp;  // header metrics of the latest accepted CPI
+};
+
+template <class TMAP> __device__ __forceinline__ double2 ld_cell(const TMAP *m, size_t i) {
+  const TMAP v = m[i];
+  return make_double2((double)v.x, (double)v.y);
+}
+
+template <class TMAP>
+__global__ void mh_push_kernel(const TMAP *__restrict__ map, size_t cells, double noise, const double *noise_dev,
+                               int32_t *__restrict__ ring, MhState *s) {
+  const double nz = noise_dev ? *noise_dev : noise;
+  int32_t *slot = ring + (size_t)s->head * cells;
+  bool bad = false;
+  for (size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x; c < cells; c += (size_t)gridDim.x * blockDim.x) {
+    const double2 z = ld_cell(map, c);
+    int32_t k;
+    if (jf::hundredths(jf::cell_db(z.x, z.y, nz), &k)) slot[c] = k;
+    else bad = true;
+  }
+  if (bad) s->bad = 1u;  // every writer stores the same value
+}
+
+__global__ void mh_commit_kernel(MhState *s, double noise, double maxp, const double *metrics_dev,
+                                 const int *filter_status) {
+  if (metrics_dev) {
+    noise = metrics_dev[0];
+    maxp = metrics_dev[1];
+  }
+  char t[jf::kMaxText];
+  int32_t st = B200DD_OK;
+  if (filter_status && *filter_status != 0) st = B200DD_FILTER_FAILED;  // blah2.cpp:270-273: no document is sent
+  else if (s->bad || jf::fmt_double_twice(noise, t) < 0 || jf::fmt_double_twice(maxp, t) < 0)
+    st = B200DD_ERR_NONFINITE;  // rapidjson stops mid-document; the stash's JSON.parse throws and skips it
+  if (st == B200DD_OK) {
+    s->head = (s->head + 1u) % kSlots;
+    if (s->count < kDepth) s->count++;
+    s->noise = noise;
+    s->maxp = maxp;
+  }
+  s->status = st;
+  s->bad = 0u;
+}
+
+struct RenderArgs {
+  const int32_t *ring;
+  const MhState *s;
+  size_t cells;
+  uint32_t nDel;
+  int32_t *held;             // [cells] the window's max, written by mh_len_kernel
+  uint32_t *tile_len;        // [nTiles]
+  const uint32_t *tile_off;  // [nTiles + 1]
+  char *body;
+};
+
+// cell c's bytes: its separator (",", "[" or ",[" at a row start), its value, "]" at a row end
+__device__ __forceinline__ int cell_text(const RenderArgs &a, size_t c, int32_t k, char *t) {
+  const uint32_t j = (uint32_t)(c % a.nDel);
+  int n = 0;
+  if (j == 0) {
+    if (c) t[n++] = ',';
+    t[n++] = '[';
+  } else {
+    t[n++] = ',';
+  }
+  n += jf::fmt_hundredths(k, t + n);
+  if (j == a.nDel - 1) t[n++] = ']';
+  return n;
+}
+
+__global__ void __launch_bounds__(kThreads) mh_len_kernel(RenderArgs a) {
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const uint32_t head = a.s->head, count = a.s->count;
+  const size_t base = (size_t)blockIdx.x * kTile;
+  char t[kCellMax];
+  uint32_t sum = 0;
+  for (int r = 0; r < kRounds; r++) {
+    const size_t c = base + (size_t)r * kThreads + threadIdx.x;
+    if (c >= a.cells) continue;
+    uint32_t slot = head;
+    int32_t m = INT32_MIN;
+    for (uint32_t i = 0; i < count; i++) {  // the held slots, newest first
+      slot = slot ? slot - 1u : kSlots - 1u;
+      m = max(m, a.ring[(size_t)slot * a.cells + c]);
+    }
+    a.held[c] = m;
+    sum += (uint32_t)cell_text(a, c, m, t);
+  }
+  uint32_t tot;
+  block_excl_scan<kThreads>(sum, wsum, tot);
+  if (threadIdx.x == 0) a.tile_len[blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(kThreads) mh_write_kernel(RenderArgs a) {
+  __shared__ __align__(16) char stage[kTile * kCellMax + 16];
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const size_t base = (size_t)blockIdx.x * kTile;
+  const uint32_t off = a.tile_off[blockIdx.x];
+  const uint32_t phase = off & 15u;  // stage[phase + i] <-> body[off + i]: same address mod 16
+  char t[kCellMax];
+  uint32_t pos = phase;
+  for (int r = 0; r < kRounds; r++) {
+    const size_t c = base + (size_t)r * kThreads + threadIdx.x;
+    const int n = c < a.cells ? cell_text(a, c, a.held[c], t) : 0;
+    uint32_t tot;
+    const uint32_t ex = block_excl_scan<kThreads>((uint32_t)n, wsum, tot);
+    for (int i = 0; i < n; i++) stage[pos + ex + i] = t[i];
+    pos += tot;
+  }
+  __syncthreads();
+  const uint32_t g0 = off, g1 = off + (pos - phase);
+  uint32_t a0 = (g0 + 15u) & ~15u, a1 = g1 & ~15u;
+  if (a0 > g1) a0 = g1;
+  if (a1 < a0) a1 = a0;
+  char *body = a.body;
+  for (uint32_t g = g0 + threadIdx.x; g < a0; g += kThreads) body[g] = stage[g - off + phase];
+  for (uint32_t g = a1 + threadIdx.x; g < g1; g += kThreads) body[g] = stage[g - off + phase];
+  for (uint32_t g = a0 + 16u * threadIdx.x; g < a1; g += 16u * kThreads)
+    *reinterpret_cast<uint4 *>(body + g) = *reinterpret_cast<const uint4 *>(stage + (g - off + phase));
+}
+
+// the /stash/map text of a cell whose only held value is v[i] (len -1: none)
+__global__ void mh_format_kernel(const double *v, uint32_t n, char *text, int *len) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    int32_t k;
+    len[i] = jf::hundredths(v[i], &k) ? jf::fmt_hundredths(k, text + (size_t)i * jf::kMaxHundredthsText) : -1;
+  }
+}
+
+// ECMAScript Number::toString (ECMA-262 6.1.6.1.20, radix 10) of a finite double: the fewest significant digits
+// that read back to d (the first precision whose correctly rounded %e text does), then the standard's layout.
+std::string js_number_text(double d) {
+  if (d == 0.0) return "0";  // -0 too
+  std::string out;
+  if (d < 0) {
+    out = "-";
+    d = -d;
+  }
+  char buf[40];
+  for (int p = 1; p <= 17; p++) {
+    snprintf(buf, sizeof(buf), "%.*e", p - 1, d);
+    if (strtod(buf, nullptr) == d) break;
+  }
+  // buf = "D[.DDD]e[+-]XX": digits s (k of them), value = s * 10^(n - k)
+  std::string s;
+  const char *p = buf;
+  for (; *p != 'e'; p++)
+    if (*p != '.') s += *p;
+  const int n = atoi(p + 1) + 1;
+  while (s.size() > 1 && s.back() == '0') s.pop_back();
+  const int k = (int)s.size();
+  if (k <= n && n <= 21) {
+    out += s;
+    out.append((size_t)(n - k), '0');
+  } else if (0 < n && n <= 21) {
+    out += s.substr(0, (size_t)n) + "." + s.substr((size_t)n);
+  } else if (-6 < n && n <= 0) {
+    out += "0." + std::string((size_t)-n, '0') + s;
+  } else {
+    out += s.substr(0, 1);
+    if (k > 1) out += "." + s.substr(1);
+    out += (n - 1 < 0 ? "e-" : "e+") + std::to_string(n - 1 < 0 ? 1 - n : n - 1);
+  }
+  return out;
+}
+
+// JSON.stringify of the array JSON.parse reads from "[a,b,..]" of the values' texts (once or twice formatted, as
+// mapjson.cu writes the axes); false when a value has no text
+bool js_array_text(const double *v, size_t n, bool twice, std::string &out) {
+  out = "[";
+  char t[jf::kMaxText + 1];
+  for (size_t i = 0; i < n; i++) {
+    const int k = twice ? jf::fmt_double_twice(v[i], t) : (jf::is_finite(v[i]) ? jf::fmt_double(v[i], t) : -1);
+    if (k < 0) return false;
+    t[k] = '\0';
+    if (i) out += ',';
+    out += js_number_text(strtod(t, nullptr));  // JSON.parse: correctly rounded
+  }
+  out += ']';
+  return true;
+}
+
+// JSON.stringify of what JSON.parse reads from a text fmt_double_twice writes for v
+bool js_metric_text(double v, std::string &out) {
+  char t[jf::kMaxText + 1];
+  const int k = jf::fmt_double_twice(v, t);
+  if (k < 0) return false;
+  t[k] = '\0';
+  out = js_number_text(strtod(t, nullptr));
+  return true;
+}
+
+int join_texts(const char *text, const int *len, uint32_t n, char *out, size_t cap, size_t *n_bytes) {
+  size_t need = n ? n - 1 : 0;
+  for (uint32_t i = 0; i < n; i++) need += len[i] > 0 ? (size_t)len[i] : 0;
+  if (n_bytes) *n_bytes = need;
+  if (need > cap) {
+    set_last_error("b200dd_maxhold_format_doubles: output capacity too small");
+    return B200DD_ERR_CAPACITY;
+  }
+  char *p = out;
+  for (uint32_t i = 0; i < n; i++) {
+    if (i) *p++ = ',';
+    if (len[i] > 0) {
+      memcpy(p, text + (size_t)i * jf::kMaxHundredthsText, (size_t)len[i]);
+      p += len[i];
+    }
+  }
+  return B200DD_OK;
+}
+
+}  // namespace
+
+struct b200dd_maxhold {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  uint32_t nDop = 0, nDel = 0, nTiles = 0;
+  size_t cells = 0;
+  std::string delay_txt, doppler_txt;  // the two axis arrays as JSON.stringify prints them
+  bool axes_ok = true;                 // false: an axis value has no text, every document fails
+  size_t body_max = 0, max_bytes = 0;
+  int32_t *d_ring = nullptr;  // [kSlots][cells] hundredths
+  int32_t *d_held = nullptr;  // [cells]
+  MhState *d_state = nullptr;
+  char *d_body = nullptr;
+  uint32_t *d_tile_len = nullptr, *d_tile_off = nullptr;
+  uint32_t *d_total = nullptr;
+};
+
+namespace {
+
+std::string compose_header(const b200dd_maxhold *h, const std::string &ts, const std::string &noise,
+                           const std::string &maxp) {
+  std::string s;
+  s.reserve(160 + h->delay_txt.size() + h->doppler_txt.size());
+  s += "{\"timestamp\":" + ts + ",\"nRows\":" + std::to_string(h->nDop) + ",\"nCols\":" + std::to_string(h->nDel);
+  s += ",\"noisePower\":" + noise + ",\"maxPower\":" + maxp;
+  s += ",\"delay\":" + h->delay_txt + ",\"doppler\":" + h->doppler_txt + ",\"data\":[";
+  return s;
+}
+
+int enqueue_push(b200dd_maxhold *h, const void *d_map, bool f64, double noise, double maxp, const double *d_metrics,
+                 const int *d_filter_status, cudaStream_t st) {
+  const size_t want = (h->cells + 255) / 256;
+  const int blocks = (int)(want < 132 * 8 ? want : 132 * 8);
+  const double *noise_dev = d_metrics;  // d_metrics[0] = noisePower
+  if (f64)
+    mh_push_kernel<double2><<<blocks, 256, 0, st>>>((const double2 *)d_map, h->cells, noise, noise_dev, h->d_ring, h->d_state);
+  else
+    mh_push_kernel<float2><<<blocks, 256, 0, st>>>((const float2 *)d_map, h->cells, noise, noise_dev, h->d_ring, h->d_state);
+  B2_LAUNCH_CHECK();
+  mh_commit_kernel<<<1, 1, 0, st>>>(h->d_state, noise, maxp, d_metrics, d_filter_status);
+  B2_LAUNCH_CHECK();
+  return B200DD_OK;
+}
+
+}  // namespace
+
+int b2::maxhold_enqueue_with_metrics(b200dd_maxhold *h, const void *d_map, const double *d_metrics,
+                                     const int *d_filter_status, cudaStream_t st) {
+  return enqueue_push(h, d_map, false, 0.0, 0.0, d_metrics, d_filter_status, st);
+}
+
+extern "C" {
+
+int b200dd_maxhold_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, const double *doppler, uint32_t fs,
+                          int32_t device, b200dd_maxhold **out) {
+  if (!out || !delay || !doppler) return arg_fail("b200dd_maxhold_create: null argument");
+  *out = nullptr;
+  if (n_dop == 0 || n_del == 0) return arg_fail("b200dd_maxhold_create: empty map");
+  if (fs == 0) return arg_fail("b200dd_maxhold_create: fs must be positive");
+  b200dd_maxhold *h = new (std::nothrow) b200dd_maxhold();
+  if (!h) return arg_fail("b200dd_maxhold_create: out of host memory");
+  auto fail = [&](int rc) { b200dd_maxhold_destroy(h); return rc; };
+  h->nDop = n_dop;
+  h->nDel = n_del;
+  h->cells = (size_t)n_dop * n_del;
+  h->nTiles = (uint32_t)((h->cells + kTile - 1) / kTile);
+  // the axes as the map document carries them (mapjson.cu), then parsed and re-printed by the stash
+  std::vector<double> km(n_del);
+  for (uint32_t i = 0; i < n_del; i++) km[i] = 1.0 * delay[i] * (kC / (double)fs) / 1000;
+  h->axes_ok = js_array_text(km.data(), n_del, false, h->delay_txt) &&
+               js_array_text(doppler, n_dop, true, h->doppler_txt);
+  h->body_max = h->cells * jf::kMaxHundredthsText + (size_t)n_dop * (n_del + 1) + (n_dop - 1);
+  if (h->body_max > 0xFFFFFFF0ull) return fail(geom_fail("b200dd_maxhold_create: map too large for 32-bit text offsets"));
+  // the longest texts: a timestamp, and a metric (Number::toString of a double is at most 25 bytes)
+  const std::string widest(25, '0');
+  h->max_bytes = compose_header(h, "18446744073709552000", widest, widest).size() + h->body_max + 2;
+  int dev = device;
+  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
+  h->device = dev;
+  DeviceGuard guard(dev);
+  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
+  auto body = [&]() -> int {
+    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    B2_CUDA(cudaMalloc(&h->d_ring, sizeof(int32_t) * kSlots * h->cells));
+    B2_CUDA(cudaMalloc(&h->d_held, sizeof(int32_t) * h->cells));
+    B2_CUDA(cudaMalloc(&h->d_state, sizeof(MhState)));
+    B2_CUDA(cudaMemsetAsync(h->d_state, 0, sizeof(MhState), h->stream));
+    B2_CUDA(cudaMalloc(&h->d_body, (h->body_max + 15) & ~(size_t)15));
+    B2_CUDA(cudaMalloc(&h->d_tile_len, sizeof(uint32_t) * h->nTiles));
+    B2_CUDA(cudaMalloc(&h->d_tile_off, sizeof(uint32_t) * (h->nTiles + 1)));
+    B2_CUDA(cudaMalloc(&h->d_total, sizeof(uint32_t)));
+    B2_CUDA(cudaStreamSynchronize(h->stream));  // the state is cleared before a push on another stream
+    return B200DD_OK;
+  };
+  const int rc = body();
+  if (rc != B200DD_OK) return fail(rc);
+  *out = h;
+  return B200DD_OK;
+}
+
+size_t b200dd_maxhold_max_bytes(const b200dd_maxhold *h) { return h ? h->max_bytes : 0; }
+
+void b200dd_maxhold_destroy(b200dd_maxhold *h) {
+  if (!h) return;
+  {
+    DeviceGuard guard(h->device);
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    free_dev(h->d_ring);
+    free_dev(h->d_held);
+    free_dev(h->d_state);
+    free_dev(h->d_body);
+    free_dev(h->d_tile_len);
+    free_dev(h->d_tile_off);
+    free_dev(h->d_total);
+    if (h->stream) cudaStreamDestroy(h->stream);
+  }
+  delete h;
+}
+
+int b200dd_maxhold_push_device(b200dd_maxhold *h, const void *d_map, int is_f64, double noise_power, double max_power,
+                               void *stream) {
+  if (!h || !d_map) return arg_fail("b200dd_maxhold_push_device: null argument");
+  if (jf::is_finite(noise_power) && fabs(noise_power) > kNoiseBound)
+    return arg_fail("b200dd_maxhold_push_device: |noise_power| > 1e7 dB");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  return enqueue_push(h, d_map, is_f64 != 0, noise_power, max_power, nullptr, nullptr, st);
+}
+
+int b200dd_maxhold_fetch(b200dd_maxhold *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes, void *stream) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_maxhold_fetch: null argument");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  MhState s;
+  B2_CUDA(cudaMemcpyAsync(&s, h->d_state, sizeof(s), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  if (s.status == B200DD_FILTER_FAILED) {
+    set_last_error("b200dd_maxhold_fetch: the last CPI's clutter-filter solve failed; it has no map");
+    return B200DD_FILTER_FAILED;
+  }
+  if (s.status == B200DD_ERR_NONFINITE) {
+    set_last_error("b200dd_maxhold_fetch: the last CPI has a value without JSON text (a map cell is zero, infinite "
+                   "or NaN, or a metric is not finite)");
+    return B200DD_ERR_NONFINITE;
+  }
+  if (s.count == 0) return arg_fail("b200dd_maxhold_fetch: nothing held yet");
+  if (!h->axes_ok) {
+    set_last_error("b200dd_maxhold_fetch: an axis value has no JSON text");
+    return B200DD_ERR_NONFINITE;
+  }
+  std::string tn, tm;
+  js_metric_text(s.noise, tn);  // the commit accepted only metrics with a text
+  js_metric_text(s.maxp, tm);
+  const std::string hdr = compose_header(h, js_number_text((double)timestamp), tn, tm);
+  RenderArgs a;
+  a.ring = h->d_ring; a.s = h->d_state; a.cells = h->cells; a.nDel = h->nDel; a.held = h->d_held;
+  a.tile_len = h->d_tile_len; a.tile_off = h->d_tile_off; a.body = h->d_body;
+  mh_len_kernel<<<h->nTiles, kThreads, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)h->nTiles, h->d_total);
+  B2_LAUNCH_CHECK();
+  mh_write_kernel<<<h->nTiles, kThreads, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  uint32_t body = 0;
+  B2_CUDA(cudaMemcpyAsync(&body, h->d_total, sizeof(body), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  const size_t total = hdr.size() + body + 2;
+  if (total > cap) {
+    if (n_bytes) *n_bytes = total;
+    set_last_error("b200dd_maxhold_fetch: output capacity too small (see b200dd_maxhold_max_bytes)");
+    return B200DD_ERR_CAPACITY;
+  }
+  memcpy(out, hdr.data(), hdr.size());
+  B2_CUDA(cudaMemcpyAsync(out + hdr.size(), h->d_body, body, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  out[total - 2] = ']';
+  out[total - 1] = '}';
+  if (n_bytes) *n_bytes = total;
+  return B200DD_OK;
+}
+
+int b200dd_maxhold_format_doubles_host(const double *v, uint32_t n, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if ((n && !v) || (cap && !out)) return arg_fail("b200dd_maxhold_format_doubles_host: null argument");
+  std::vector<char> text((size_t)n * jf::kMaxHundredthsText);
+  std::vector<int> len(n);
+  for (uint32_t i = 0; i < n; i++) {
+    int32_t k;
+    len[i] = jf::hundredths(v[i], &k) ? jf::fmt_hundredths(k, text.data() + (size_t)i * jf::kMaxHundredthsText) : -1;
+  }
+  return join_texts(text.data(), len.data(), n, out, cap, n_bytes);
+}
+
+int b200dd_maxhold_format_doubles_device(const double *v, uint32_t n, char *out, size_t cap, size_t *n_bytes,
+                                         int32_t device) {
+  if (n_bytes) *n_bytes = 0;
+  if ((n && !v) || (cap && !out)) return arg_fail("b200dd_maxhold_format_doubles_device: null argument");
+  int dev = device;
+  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__);
+  DeviceGuard guard(dev);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+  if (n == 0) return join_texts(nullptr, nullptr, 0, out, cap, n_bytes);
+  std::vector<char> text((size_t)n * jf::kMaxHundredthsText);
+  std::vector<int> len(n);
+  double *d_v = nullptr;
+  char *d_text = nullptr;
+  int *d_len = nullptr;
+  auto body = [&]() -> int {
+    B2_CUDA(cudaMalloc(&d_v, sizeof(double) * n));
+    B2_CUDA(cudaMalloc(&d_text, text.size()));
+    B2_CUDA(cudaMalloc(&d_len, sizeof(int) * n));
+    B2_CUDA(cudaMemcpy(d_v, v, sizeof(double) * n, cudaMemcpyHostToDevice));
+    const uint32_t blocks = (n + 255) / 256 < 132 * 16 ? (n + 255) / 256 : 132 * 16;
+    mh_format_kernel<<<blocks, 256>>>(d_v, n, d_text, d_len);
+    B2_LAUNCH_CHECK();
+    B2_CUDA(cudaMemcpy(text.data(), d_text, text.size(), cudaMemcpyDeviceToHost));
+    B2_CUDA(cudaMemcpy(len.data(), d_len, sizeof(int) * n, cudaMemcpyDeviceToHost));
+    return B200DD_OK;
+  };
+  const int rc = body();
+  free_dev(d_v);
+  free_dev(d_text);
+  free_dev(d_len);
+  if (rc != B200DD_OK) return rc;
+  return join_texts(text.data(), len.data(), n, out, cap, n_bytes);
+}
+
+}  // extern "C"

@@ -1,6 +1,6 @@
 // pipeline.cu -- one CPI through WienerHopf -> Ambiguity -> set_metrics -> detection with all
 // intermediates resident in HBM (the body of the reference's process thread, src/blah2.cpp:268-287).
-// Composes the per-class handles of caf.cu / wh.cu / det.cu / mapjson.cu through their C ABI; the only kernels
+// Composes the per-class handles of caf.cu / wh.cu / det.cu / mapjson.cu / maxhold.cu through their C ABI; the only kernels
 // defined here are the complex128 <-> complex64 conversions of the host entry point.
 #include "common.cuh"
 
@@ -54,6 +54,8 @@ struct b200dd_pipeline {
   b200dd_spectrum *spec = nullptr;  // optional first stage (blah2.cpp:263-265)
   b200dd_mapjson *mj = nullptr;     // optional last stage: the map document (blah2.cpp:303-304)
   void *mj_stream = nullptr;        // stream of the last submit, where its document was rendered
+  b200dd_maxhold *mh = nullptr;     // optional: the API's max-hold window (api/stash/maxhold.js)
+  void *mh_stream = nullptr;        // stream of the last submit, where its push was enqueued
   uint32_t spec_bins = 0, spec_nfft = 0;
   b200dd_caf_geometry g;
   std::vector<int32_t> delay;
@@ -132,6 +134,7 @@ void b200dd_pipeline_destroy(b200dd_pipeline *h) {
     b200dd_det_destroy(h->det);
     b200dd_spectrum_destroy(h->spec);
     b200dd_mapjson_destroy(h->mj);
+    b200dd_maxhold_destroy(h->mh);
     free_dev(h->d_yf);
     free_dev(h->d_xd);
     free_dev(h->d_yd);
@@ -158,6 +161,21 @@ int b200dd_pipeline_get_axes(const b200dd_pipeline *h, int32_t *delay, double *d
 
 void *b200dd_pipeline_stream(b200dd_pipeline *h) { return h ? (void *)h->stream : nullptr; }
 
+// the optional stages after set_metrics, on the map `map` of the CPI just enqueued on `st`
+static int pipeline_enqueue_products(b200dd_pipeline *h, float2 *map, void *st) {
+  if (h->mj) {
+    h->mj_stream = st;
+    const int rc = mapjson_enqueue_with_metrics(h->mj, map, det_device_metrics(h->det), (cudaStream_t)st);
+    if (rc != B200DD_OK) return rc;
+  }
+  if (h->mh) {
+    h->mh_stream = st;
+    return maxhold_enqueue_with_metrics(h->mh, map, det_device_metrics(h->det),
+                                        h->wh ? b200dd_wh_device_status(h->wh) : nullptr, (cudaStream_t)st);
+  }
+  return B200DD_OK;
+}
+
 // the kernels of one CPI on device-resident IQ, enqueued on `st` (also what a graph capture records)
 static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map, void *st) {
   const void *y = d_y;
@@ -180,9 +198,8 @@ static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const vo
   const int last = h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0;
   rc = b200dd_det_chain_device_async(h->det, last, map, h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(),
                                      h->doppler.data(), st);
-  if (rc != B200DD_OK || !h->mj) return rc;
-  h->mj_stream = st;
-  return mapjson_enqueue_with_metrics(h->mj, map, det_device_metrics(h->det), (cudaStream_t)st);
+  if (rc != B200DD_OK) return rc;
+  return pipeline_enqueue_products(h, map, st);
 }
 
 
@@ -214,6 +231,7 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   if (!g) return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
   h->last_had_filter = h->wh != nullptr;
   h->mj_stream = st;
+  h->mh_stream = st;
   B2_CUDA(cudaGraphLaunch(g->exec, (cudaStream_t)st));
   return B200DD_OK;
 }
@@ -320,11 +338,8 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   rc = b200dd_det_chain_device_async(h->det, h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0, h->d_map,
                                      h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(), st);
   if (rc != B200DD_OK) return rc;
-  if (h->mj) {
-    h->mj_stream = st;
-    rc = mapjson_enqueue_with_metrics(h->mj, h->d_map, det_device_metrics(h->det), st);
-    if (rc != B200DD_OK) return rc;
-  }
+  rc = pipeline_enqueue_products(h, h->d_map, st);
+  if (rc != B200DD_OK) return rc;
   if (map_out) {
     const uint32_t cells = h->g.n_doppler_bins * h->g.n_delay_bins;
     pl_widen_kernel<<<grid_for(cells), 256, 0, st>>>(h->d_map, h->d_mapd, cells);
@@ -426,6 +441,30 @@ int b200dd_pipeline_fetch_map_json(b200dd_pipeline *h, uint64_t timestamp, char 
     }
   }
   return b200dd_mapjson_fetch(h->mj, timestamp, out, cap, n_bytes, st);
+}
+
+int b200dd_pipeline_enable_maxhold(b200dd_pipeline *h, size_t *max_bytes) {
+  if (!h) return arg_fail("b200dd_pipeline_enable_maxhold: null handle");
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  pipeline_drop_graphs(h);  // the chain changes
+  b200dd_maxhold_destroy(h->mh);
+  h->mh = nullptr;
+  h->mh_stream = nullptr;
+  const int rc = b200dd_maxhold_create(h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(),
+                                       h->p.caf.fs, h->device, &h->mh);
+  if (rc != B200DD_OK) return rc;
+  if (max_bytes) *max_bytes = b200dd_maxhold_max_bytes(h->mh);
+  return B200DD_OK;
+}
+
+int b200dd_pipeline_fetch_maxhold(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_maxhold: null argument");
+  if (!h->mh) return arg_fail("b200dd_pipeline_fetch_maxhold: the max-hold stage is not enabled");
+  if (!h->mh_stream) return arg_fail("b200dd_pipeline_fetch_maxhold: no CPI submitted since the stage was enabled");
+  DeviceGuard guard(h->device);
+  return b200dd_maxhold_fetch(h->mh, timestamp, out, cap, n_bytes, h->mh_stream);
 }
 
 int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out,

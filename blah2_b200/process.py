@@ -548,13 +548,57 @@ class MapJson:
             pass
 
 
+class MaxHold:
+    """The max-hold map document blah2's API serves at /stash/map (api/stash/maxhold.js): per cell the maximum
+    over the last 20 accepted CPIs, with the latest one's header.  ``push_device`` adds a CPI's device map
+    (complex64 or complex128) with its set_metrics values; ``fetch`` renders the document.  ``fetch`` raises
+    B200ddError with code ERR_NONFINITE when the last push was rejected (a cell or metric without JSON text) and
+    ERR_ARG when nothing is held yet."""
+
+    def __init__(self, delay, doppler, fs, device=-1):
+        lib = capi.load()
+        self.delay = np.ascontiguousarray(np.asarray(delay, dtype=np.int32))
+        self.doppler = np.ascontiguousarray(np.asarray(doppler, dtype=np.float64))
+        h = C.c_void_p()
+        capi.check(lib.b200dd_maxhold_create(self.doppler.size, self.delay.size, capi.ptr(self.delay),
+                                             capi.ptr(self.doppler), int(fs), int(device), C.byref(h)))
+        self._lib, self._h = lib, h
+        self.max_bytes = int(lib.b200dd_maxhold_max_bytes(h))
+        self._out = np.empty(self.max_bytes, dtype=np.uint8)
+
+    def push_device(self, d_map, noisePower, maxPower, stream=None):
+        """Asynchronous: d_map is a torch tensor [nDop, nDel] of complex64 / complex128 (or a float view of it)."""
+        import torch
+        f64 = d_map.dtype in (torch.complex128, torch.float64)
+        capi.check(self._lib.b200dd_maxhold_push_device(self._h, capi.ptr(d_map), int(f64), float(noisePower),
+                                                        float(maxPower), capi.ptr(stream) if stream else None))
+
+    def fetch(self, timestamp, stream=None) -> bytes:
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_maxhold_fetch(self._h, int(timestamp), capi.ptr(self._out), self._out.size,
+                                                  C.byref(n), capi.ptr(stream) if stream else None))
+        return self._out[:n.value].tobytes()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.b200dd_maxhold_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Pipeline:
     """One CPI through the body of the reference's process thread (src/blah2.cpp:268-287):
     [WienerHopf] -> Ambiguity -> Map::set_metrics -> [CfarDetector1D -> Centroid -> Interpolate],
     intermediates resident on the device.  Parameters are named like config/config.yml."""
 
     def __init__(self, delayMin, delayMax, dopplerMin, dopplerMax, fs, nSamples, roundHamming=True, clutter=None,
-                 detection=None, device=-1, max_detections=4096, spectrum_bandwidth=None, map_json=False):
+                 detection=None, device=-1, max_detections=4096, spectrum_bandwidth=None, map_json=False,
+                 maxhold=False):
         lib = capi.load()
         p = capi.PipelineParams()
         p.caf = capi.CafParams(int(delayMin), int(delayMax), int(dopplerMin), int(dopplerMax), int(fs),
@@ -591,6 +635,21 @@ class Pipeline:
             capi.check(lib.b200dd_pipeline_enable_map_json(h, C.byref(mb)))
             self.map_json_max_bytes = int(mb.value)
         self._json = np.empty(max(self.map_json_max_bytes, 1), dtype=np.uint8)
+        self.maxhold_max_bytes = 0
+        if maxhold:  # the API's /stash/map window over the last 20 CPIs, api/stash/maxhold.js
+            mb = C.c_size_t()
+            capi.check(lib.b200dd_pipeline_enable_maxhold(h, C.byref(mb)))
+            self.maxhold_max_bytes = int(mb.value)
+        self._maxhold = np.empty(max(self.maxhold_max_bytes, 1), dtype=np.uint8)
+
+    def fetch_maxhold(self, timestamp) -> bytes:
+        """The /stash/map document after the last fetched CPI (call after fetch()).  Raises B200ddError with code
+        FILTER_FAILED when that CPI's clutter-filter solve failed (the window is unchanged), ERR_ARG when the stage
+        is not enabled or nothing has been submitted."""
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_fetch_maxhold(self._h, int(timestamp), capi.ptr(self._maxhold),
+                                                           self._maxhold.size, C.byref(n)))
+        return self._maxhold[:n.value].tobytes()
 
     def fetch_map_json(self, timestamp) -> bytes:
         """The map document of the last fetched CPI (call after fetch()).  Raises B200ddError with code

@@ -20,6 +20,7 @@
  *                    src/process/spectrum/SpectrumAnalyser.h:48-57, SpectrumAnalyser.cpp:9-74
  *   b200dd_next_hamming   next_hamming, src/process/meta/HammingNumber.h:36
  *   b200dd_mapjson_*    Map::to_json + Map::delay_bin_to_km, src/data/Map.cpp:116-185 (blah2.cpp:303-304)
+ *   b200dd_maxhold_*    the API's max-hold stash, api/stash/maxhold.js (served at /stash/map, api/server.js:96-97)
  *
  * Data conventions
  *   host IQ      interleaved complex128 (re, im doubles) -- what IqData holds
@@ -399,6 +400,44 @@ B200DD_API int b200dd_mapjson_format_doubles_device(const double *v, uint32_t n,
 B200DD_API int b200dd_mapjson_debug_cell_values(b200dd_mapjson *h, const void *d_map, int is_f64, double noise_power,
                                                 void *d_out, void *stream);
 
+/* ------------------------------------------------------------------ max-hold map document
+ *
+ * The document blah2's API serves at /stash/map (api/stash/maxhold.js, api/server.js:96-97): the latest map
+ * document (b200dd_mapjson_*) parsed by JSON.parse, its `data` replaced by the per-cell maximum over the last 20
+ * documents, and sent as JSON.stringify of the result.  Every number is ECMAScript's Number::toString of the parsed
+ * value: shortest round-trip digits, "12" for 12.0, "0" for -0.0, integers above 2^53 rounded
+ * (18446744073709551615 -> "18446744073709552000").  A cell of a map document is always k/100 for an integer k,
+ * so the window is kept on the device as int32 hundredths, and the maximum is taken on those.
+ *
+ * Each push is accepted or rejected on the device.  A rejected push leaves the window and header unchanged; it is
+ * a CPI blah2 publishes no map document for: a cell with |z| = 0, inf or NaN, a noisePower or maxPower without
+ * text (B200DD_ERR_NONFINITE), or a failed clutter-filter solve in the pipeline (B200DD_FILTER_FAILED).
+ * Device memory: n_dop * n_del * 88 bytes (21 ring slots of int32, the window's maximum) plus the document. */
+typedef struct b200dd_maxhold b200dd_maxhold;
+
+/* Axes as Map holds them (see b200dd_mapjson_create). */
+B200DD_API int b200dd_maxhold_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, const double *doppler,
+                                     uint32_t fs, int32_t device, b200dd_maxhold **out);
+/* Upper bound of a document's size in bytes for this handle. */
+B200DD_API size_t b200dd_maxhold_max_bytes(const b200dd_maxhold *h);
+B200DD_API void b200dd_maxhold_destroy(b200dd_maxhold *h);
+/* Adds one CPI's map d_map ([n_dop][n_del] float2, or double2 when is_f64) with its set_metrics values,
+ * asynchronously on `stream` (NULL = the handle's stream).  A finite |noise_power| > 1e7 dB returns
+ * B200DD_ERR_ARG at once (the bound keeps every cell's hundredths inside int32); a non-finite one rejects the push. */
+B200DD_API int b200dd_maxhold_push_device(b200dd_maxhold *h, const void *d_map, int is_f64, double noise_power,
+                                          double max_power, void *stream);
+/* Renders the window and writes header and body into out; *n_bytes = document length.  Synchronises `stream`.
+ * B200DD_ERR_ARG: nothing held yet.  The last push's code when that push was rejected (nothing written: blah2
+ * publishes nothing for that CPI).  B200DD_ERR_CAPACITY: cap < *n_bytes. */
+B200DD_API int b200dd_maxhold_fetch(b200dd_maxhold *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
+                                    void *stream);
+/* Test entry points: for each of n doubles, the /stash/map text of a cell whose only held value is v,
+ * comma-separated, an empty field where there is none (no map-document text, or hundredths outside int32).
+ * _host runs on the CPU (no device needed), _device in a kernel. */
+B200DD_API int b200dd_maxhold_format_doubles_host(const double *v, uint32_t n, char *out, size_t cap, size_t *n_bytes);
+B200DD_API int b200dd_maxhold_format_doubles_device(const double *v, uint32_t n, char *out, size_t cap,
+                                                    size_t *n_bytes, int32_t device);
+
 /* ------------------------------------------------------------------ whole CPI pipeline
  *
  * One coherent-processing interval through the body of the reference's process thread
@@ -485,6 +524,16 @@ B200DD_API int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectr
 B200DD_API int b200dd_pipeline_enable_map_json(b200dd_pipeline *h, size_t *max_bytes);
 B200DD_API int b200dd_pipeline_fetch_map_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
                                               size_t *n_bytes);
+
+/* Optional stage after set_metrics: pushes every CPI submitted afterwards into a max-hold window (see
+ * b200dd_maxhold_*), with the metrics set_metrics left on the device and the clutter filter's status word (no host
+ * round trip); works in recorded graphs.  Independent of the map JSON stage.  Drops the graphs recorded so far.
+ * b200dd_pipeline_fetch_maxhold, called after b200dd_pipeline_fetch, writes the /stash/map document after the last
+ * CPI; it returns B200DD_FILTER_FAILED, with the window unchanged, when that CPI's solve failed, and
+ * B200DD_ERR_ARG when the stage is not enabled or no CPI was accepted yet. */
+B200DD_API int b200dd_pipeline_enable_maxhold(b200dd_pipeline *h, size_t *max_bytes);
+B200DD_API int b200dd_pipeline_fetch_maxhold(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
+                                             size_t *n_bytes);
 
 /* ------------------------------------------------------------------------------------------------
  * Inter-GPU exchanges (one process per GPU, NCCL over NVLink / NVSwitch).  The reference has no
