@@ -157,6 +157,10 @@ SIGNATURES = [
     ("b200dd_pipeline_fetch_map_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_enable_maxhold", C.c_int, [_VP, C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_maxhold", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_enable_detection_json", C.c_int, [_VP, C.c_uint32, C.POINTER(C.c_size_t),
+                                                        C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_detection_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_detection_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),
     ("b200dd_mapjson_destroy", None, [_VP]),
@@ -176,6 +180,15 @@ SIGNATURES = [
     ("b200dd_maxhold_format_doubles_host", C.c_int, [_VP, C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_maxhold_format_doubles_device", C.c_int, [_VP, C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t),
                                                        C.c_int32]),
+    ("b200dd_detjson_create", C.c_int, [C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
+    ("b200dd_detjson_max_bytes", C.c_size_t, [_VP]),
+    ("b200dd_detjson_stash_max_bytes", C.c_size_t, [_VP]),
+    ("b200dd_detjson_destroy", None, [_VP]),
+    ("b200dd_detjson_render_device", C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
+    ("b200dd_detjson_fetch", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
+    ("b200dd_detjson_fetch_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
+    ("b200dd_detjson_render_host", C.c_int, [_VP, _VP, _VP, C.c_uint32, C.c_uint64, C.c_uint32, _VP, C.c_size_t,
+                                             C.POINTER(C.c_size_t)]),
     ("b200dd_comm_get_unique_id", C.c_int, [_VP]),
     ("b200dd_comm_create", C.c_int, [C.c_int32, C.c_int32, _VP, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_comm_destroy", None, [_VP]),

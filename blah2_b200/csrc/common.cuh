@@ -70,5 +70,22 @@ int mapjson_enqueue_with_metrics(b200dd_mapjson *h, const void *d_map, const dou
 // time; the CPI is rejected with B200DD_FILTER_FAILED when *d_filter_status (nullable) is non-zero.
 int maxhold_enqueue_with_metrics(b200dd_maxhold *h, const void *d_map, const double *d_metrics,
                                  const int *d_filter_status, cudaStream_t st);
+// maxhold.cu: ECMAScript Number::toString (radix 10) of a finite double, as JSON.stringify prints numbers.
+std::string js_number_text(double d);
+// det.cu: the detection list the last async chain left, the one b200dd_det_chain_fetch reads: its three device
+// arrays, the device word holding its length, the device word holding CFAR's count (the list is invalid when that
+// exceeds cap) and the list capacity.  B200DD_ERR_ARG when that chain ran no detection stage.
+struct DetDeviceList {
+  const double *delay, *doppler, *snr;
+  const uint32_t *count, *cfar_count;
+  uint32_t cap;
+};
+int det_device_list(b200dd_det *h, DetDeviceList *out);
+// detjson.cu: a render recorded in a graph was replayed (true), or the pipeline dropped the CPI's document (false).
+void detjson_mark_rendered(b200dd_detjson *h, bool rendered);
+// detjson.cu: B200DD_OK when no Interpolate result on these axes -- delay within one bin of the delay axis, Doppler
+// within one bin of the Doppler axis -- has hundredths outside int32 in the detection document; else
+// B200DD_ERR_GEOMETRY.
+int detjson_check_axes(const int32_t *delay, uint32_t n_del, const double *doppler, uint32_t n_dop, uint32_t fs);
 
 }  // namespace b2

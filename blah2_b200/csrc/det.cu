@@ -778,3 +778,14 @@ int b200dd_det_interpolate_host(b200dd_det *h, const double *delay, const double
 
 // the device word pair {noisePower, maxPower} that the async chain's set_metrics writes (for the map-JSON stage)
 const double *b2::det_device_metrics(b200dd_det *h) { return h->d_metrics; }
+
+int b2::det_device_list(b200dd_det *h, DetDeviceList *out) {
+  if (h->chain_slot < 0) return arg_fail("det_device_list: the last chain ran no detection stage");
+  out->delay = h->d_buf[h->chain_buf][0];
+  out->doppler = h->d_buf[h->chain_buf][1];
+  out->snr = h->d_buf[h->chain_buf][2];
+  out->count = h->d_n + h->chain_slot;
+  out->cfar_count = h->d_n;
+  out->cap = h->cap;
+  return B200DD_OK;
+}

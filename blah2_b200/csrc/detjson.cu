@@ -1,0 +1,595 @@
+// detjson.cu -- the detection document blah2 sends on its detection socket, and the API's 300-second detection
+// history served at /stash/detection, both rendered on the device.
+//
+// blah2 publishes every CPI's detections as  Detection::delay_bin_to_km(Detection::to_json(ts), fs)
+// (src/blah2.cpp:312-317, src/data/Detection.cpp:47-106):
+//   {"timestamp":T,"delay":[..km..],"doppler":[..Hz..],"snr":[..dB..]}
+// doppler and snr are written, read back and written again (jf::fmt_double_twice); delay is replaced by the km
+// value jf::bin_to_km and written once.  The API (api/stash/detection.js) parses every document, keeps those of the
+// last 300 s and serves the detections of all of them flattened into four arrays,
+//   {"timestamp":[..],"delay":[..],"doppler":[..],"snr":[..]}
+// each number re-printed by Number::toString.  Every delay, Doppler and SNR text is k/100 for an integer k (its
+// sent hundredths, json_fmt.cuh), so the history is a device ring of int32 triples.
+//
+// Per CPI (recordable in a graph: the launch shape is fixed by the list capacity, the count is read from a device
+// word, and tiles past the count exit at once):
+//   dj_len_kernel    formats each value with its separator, counts each tile's bytes, and writes the value's sent
+//                    hundredths to the ring position the stash will hold it at;
+//   scan_kernel      turns the tile counts of the three arrays into offsets in one body;
+//   dj_write_kernel  formats again, stages each tile at its 16-byte phase and stores it aligned (mapjson.cu).
+// The fetch composes the document around the three sections on the host, then commits the CPI's entries to the
+// stash with the timestamp and prunes as detection.js does.  The per-document records (timestamp, first entry,
+// count) stay on the host; the stash fetch renders the four arrays with the same three-kernel pattern, with the
+// timestamp texts made on the host once per document.
+#include "common.cuh"
+#include "json_fmt.cuh"
+#include "scan.cuh"
+
+#include <math.h>
+
+#include <cstring>
+#include <deque>
+#include <new>
+#include <string>
+#include <vector>
+
+using namespace b2;
+
+namespace {
+
+constexpr uint32_t kListCap = 1u << 18;  // the detection lists' capacity (det.cu)
+constexpr int kThreads = 256;
+constexpr int kRounds = 4;
+constexpr int kTile = kThreads * kRounds;
+constexpr uint32_t kDocTiles = kListCap / kTile;  // per array
+constexpr int kDocItemMax = jf::kMaxText + 1;     // "," before the value
+constexpr int kTsText = 20;                        // Number::toString of a uint64 as a double: "18446744073709552000"
+constexpr int kStashItemMax = kTsText + 1;
+constexpr uint32_t kMaxHeld = 1u << 25;            // keeps the stash text inside 32-bit offsets
+constexpr double kTime = 300.0;                    // seconds held, api/stash/detection.js:3
+
+// where the next document's entries go in the ring, and how many entries fit before a held one is overwritten;
+// written by the host after every commit
+struct DjRing {
+  uint32_t tail;
+  uint32_t room;
+};
+
+// what a render leaves for the fetch
+struct DjInfo {
+  uint32_t count;      // the list's count as read (may exceed the capacity)
+  uint32_t nonfinite;  // a value has no JSON text
+  uint32_t range;      // a value's hundredths lie outside int32
+  uint32_t body;       // body bytes (scan_kernel's total)
+};
+
+// The text of list value v of array arr (0 delay in bins, 1 Doppler, 2 SNR) as the document carries it; -1 when
+// blah2 sends no valid document for it.  Doppler and SNR: written, read back, written.  Delay: to_json writes the
+// bin and delay_bin_to_km parses that text (only a bin of |v| >= 1e308 can fail to read back), then the km value is
+// written once.
+__host__ __device__ __forceinline__ int value_text(int arr, double v, uint32_t fs, char *t) {
+  if (arr != 0) return jf::fmt_double_twice(v, t);
+  if (!jf::is_finite(v)) return -1;
+  if (!(fabs(v) < 1e308) && jf::fmt_double_twice(v, t) < 0) return -1;
+  const double km = jf::bin_to_km(v, fs);
+  return jf::is_finite(km) ? jf::fmt_double(km, t) : -1;
+}
+
+struct DocArgs {
+  const double *v[3];  // delay (bins), doppler (Hz), snr (dB)
+  const uint32_t *count;
+  uint32_t fs;
+  int32_t *ring;  // [3][ring_cap] sent hundredths
+  uint32_t ring_cap;
+  const DjRing *rs;
+  DjInfo *info;
+  uint32_t *tile_len;        // [3][kDocTiles]
+  const uint32_t *tile_off;  // [3 kDocTiles + 1]
+  char *body;
+};
+
+// item j of array arr: its separator and its text (*vlen = the text's length, -1 when the value has none)
+__device__ __forceinline__ int doc_item(const DocArgs &a, int arr, uint32_t j, char *t, int *vlen) {
+  int n = 0;
+  if (j) t[n++] = ',';
+  *vlen = value_text(arr, a.v[arr][j], a.fs, t + n);
+  return *vlen < 0 ? n : n + *vlen;
+}
+
+// __maxnreg__(64): at ptxas's own choice of 32 registers the formatting spills here
+__global__ void __maxnreg__(64) dj_len_kernel(DocArgs a) {
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const int arr = blockIdx.y;
+  const uint32_t tile = arr * kDocTiles + blockIdx.x;
+  const uint32_t raw = *a.count, n = raw < kListCap ? raw : kListCap;
+  if (blockIdx.x == 0 && arr == 0 && threadIdx.x == 0) a.info->count = raw;
+  const uint32_t base = blockIdx.x * kTile;
+  if (base >= n) {  // the same for the whole block
+    if (threadIdx.x == 0) a.tile_len[tile] = 0;
+    return;
+  }
+  const DjRing rs = *a.rs;
+  const bool stash = n <= rs.room;  // otherwise the commit overflows: leave the held entries alone
+  int32_t *plane = a.ring + (size_t)arr * a.ring_cap;
+  char t[kDocItemMax];
+  bool bad = false, range = false;
+  uint32_t sum = 0;
+#pragma unroll 1
+  for (int r = 0; r < kRounds; r++) {
+    const uint32_t j = base + r * kThreads + threadIdx.x;
+    if (j >= n) continue;
+    int vlen;
+    sum += (uint32_t)doc_item(a, arr, j, t, &vlen);
+    if (vlen < 0) {
+      bad = true;
+      continue;
+    }
+    int32_t k;
+    const char *vt = t + (j ? 1 : 0);
+    if (!jf::hundredths_of_text(vt, vlen, &k)) range = true;
+    else if (stash) plane[(uint32_t)(((uint64_t)rs.tail + j) % a.ring_cap)] = k;
+  }
+  if (bad) a.info->nonfinite = 1u;  // every writer stores the same value
+  if (range) a.info->range = 1u;
+  uint32_t tot;
+  block_excl_scan<kThreads>(sum, wsum, tot);
+  if (threadIdx.x == 0) a.tile_len[tile] = tot;
+}
+
+// Stages a tile's texts at the 16-byte phase of its offset and stores them aligned (mapjson.cu: mj_write_kernel).
+template <int ITEM_MAX, class F>
+__device__ __forceinline__ void write_tile(uint32_t off, char *body, char *stage, uint32_t *wsum, F item) {
+  const uint32_t phase = off & 15u;  // stage[phase + i] <-> body[off + i]: same address mod 16
+  char t[ITEM_MAX];
+  uint32_t pos = phase;
+  for (int r = 0; r < kRounds; r++) {
+    const int n = item(r, t);
+    uint32_t tot;
+    const uint32_t ex = block_excl_scan<kThreads>((uint32_t)n, wsum, tot);
+    for (int i = 0; i < n; i++) stage[pos + ex + i] = t[i];
+    pos += tot;
+  }
+  __syncthreads();
+  const uint32_t g0 = off, g1 = off + (pos - phase);
+  uint32_t a0 = (g0 + 15u) & ~15u, a1 = g1 & ~15u;
+  if (a0 > g1) a0 = g1;
+  if (a1 < a0) a1 = a0;
+  for (uint32_t g = g0 + threadIdx.x; g < a0; g += kThreads) body[g] = stage[g - off + phase];
+  for (uint32_t g = a1 + threadIdx.x; g < g1; g += kThreads) body[g] = stage[g - off + phase];
+  for (uint32_t g = a0 + 16u * threadIdx.x; g < a1; g += 16u * kThreads)
+    *reinterpret_cast<uint4 *>(body + g) = *reinterpret_cast<const uint4 *>(stage + (g - off + phase));
+}
+
+__global__ void __launch_bounds__(kThreads) dj_write_kernel(DocArgs a) {
+  __shared__ __align__(16) char stage[kTile * kDocItemMax + 16];
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const int arr = blockIdx.y;
+  const uint32_t raw = *a.count, n = raw < kListCap ? raw : kListCap;
+  const uint32_t base = blockIdx.x * kTile;
+  if (base >= n) return;
+  write_tile<kDocItemMax>(a.tile_off[arr * kDocTiles + blockIdx.x], a.body, stage, wsum, [&](int r, char *t) {
+    const uint32_t j = base + r * kThreads + threadIdx.x;
+    if (j >= n) return 0;
+    int vlen;
+    return doc_item(a, arr, j, t, &vlen);
+  });
+}
+
+struct StashArgs {
+  const int32_t *ring;  // [3][ring_cap]
+  uint32_t ring_cap, head, held;
+  const uint32_t *doc_first;  // [n_docs] first entry (relative to head) of each held document with entries
+  const uint32_t *doc_text;   // [n_docs + 1] offsets of their timestamp texts in texts
+  const char *texts;
+  uint32_t n_docs, tiles;     // tiles per array
+  uint32_t *tile_len;         // [4][tiles]
+  const uint32_t *tile_off;   // [4 tiles + 1]
+  char *body;
+};
+
+// entry e of array arr (0 timestamp, 1 delay, 2 doppler, 3 snr) of the /stash/detection text, with its separator
+__device__ __forceinline__ int stash_item(const StashArgs &a, int arr, uint32_t e, char *t) {
+  int n = 0;
+  if (e) t[n++] = ',';
+  if (arr == 0) {  // the last document whose first entry is <= e holds e
+    uint32_t lo = 0, hi = a.n_docs;
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (a.doc_first[mid] <= e) lo = mid;
+      else hi = mid;
+    }
+    for (uint32_t i = a.doc_text[lo]; i < a.doc_text[lo + 1]; i++) t[n++] = a.texts[i];
+    return n;
+  }
+  const uint32_t slot = (uint32_t)(((uint64_t)a.head + e) % a.ring_cap);
+  return n + jf::fmt_hundredths(a.ring[(size_t)(arr - 1) * a.ring_cap + slot], t + n);
+}
+
+__global__ void __launch_bounds__(kThreads) ds_len_kernel(StashArgs a) {
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const int arr = blockIdx.y;
+  const uint32_t base = blockIdx.x * kTile;
+  char t[kStashItemMax];
+  uint32_t sum = 0;
+  for (int r = 0; r < kRounds; r++) {
+    const uint32_t e = base + r * kThreads + threadIdx.x;
+    if (e < a.held) sum += (uint32_t)stash_item(a, arr, e, t);
+  }
+  uint32_t tot;
+  block_excl_scan<kThreads>(sum, wsum, tot);
+  if (threadIdx.x == 0) a.tile_len[arr * a.tiles + blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(kThreads) ds_write_kernel(StashArgs a) {
+  __shared__ __align__(16) char stage[kTile * kStashItemMax + 16];
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const int arr = blockIdx.y;
+  const uint32_t base = blockIdx.x * kTile;
+  write_tile<kStashItemMax>(a.tile_off[arr * a.tiles + blockIdx.x], a.body, stage, wsum, [&](int r, char *t) {
+    const uint32_t e = base + r * kThreads + threadIdx.x;
+    return e < a.held ? stash_item(a, arr, e, t) : 0;
+  });
+}
+
+inline int nonfinite_fail(const char *msg) {
+  set_last_error(msg);
+  return B200DD_ERR_NONFINITE;
+}
+
+const char *const kDocHead[3] = {",\"delay\":[", "],\"doppler\":[", "],\"snr\":["};
+const char *const kStashHead[4] = {"{\"timestamp\":[", "],\"delay\":[", "],\"doppler\":[", "],\"snr\":["};
+
+}  // namespace
+
+struct b200dd_detjson {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  uint32_t fs = 0, ring_cap = 0, stash_tiles = 0;
+  size_t max_bytes = 0, stash_max_bytes = 0;
+  // per-CPI render
+  char *d_body = nullptr;
+  uint32_t *d_tile_len = nullptr, *d_tile_off = nullptr;  // [3 kDocTiles], [3 kDocTiles + 1]
+  DjInfo *d_info = nullptr;
+  DjRing *d_ring_state = nullptr;
+  bool pending = false;  // a render not fetched yet
+  // stash
+  int32_t *d_ring = nullptr;  // [3][ring_cap]
+  char *d_stash = nullptr;
+  uint32_t *d_stile_len = nullptr, *d_stile_off = nullptr;
+  uint32_t *d_doc_first = nullptr, *d_doc_text = nullptr;
+  char *d_texts = nullptr;
+  size_t first_alloc = 0, toff_alloc = 0, texts_alloc = 0;  // elements allocated
+  struct Record {
+    uint64_t ts, first;  // first: absolute entry number
+    uint32_t count;
+    std::string text;  // Number::toString of the timestamp
+  };
+  std::deque<Record> records;
+  uint64_t head = 0, tail = 0;  // absolute entry numbers: [head, tail) held
+  bool overflowed = false;
+  DjRing ring_state{0, 0};
+};
+
+namespace {
+
+int upload_ring_state(b200dd_detjson *h, cudaStream_t st) {
+  h->ring_state.tail = (uint32_t)(h->tail % h->ring_cap);
+  h->ring_state.room = h->ring_cap - (uint32_t)(h->tail - h->head);
+  B2_CUDA(cudaMemcpyAsync(h->d_ring_state, &h->ring_state, sizeof(DjRing), cudaMemcpyHostToDevice, st));
+  return B200DD_OK;
+}
+
+// detection.js:39-51: push the document, then the prune loop that shifts the array while its index advances
+int commit(b200dd_detjson *h, uint64_t ts, uint32_t n, cudaStream_t st) {
+  if (h->overflowed) return B200DD_OK;  // the stash is lost already; the document stands on its own
+  if ((h->tail - h->head) + n > h->ring_cap) {
+    h->overflowed = true;
+    set_last_error("b200dd_detjson_fetch: the stash's ring is full (see max_held): the document was written, the "
+                   "stash is lost until the stage is created again");
+    return B200DD_ERR_CAPACITY;
+  }
+  h->records.push_back({ts, h->tail, n, js_number_text((double)ts)});
+  h->tail += n;
+  const double now = (double)ts;  // JS numbers: the timestamps as JSON.parse reads them
+  for (size_t i = 0; i < h->records.size(); i++) {
+    if ((now - (double)h->records[i].ts) / 1000 > kTime) {
+      h->head += h->records.front().count;
+      h->records.pop_front();
+    } else {
+      break;
+    }
+  }
+  return upload_ring_state(h, st);
+}
+
+// device array p of `have` elements grown to at least `need` (doubling), contents not kept
+template <class T> int grow(T *&p, size_t &have, size_t need) {
+  if (need <= have) return B200DD_OK;
+  free_dev(p);
+  have = 0;
+  const size_t n = need * 2;
+  B2_CUDA(cudaMalloc(&p, sizeof(T) * n));
+  have = n;
+  return B200DD_OK;
+}
+
+}  // namespace
+
+void b2::detjson_mark_rendered(b200dd_detjson *h, bool rendered) { h->pending = rendered; }
+
+int b2::detjson_check_axes(const int32_t *delay, uint32_t n_del, const double *doppler, uint32_t n_dop, uint32_t fs) {
+  char t[jf::kMaxText];
+  int32_t k;
+  // an interpolated value lies within half a bin of its cell (the peak of a parabola through a local maximum)
+  for (const double bin : {(double)delay[0] - 1.0, (double)delay[n_del - 1] + 1.0}) {
+    const double km = jf::bin_to_km(bin, fs);
+    if (!jf::is_finite(km) || !jf::hundredths_of_text(t, jf::fmt_double(km, t), &k))
+      return geom_fail("detection JSON: a delay near the axis has hundredths of a km outside int32");
+  }
+  const double res = n_dop > 1 ? doppler[1] - doppler[0] : 0.0;
+  for (const double hz : {doppler[0] - res, doppler[n_dop - 1] + res})
+    if (!jf::hundredths(hz, &k)) return geom_fail("detection JSON: a Doppler near the axis has hundredths outside int32");
+  return B200DD_OK;
+}
+
+extern "C" {
+
+int b200dd_detjson_create(uint32_t fs, uint32_t max_held, int32_t device, b200dd_detjson **out) {
+  if (!out) return arg_fail("b200dd_detjson_create: null argument");
+  *out = nullptr;
+  if (fs == 0) return arg_fail("b200dd_detjson_create: fs must be positive");
+  if (max_held == 0 || max_held > kMaxHeld) return arg_fail("b200dd_detjson_create: max_held must be in [1, 2^25]");
+  b200dd_detjson *h = new (std::nothrow) b200dd_detjson();
+  if (!h) return arg_fail("b200dd_detjson_create: out of host memory");
+  auto fail = [&](int rc) { b200dd_detjson_destroy(h); return rc; };
+  h->fs = fs;
+  h->ring_cap = max_held;
+  h->stash_tiles = (max_held + kTile - 1) / kTile;
+  // every value's text is at most kMaxText bytes plus its comma
+  h->max_bytes = strlen("{\"timestamp\":18446744073709551615") + strlen(kDocHead[0]) + strlen(kDocHead[1]) +
+                 strlen(kDocHead[2]) + 2 + 3 * (size_t)kListCap * kDocItemMax;
+  h->stash_max_bytes = strlen(kStashHead[0]) + strlen(kStashHead[1]) + strlen(kStashHead[2]) +
+                       strlen(kStashHead[3]) + 2 + (size_t)max_held * (kStashItemMax + 3 * (jf::kMaxHundredthsText + 1));
+  int dev = device;
+  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
+  h->device = dev;
+  DeviceGuard guard(dev);
+  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
+  auto body = [&]() -> int {
+    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    B2_CUDA(cudaMalloc(&h->d_body, (3 * (size_t)kListCap * kDocItemMax + 15) & ~(size_t)15));
+    B2_CUDA(cudaMalloc(&h->d_tile_len, sizeof(uint32_t) * 3 * kDocTiles));
+    B2_CUDA(cudaMalloc(&h->d_tile_off, sizeof(uint32_t) * (3 * kDocTiles + 1)));
+    B2_CUDA(cudaMalloc(&h->d_info, sizeof(DjInfo)));
+    B2_CUDA(cudaMalloc(&h->d_ring_state, sizeof(DjRing)));
+    B2_CUDA(cudaMalloc(&h->d_ring, sizeof(int32_t) * 3 * (size_t)max_held));
+    B2_CUDA(cudaMalloc(&h->d_stash, (h->stash_max_bytes + 15) & ~(size_t)15));
+    B2_CUDA(cudaMalloc(&h->d_stile_len, sizeof(uint32_t) * 4 * h->stash_tiles));
+    B2_CUDA(cudaMalloc(&h->d_stile_off, sizeof(uint32_t) * (4 * h->stash_tiles + 1)));
+    const int rc = upload_ring_state(h, h->stream);
+    if (rc != B200DD_OK) return rc;
+    B2_CUDA(cudaStreamSynchronize(h->stream));  // the ring state is set before a render on another stream
+    return B200DD_OK;
+  };
+  const int rc = body();
+  if (rc != B200DD_OK) return fail(rc);
+  *out = h;
+  return B200DD_OK;
+}
+
+size_t b200dd_detjson_max_bytes(const b200dd_detjson *h) { return h ? h->max_bytes : 0; }
+size_t b200dd_detjson_stash_max_bytes(const b200dd_detjson *h) { return h ? h->stash_max_bytes : 0; }
+
+void b200dd_detjson_destroy(b200dd_detjson *h) {
+  if (!h) return;
+  {
+    DeviceGuard guard(h->device);
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    free_dev(h->d_body);
+    free_dev(h->d_tile_len);
+    free_dev(h->d_tile_off);
+    free_dev(h->d_info);
+    free_dev(h->d_ring_state);
+    free_dev(h->d_ring);
+    free_dev(h->d_stash);
+    free_dev(h->d_stile_len);
+    free_dev(h->d_stile_off);
+    free_dev(h->d_doc_first);
+    free_dev(h->d_doc_text);
+    free_dev(h->d_texts);
+    if (h->stream) cudaStreamDestroy(h->stream);
+  }
+  delete h;
+}
+
+int b200dd_detjson_render_device(b200dd_detjson *h, const double *d_delay, const double *d_doppler,
+                                 const double *d_snr, const uint32_t *d_count, void *stream) {
+  if (!h || !d_delay || !d_doppler || !d_snr || !d_count) return arg_fail("b200dd_detjson_render_device: null argument");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  DocArgs a;
+  a.v[0] = d_delay; a.v[1] = d_doppler; a.v[2] = d_snr; a.count = d_count; a.fs = h->fs;
+  a.ring = h->d_ring; a.ring_cap = h->ring_cap; a.rs = h->d_ring_state; a.info = h->d_info;
+  a.tile_len = h->d_tile_len; a.tile_off = h->d_tile_off; a.body = h->d_body;
+  B2_CUDA(cudaMemsetAsync(h->d_info, 0, sizeof(DjInfo), st));
+  dj_len_kernel<<<dim3(kDocTiles, 3), kThreads, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)(3 * kDocTiles), &h->d_info->body);
+  B2_LAUNCH_CHECK();
+  dj_write_kernel<<<dim3(kDocTiles, 3), kThreads, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  h->pending = true;
+  return B200DD_OK;
+}
+
+int b200dd_detjson_fetch(b200dd_detjson *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes, void *stream) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_detjson_fetch: null argument");
+  if (!h->pending) return arg_fail("b200dd_detjson_fetch: nothing rendered since the last fetch");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  DjInfo info;
+  uint32_t ends[3];  // where the delay, doppler and snr sections end in the body
+  B2_CUDA(cudaMemcpyAsync(&info, h->d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpy2DAsync(ends, sizeof(uint32_t), h->d_tile_off + kDocTiles, sizeof(uint32_t) * kDocTiles,
+                            sizeof(uint32_t), 3, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  if (info.count > kListCap) {
+    h->pending = false;
+    set_last_error("b200dd_detjson_fetch: more detections than the list capacity (2^18): no document");
+    return B200DD_ERR_CAPACITY;
+  }
+  if (info.nonfinite) {
+    h->pending = false;
+    return nonfinite_fail("b200dd_detjson_fetch: a delay, Doppler or SNR has no JSON text: no document");
+  }
+  const std::string hdr = "{\"timestamp\":" + std::to_string((unsigned long long)timestamp);
+  const uint32_t sec[3] = {ends[0], ends[1] - ends[0], ends[2] - ends[1]};
+  size_t total = hdr.size() + 2;
+  for (int i = 0; i < 3; i++) total += strlen(kDocHead[i]) + sec[i];
+  if (n_bytes) *n_bytes = total;
+  if (total > cap) {
+    set_last_error("b200dd_detjson_fetch: output capacity too small (see b200dd_detjson_max_bytes)");
+    return B200DD_ERR_CAPACITY;
+  }
+  char *p = out;
+  memcpy(p, hdr.data(), hdr.size());
+  p += hdr.size();
+  uint32_t from = 0;
+  for (int i = 0; i < 3; i++) {
+    memcpy(p, kDocHead[i], strlen(kDocHead[i]));
+    p += strlen(kDocHead[i]);
+    if (sec[i]) B2_CUDA(cudaMemcpyAsync(p, h->d_body + from, sec[i], cudaMemcpyDeviceToHost, st));
+    p += sec[i];
+    from += sec[i];
+  }
+  p[0] = ']';
+  p[1] = '}';
+  B2_CUDA(cudaStreamSynchronize(st));
+  h->pending = false;
+  if (info.range) {
+    set_last_error("b200dd_detjson_fetch: a value's hundredths lie outside int32: the document was written, the "
+                   "stash does not take it");
+    return B200DD_ERR_ARG;
+  }
+  return commit(h, timestamp, info.count, st);
+}
+
+int b200dd_detjson_fetch_stash(b200dd_detjson *h, char *out, size_t cap, size_t *n_bytes, void *stream) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_detjson_fetch_stash: null argument");
+  if (h->overflowed) {
+    set_last_error("b200dd_detjson_fetch_stash: the stash's ring overflowed (see max_held)");
+    return B200DD_ERR_CAPACITY;
+  }
+  if (h->records.empty()) {  // detection.js:10, output = []
+    if (n_bytes) *n_bytes = 2;
+    if (cap < 2) return B200DD_ERR_CAPACITY;
+    out[0] = '[';
+    out[1] = ']';
+    return B200DD_OK;
+  }
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  const uint32_t held = (uint32_t)(h->tail - h->head);
+  std::vector<uint32_t> first, toff{0};
+  std::string texts;
+  for (const auto &r : h->records) {
+    if (!r.count) continue;
+    first.push_back((uint32_t)(r.first - h->head));
+    texts += r.text;
+    toff.push_back((uint32_t)texts.size());
+  }
+  uint32_t ends[4] = {0, 0, 0, 0};
+  const uint32_t tiles = (held + kTile - 1) / kTile;
+  if (held) {
+    int rc = grow(h->d_doc_first, h->first_alloc, first.size());
+    if (rc == B200DD_OK) rc = grow(h->d_doc_text, h->toff_alloc, toff.size());
+    if (rc == B200DD_OK) rc = grow(h->d_texts, h->texts_alloc, texts.size());
+    if (rc != B200DD_OK) return rc;
+    B2_CUDA(cudaMemcpyAsync(h->d_doc_first, first.data(), sizeof(uint32_t) * first.size(), cudaMemcpyHostToDevice, st));
+    B2_CUDA(cudaMemcpyAsync(h->d_doc_text, toff.data(), sizeof(uint32_t) * toff.size(), cudaMemcpyHostToDevice, st));
+    B2_CUDA(cudaMemcpyAsync(h->d_texts, texts.data(), texts.size(), cudaMemcpyHostToDevice, st));
+    StashArgs a;
+    a.ring = h->d_ring; a.ring_cap = h->ring_cap; a.head = (uint32_t)(h->head % h->ring_cap); a.held = held;
+    a.doc_first = h->d_doc_first; a.doc_text = h->d_doc_text; a.texts = h->d_texts; a.n_docs = (uint32_t)first.size();
+    a.tiles = tiles; a.tile_len = h->d_stile_len; a.tile_off = h->d_stile_off; a.body = h->d_stash;
+    ds_len_kernel<<<dim3(tiles, 4), kThreads, 0, st>>>(a);
+    B2_LAUNCH_CHECK();
+    scan_kernel<<<1, 1024, 0, st>>>(h->d_stile_len, h->d_stile_off, (int)(4 * tiles), h->d_stile_off + 4 * tiles);
+    B2_LAUNCH_CHECK();
+    ds_write_kernel<<<dim3(tiles, 4), kThreads, 0, st>>>(a);
+    B2_LAUNCH_CHECK();
+    B2_CUDA(cudaMemcpy2DAsync(ends, sizeof(uint32_t), h->d_stile_off + tiles, sizeof(uint32_t) * tiles,
+                              sizeof(uint32_t), 4, cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaStreamSynchronize(st));
+  }
+  size_t total = 2;
+  uint32_t sec[4];
+  for (int i = 0; i < 4; i++) {
+    sec[i] = ends[i] - (i ? ends[i - 1] : 0);
+    total += strlen(kStashHead[i]) + sec[i];
+  }
+  if (n_bytes) *n_bytes = total;
+  if (total > cap) {
+    set_last_error("b200dd_detjson_fetch_stash: output capacity too small (see b200dd_detjson_stash_max_bytes)");
+    return B200DD_ERR_CAPACITY;
+  }
+  char *p = out;
+  uint32_t from = 0;
+  for (int i = 0; i < 4; i++) {
+    memcpy(p, kStashHead[i], strlen(kStashHead[i]));
+    p += strlen(kStashHead[i]);
+    if (sec[i]) B2_CUDA(cudaMemcpyAsync(p, h->d_stash + from, sec[i], cudaMemcpyDeviceToHost, st));
+    p += sec[i];
+    from += sec[i];
+  }
+  p[0] = ']';
+  p[1] = '}';
+  B2_CUDA(cudaStreamSynchronize(st));
+  return B200DD_OK;
+}
+
+int b200dd_detjson_render_host(const double *delay, const double *doppler, const double *snr, uint32_t n,
+                               uint64_t timestamp, uint32_t fs, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if ((n && (!delay || !doppler || !snr)) || !out) return arg_fail("b200dd_detjson_render_host: null argument");
+  if (fs == 0) return arg_fail("b200dd_detjson_render_host: fs must be positive");
+  const double *v[3] = {delay, doppler, snr};
+  std::vector<char> text((size_t)n * 3 * jf::kMaxText);
+  std::vector<int> len((size_t)n * 3);
+  const std::string hdr = "{\"timestamp\":" + std::to_string((unsigned long long)timestamp);
+  size_t total = hdr.size() + 2;
+  for (int arr = 0; arr < 3; arr++) {
+    total += strlen(kDocHead[arr]) + (n ? n - 1 : 0);
+    for (uint32_t j = 0; j < n; j++) {
+      const size_t i = (size_t)arr * n + j;
+      len[i] = value_text(arr, v[arr][j], fs, text.data() + i * jf::kMaxText);
+      if (len[i] < 0) return nonfinite_fail("b200dd_detjson_render_host: a delay, Doppler or SNR has no JSON text");
+      total += (size_t)len[i];
+    }
+  }
+  if (n_bytes) *n_bytes = total;
+  if (total > cap) {
+    set_last_error("b200dd_detjson_render_host: output capacity too small");
+    return B200DD_ERR_CAPACITY;
+  }
+  char *p = out;
+  memcpy(p, hdr.data(), hdr.size());
+  p += hdr.size();
+  for (int arr = 0; arr < 3; arr++) {
+    memcpy(p, kDocHead[arr], strlen(kDocHead[arr]));
+    p += strlen(kDocHead[arr]);
+    for (uint32_t j = 0; j < n; j++) {
+      const size_t i = (size_t)arr * n + j;
+      if (j) *p++ = ',';
+      memcpy(p, text.data() + i * jf::kMaxText, (size_t)len[i]);
+      p += len[i];
+    }
+  }
+  p[0] = ']';
+  p[1] = '}';
+  return B200DD_OK;
+}
+
+}  // extern "C"

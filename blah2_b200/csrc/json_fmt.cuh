@@ -507,12 +507,9 @@ JF_HD double cell_db(double re, double im, double noise) {
 // longest text fmt_hundredths() can produce: "-21474836.48"
 constexpr int kMaxHundredthsText = 12;
 
-// The sent hundredths of v: parses the text fmt_double_twice gives (no floating-point step of its own).  False when
-// v has no text (not finite, or not readable back) or k lies outside int32 (an exponent form included).
-JF_HD bool hundredths(double v, int32_t *k) {
-  char t[kMaxText];
-  const int n = fmt_double_twice(v, t);
-  if (n < 0) return false;
+// The hundredths k of a text t[0..n) as fmt_double writes it (no floating-point step).  False when k lies outside
+// int32 (an exponent form included).
+JF_HD bool hundredths_of_text(const char *t, int n, int32_t *k) {
   int p = t[0] == '-' ? 1 : 0;
   const bool minus = p == 1;
   int64_t a = 0;
@@ -534,6 +531,22 @@ JF_HD bool hundredths(double v, int32_t *k) {
   if (a > 2147483647) return false;
   *k = (int32_t)(minus ? -a : a);
   return true;
+}
+
+// The sent hundredths of v: parses the text fmt_double_twice gives.  False when v has no text (not finite, or not
+// readable back) or k lies outside int32.
+JF_HD bool hundredths(double v, int32_t *k) {
+  char t[kMaxText];
+  const int n = fmt_double_twice(v, t);
+  if (n < 0) return false;
+  return hundredths_of_text(t, n, k);
+}
+
+// A delay in bins as the km value delay_bin_to_km pushes: 1.0 * bin * (Constants::c / (double)fs) / 1000 with
+// Constants::c the uint32_t 299792458 (Map.cpp:176, Detection.cpp:98).  1.0 * bin is exact; the other three
+// operations are rounded one by one.
+JF_HD double bin_to_km(double bin, uint32_t fs) {
+  return div_rn(mul_rn(bin, div_rn(299792458.0, (double)fs)), 1000.0);
 }
 
 // ECMAScript Number::toString of the double nearest k/100: the canonical decimal of k/100 (sign, integer part,

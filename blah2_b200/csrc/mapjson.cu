@@ -34,7 +34,6 @@ constexpr int kThreads = 256;
 constexpr int kRounds = 4;
 constexpr int kTile = kThreads * kRounds;    // cells per CTA
 constexpr int kCellMax = jf::kMaxText + 3;  // ",[" before the value, "]" after it
-constexpr uint32_t kC = 299792458u;          // Constants::c (src/data/meta/Constants.h), uint32_t
 
 template <class TMAP> __device__ __forceinline__ double2 ld_cell(const TMAP *m, size_t i) {
   const TMAP v = m[i];
@@ -246,7 +245,7 @@ int b200dd_mapjson_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, 
   h->nTiles = (uint32_t)((h->cells + kTile - 1) / kTile);
   // delay axis in km, written once (Map.cpp:176); the Doppler axis goes through to_json and delay_bin_to_km
   std::vector<double> km(n_del);
-  for (uint32_t i = 0; i < n_del; i++) km[i] = 1.0 * delay[i] * (kC / (double)fs) / 1000;
+  for (uint32_t i = 0; i < n_del; i++) km[i] = jf::bin_to_km(delay[i], fs);
   h->axes_ok = array_text(km.data(), n_del, false, h->delay_txt) && array_text(doppler, n_dop, true, h->doppler_txt);
   // body: every cell's text is at most kMaxText bytes, plus n_del - 1 commas and two brackets per row, plus a
   // comma between rows

@@ -36,7 +36,6 @@ constexpr int kThreads = 256;
 constexpr int kRounds = 4;
 constexpr int kTile = kThreads * kRounds;
 constexpr int kCellMax = jf::kMaxHundredthsText + 3;  // ",[" before the value, "]" after it
-constexpr uint32_t kC = 299792458u;                   // Constants::c, as in mapjson.cu
 constexpr double kNoiseBound = 1e7;  // |noisePower| <= 1e7 dB keeps every finite double cell inside int32 hundredths
 
 // ring state, one device copy per handle
@@ -174,43 +173,6 @@ __global__ void mh_format_kernel(const double *v, uint32_t n, char *text, int *l
   }
 }
 
-// ECMAScript Number::toString (ECMA-262 6.1.6.1.20, radix 10) of a finite double: the fewest significant digits
-// that read back to d (the first precision whose correctly rounded %e text does), then the standard's layout.
-std::string js_number_text(double d) {
-  if (d == 0.0) return "0";  // -0 too
-  std::string out;
-  if (d < 0) {
-    out = "-";
-    d = -d;
-  }
-  char buf[40];
-  for (int p = 1; p <= 17; p++) {
-    snprintf(buf, sizeof(buf), "%.*e", p - 1, d);
-    if (strtod(buf, nullptr) == d) break;
-  }
-  // buf = "D[.DDD]e[+-]XX": digits s (k of them), value = s * 10^(n - k)
-  std::string s;
-  const char *p = buf;
-  for (; *p != 'e'; p++)
-    if (*p != '.') s += *p;
-  const int n = atoi(p + 1) + 1;
-  while (s.size() > 1 && s.back() == '0') s.pop_back();
-  const int k = (int)s.size();
-  if (k <= n && n <= 21) {
-    out += s;
-    out.append((size_t)(n - k), '0');
-  } else if (0 < n && n <= 21) {
-    out += s.substr(0, (size_t)n) + "." + s.substr((size_t)n);
-  } else if (-6 < n && n <= 0) {
-    out += "0." + std::string((size_t)-n, '0') + s;
-  } else {
-    out += s.substr(0, 1);
-    if (k > 1) out += "." + s.substr(1);
-    out += (n - 1 < 0 ? "e-" : "e+") + std::to_string(n - 1 < 0 ? 1 - n : n - 1);
-  }
-  return out;
-}
-
 // JSON.stringify of the array JSON.parse reads from "[a,b,..]" of the values' texts (once or twice formatted, as
 // mapjson.cu writes the axes); false when a value has no text
 bool js_array_text(const double *v, size_t n, bool twice, std::string &out) {
@@ -257,6 +219,43 @@ int join_texts(const char *text, const int *len, uint32_t n, char *out, size_t c
 }
 
 }  // namespace
+
+// ECMAScript Number::toString (ECMA-262 6.1.6.1.20, radix 10) of a finite double: the fewest significant digits
+// that read back to d (the first precision whose correctly rounded %e text does), then the standard's layout.
+std::string b2::js_number_text(double d) {
+  if (d == 0.0) return "0";  // -0 too
+  std::string out;
+  if (d < 0) {
+    out = "-";
+    d = -d;
+  }
+  char buf[40];
+  for (int p = 1; p <= 17; p++) {
+    snprintf(buf, sizeof(buf), "%.*e", p - 1, d);
+    if (strtod(buf, nullptr) == d) break;
+  }
+  // buf = "D[.DDD]e[+-]XX": digits s (k of them), value = s * 10^(n - k)
+  std::string s;
+  const char *p = buf;
+  for (; *p != 'e'; p++)
+    if (*p != '.') s += *p;
+  const int n = atoi(p + 1) + 1;
+  while (s.size() > 1 && s.back() == '0') s.pop_back();
+  const int k = (int)s.size();
+  if (k <= n && n <= 21) {
+    out += s;
+    out.append((size_t)(n - k), '0');
+  } else if (0 < n && n <= 21) {
+    out += s.substr(0, (size_t)n) + "." + s.substr((size_t)n);
+  } else if (-6 < n && n <= 0) {
+    out += "0." + std::string((size_t)-n, '0') + s;
+  } else {
+    out += s.substr(0, 1);
+    if (k > 1) out += "." + s.substr(1);
+    out += (n - 1 < 0 ? "e-" : "e+") + std::to_string(n - 1 < 0 ? 1 - n : n - 1);
+  }
+  return out;
+}
 
 struct b200dd_maxhold {
   int device = 0;
@@ -325,7 +324,7 @@ int b200dd_maxhold_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, 
   h->nTiles = (uint32_t)((h->cells + kTile - 1) / kTile);
   // the axes as the map document carries them (mapjson.cu), then parsed and re-printed by the stash
   std::vector<double> km(n_del);
-  for (uint32_t i = 0; i < n_del; i++) km[i] = 1.0 * delay[i] * (kC / (double)fs) / 1000;
+  for (uint32_t i = 0; i < n_del; i++) km[i] = jf::bin_to_km(delay[i], fs);
   h->axes_ok = js_array_text(km.data(), n_del, false, h->delay_txt) &&
                js_array_text(doppler, n_dop, true, h->doppler_txt);
   h->body_max = h->cells * jf::kMaxHundredthsText + (size_t)n_dop * (n_del + 1) + (n_dop - 1);

@@ -1,6 +1,6 @@
 // pipeline.cu -- one CPI through WienerHopf -> Ambiguity -> set_metrics -> detection with all
 // intermediates resident in HBM (the body of the reference's process thread, src/blah2.cpp:268-287).
-// Composes the per-class handles of caf.cu / wh.cu / det.cu / mapjson.cu / maxhold.cu through their C ABI; the only kernels
+// Composes the per-class handles of caf.cu / wh.cu / det.cu / mapjson.cu / maxhold.cu / detjson.cu through their C ABI; the only kernels
 // defined here are the complex128 <-> complex64 conversions of the host entry point.
 #include "common.cuh"
 
@@ -56,6 +56,8 @@ struct b200dd_pipeline {
   void *mj_stream = nullptr;        // stream of the last submit, where its document was rendered
   b200dd_maxhold *mh = nullptr;     // optional: the API's max-hold window (api/stash/maxhold.js)
   void *mh_stream = nullptr;        // stream of the last submit, where its push was enqueued
+  b200dd_detjson *dj = nullptr;     // optional: the detection document (blah2.cpp:312-317) and its stash
+  void *dj_stream = nullptr;        // stream of the last submit, where its document was rendered
   uint32_t spec_bins = 0, spec_nfft = 0;
   b200dd_caf_geometry g;
   std::vector<int32_t> delay;
@@ -135,6 +137,7 @@ void b200dd_pipeline_destroy(b200dd_pipeline *h) {
     b200dd_spectrum_destroy(h->spec);
     b200dd_mapjson_destroy(h->mj);
     b200dd_maxhold_destroy(h->mh);
+    b200dd_detjson_destroy(h->dj);
     free_dev(h->d_yf);
     free_dev(h->d_xd);
     free_dev(h->d_yd);
@@ -170,8 +173,16 @@ static int pipeline_enqueue_products(b200dd_pipeline *h, float2 *map, void *st) 
   }
   if (h->mh) {
     h->mh_stream = st;
-    return maxhold_enqueue_with_metrics(h->mh, map, det_device_metrics(h->det),
-                                        h->wh ? b200dd_wh_device_status(h->wh) : nullptr, (cudaStream_t)st);
+    const int rc = maxhold_enqueue_with_metrics(h->mh, map, det_device_metrics(h->det),
+                                                h->wh ? b200dd_wh_device_status(h->wh) : nullptr, (cudaStream_t)st);
+    if (rc != B200DD_OK) return rc;
+  }
+  if (h->dj) {
+    h->dj_stream = st;
+    DetDeviceList l;
+    const int rc = det_device_list(h->det, &l);
+    if (rc != B200DD_OK) return rc;
+    return b200dd_detjson_render_device(h->dj, l.delay, l.doppler, l.snr, l.count, st);
   }
   return B200DD_OK;
 }
@@ -232,6 +243,10 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   h->last_had_filter = h->wh != nullptr;
   h->mj_stream = st;
   h->mh_stream = st;
+  if (h->dj) {
+    h->dj_stream = st;
+    detjson_mark_rendered(h->dj, true);
+  }
   B2_CUDA(cudaGraphLaunch(g->exec, (cudaStream_t)st));
   return B200DD_OK;
 }
@@ -465,6 +480,62 @@ int b200dd_pipeline_fetch_maxhold(b200dd_pipeline *h, uint64_t timestamp, char *
   if (!h->mh_stream) return arg_fail("b200dd_pipeline_fetch_maxhold: no CPI submitted since the stage was enabled");
   DeviceGuard guard(h->device);
   return b200dd_maxhold_fetch(h->mh, timestamp, out, cap, n_bytes, h->mh_stream);
+}
+
+int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held, size_t *doc_bytes,
+                                          size_t *stash_bytes) {
+  if (!h) return arg_fail("b200dd_pipeline_enable_detection_json: null handle");
+  if (!h->p.detection_enable) return arg_fail("b200dd_pipeline_enable_detection_json: detection is not enabled");
+  int rc = detjson_check_axes(h->delay.data(), h->g.n_delay_bins, h->doppler.data(), h->g.n_doppler_bins, h->p.caf.fs);
+  if (rc != B200DD_OK) return rc;
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  pipeline_drop_graphs(h);  // the chain changes
+  b200dd_detjson_destroy(h->dj);
+  h->dj = nullptr;
+  h->dj_stream = nullptr;
+  rc = b200dd_detjson_create(h->p.caf.fs, max_held, h->device, &h->dj);
+  if (rc != B200DD_OK) return rc;
+  if (doc_bytes) *doc_bytes = b200dd_detjson_max_bytes(h->dj);
+  if (stash_bytes) *stash_bytes = b200dd_detjson_stash_max_bytes(h->dj);
+  return B200DD_OK;
+}
+
+int b200dd_pipeline_fetch_detection_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
+                                         size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_detection_json: null argument");
+  if (!h->dj) return arg_fail("b200dd_pipeline_fetch_detection_json: the detection JSON stage is not enabled");
+  if (!h->dj_stream) return arg_fail("b200dd_pipeline_fetch_detection_json: no CPI submitted since the stage was enabled");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = (cudaStream_t)h->dj_stream;
+  DetDeviceList l;
+  int rc = det_device_list(h->det, &l);
+  if (rc != B200DD_OK) return rc;
+  int fs = 0;
+  uint32_t cfar = 0;
+  if (h->last_had_filter) B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(&cfar, l.cfar_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  if (fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273): no detections are sent
+    detjson_mark_rendered(h->dj, false);
+    set_last_error("b200dd_pipeline_fetch_detection_json: the CPI's clutter-filter solve failed; it has no detections");
+    return B200DD_FILTER_FAILED;
+  }
+  if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
+    detjson_mark_rendered(h->dj, false);
+    set_last_error("b200dd_pipeline_fetch_detection_json: more CFAR detections than the list capacity (2^18)");
+    return B200DD_ERR_CAPACITY;
+  }
+  return b200dd_detjson_fetch(h->dj, timestamp, out, cap, n_bytes, st);
+}
+
+int b200dd_pipeline_fetch_detection_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_detection_stash: null argument");
+  if (!h->dj) return arg_fail("b200dd_pipeline_fetch_detection_stash: the detection JSON stage is not enabled");
+  DeviceGuard guard(h->device);
+  return b200dd_detjson_fetch_stash(h->dj, out, cap, n_bytes, h->dj_stream ? h->dj_stream : (void *)h->stream);
 }
 
 int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out,

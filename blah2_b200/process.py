@@ -591,6 +591,68 @@ class MaxHold:
             pass
 
 
+class DetectionJson:
+    """The detection document of blah2.cpp:312-317 and the API's /stash/detection history (api/stash/detection.js)
+    of up to ``max_held`` detections.  ``render_device`` renders a device detection list (float64 tensors, the count
+    in a uint32 / int32 device word); ``fetch`` writes its document and commits it to the history;
+    ``fetch_stash`` writes the history.  ``render_host`` needs no handle and no device.  Raises B200ddError with code
+    ERR_NONFINITE for a value without JSON text, ERR_CAPACITY for more than 2^18 detections or an overflowed history
+    (see include/b200dd.h)."""
+
+    def __init__(self, fs, max_held=1 << 20, device=-1):
+        lib = capi.load()
+        h = C.c_void_p()
+        capi.check(lib.b200dd_detjson_create(int(fs), int(max_held), int(device), C.byref(h)))
+        self._lib, self._h = lib, h
+        self.fs = int(fs)
+        self.max_bytes = int(lib.b200dd_detjson_max_bytes(h))
+        self.stash_max_bytes = int(lib.b200dd_detjson_stash_max_bytes(h))
+        self._out = np.empty(self.max_bytes, dtype=np.uint8)
+        self._stash = np.empty(self.stash_max_bytes, dtype=np.uint8)
+
+    def render_device(self, d_delay, d_doppler, d_snr, d_count, stream=None):
+        """Asynchronous: the three lists are float64 device tensors, d_count a one-word device tensor."""
+        capi.check(self._lib.b200dd_detjson_render_device(self._h, capi.ptr(d_delay), capi.ptr(d_doppler),
+                                                          capi.ptr(d_snr), capi.ptr(d_count),
+                                                          capi.ptr(stream) if stream else None))
+
+    def fetch(self, timestamp, stream=None) -> bytes:
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_detjson_fetch(self._h, int(timestamp), capi.ptr(self._out), self._out.size,
+                                                  C.byref(n), capi.ptr(stream) if stream else None))
+        return self._out[:n.value].tobytes()
+
+    def fetch_stash(self, stream=None) -> bytes:
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_detjson_fetch_stash(self._h, capi.ptr(self._stash), self._stash.size, C.byref(n),
+                                                        capi.ptr(stream) if stream else None))
+        return self._stash[:n.value].tobytes()
+
+    @staticmethod
+    def render_host(delay, doppler, snr, timestamp, fs) -> bytes:
+        """Detection::delay_bin_to_km(Detection::to_json(timestamp), fs) of host lists, on the CPU."""
+        lib = capi.load()
+        v = [np.ascontiguousarray(np.asarray(a, dtype=np.float64).ravel()) for a in (delay, doppler, snr)]
+        if not v[0].size == v[1].size == v[2].size:
+            raise ValueError("delay, doppler and snr differ in length")
+        out = np.empty(80 + 75 * v[0].size, dtype=np.uint8)
+        n = C.c_size_t()
+        capi.check(lib.b200dd_detjson_render_host(capi.ptr(v[0]), capi.ptr(v[1]), capi.ptr(v[2]), v[0].size,
+                                                  int(timestamp), int(fs), capi.ptr(out), out.size, C.byref(n)))
+        return out[:n.value].tobytes()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.b200dd_detjson_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Pipeline:
     """One CPI through the body of the reference's process thread (src/blah2.cpp:268-287):
     [WienerHopf] -> Ambiguity -> Map::set_metrics -> [CfarDetector1D -> Centroid -> Interpolate],
@@ -598,7 +660,7 @@ class Pipeline:
 
     def __init__(self, delayMin, delayMax, dopplerMin, dopplerMax, fs, nSamples, roundHamming=True, clutter=None,
                  detection=None, device=-1, max_detections=4096, spectrum_bandwidth=None, map_json=False,
-                 maxhold=False):
+                 maxhold=False, detection_json=False, max_held_detections=1 << 20):
         lib = capi.load()
         p = capi.PipelineParams()
         p.caf = capi.CafParams(int(delayMin), int(delayMax), int(dopplerMin), int(dopplerMax), int(fs),
@@ -641,6 +703,30 @@ class Pipeline:
             capi.check(lib.b200dd_pipeline_enable_maxhold(h, C.byref(mb)))
             self.maxhold_max_bytes = int(mb.value)
         self._maxhold = np.empty(max(self.maxhold_max_bytes, 1), dtype=np.uint8)
+        self.detection_json_max_bytes = self.detection_stash_max_bytes = 0
+        if detection_json:  # detection->to_json + delay_bin_to_km, blah2.cpp:312-317, and /stash/detection
+            db, sb = C.c_size_t(), C.c_size_t()
+            capi.check(lib.b200dd_pipeline_enable_detection_json(h, int(max_held_detections), C.byref(db),
+                                                                 C.byref(sb)))
+            self.detection_json_max_bytes, self.detection_stash_max_bytes = int(db.value), int(sb.value)
+        self._detjson = np.empty(max(self.detection_json_max_bytes, 1), dtype=np.uint8)
+        self._detstash = np.empty(max(self.detection_stash_max_bytes, 1), dtype=np.uint8)
+
+    def fetch_detection_json(self, timestamp) -> bytes:
+        """The detection document of the last fetched CPI (call after fetch()), committed to the /stash/detection
+        history.  Raises B200ddError with code FILTER_FAILED when that CPI's clutter-filter solve failed (nothing is
+        sent, the history is unchanged), ERR_CAPACITY when CFAR overflowed the list."""
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_fetch_detection_json(self._h, int(timestamp), capi.ptr(self._detjson),
+                                                                  self._detjson.size, C.byref(n)))
+        return self._detjson[:n.value].tobytes()
+
+    def fetch_detection_stash(self) -> bytes:
+        """The /stash/detection document of the documents fetched so far."""
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_fetch_detection_stash(self._h, capi.ptr(self._detstash),
+                                                                   self._detstash.size, C.byref(n)))
+        return self._detstash[:n.value].tobytes()
 
     def fetch_maxhold(self, timestamp) -> bytes:
         """The /stash/map document after the last fetched CPI (call after fetch()).  Raises B200ddError with code

@@ -21,6 +21,9 @@
  *   b200dd_next_hamming   next_hamming, src/process/meta/HammingNumber.h:36
  *   b200dd_mapjson_*    Map::to_json + Map::delay_bin_to_km, src/data/Map.cpp:116-185 (blah2.cpp:303-304)
  *   b200dd_maxhold_*    the API's max-hold stash, api/stash/maxhold.js (served at /stash/map, api/server.js:96-97)
+ *   b200dd_detjson_*    Detection::to_json + Detection::delay_bin_to_km, src/data/Detection.cpp:47-106
+ *                       (blah2.cpp:312-317), and the API's detection stash, api/stash/detection.js (served at
+ *                       /stash/detection, api/server.js:99-100)
  *
  * Data conventions
  *   host IQ      interleaved complex128 (re, im doubles) -- what IqData holds
@@ -67,7 +70,8 @@ extern "C" {
 #define B200DD_ERR_GEOMETRY 2    /* geometry outside the supported range (see DESIGN.md "limits") */
 #define B200DD_ERR_CUDA 3        /* CUDA runtime error; b200dd_last_error() has the text */
 #define B200DD_ERR_CAPACITY 4    /* output capacity too small (detections, map JSON) */
-#define B200DD_ERR_NONFINITE 5   /* map JSON: a value rapidjson cannot write (a map cell with |z| = 0, inf or NaN) */
+#define B200DD_ERR_NONFINITE 5   /* map / detection JSON: a value rapidjson cannot write (a map cell with |z| = 0,
+                                    inf or NaN; a detection that is not finite) */
 #define B200DD_FILTER_FAILED 10  /* WienerHopf: matrix not positive definite -> y left untouched
                                     (reference returns false, WienerHopf.cpp:111-122) */
 
@@ -438,6 +442,64 @@ B200DD_API int b200dd_maxhold_format_doubles_host(const double *v, uint32_t n, c
 B200DD_API int b200dd_maxhold_format_doubles_device(const double *v, uint32_t n, char *out, size_t cap,
                                                     size_t *n_bytes, int32_t device);
 
+/* ------------------------------------------------------------------ detection JSON
+ *
+ * The document blah2 sends on its detection socket for every CPI: the std::string returned by
+ * detection->delay_bin_to_km(detection->to_json(timestamp), fs) (src/blah2.cpp:312-317,
+ * src/data/Detection.cpp:47-106), byte for byte:  {"timestamp":T,"delay":[..],"doppler":[..],"snr":[..]}.
+ * doppler (Hz) and snr (dB) are rapidjson's text at two decimal places read back and written again; delay is
+ * 1.0 * bin * (c / fs) / 1000 km, written once.  An empty list gives "delay":[],"doppler":[],"snr":[].  A value
+ * without JSON text (inf, NaN, or a km value that overflows) makes rapidjson stop mid-document and blah2's re-parse
+ * fail: B200DD_ERR_NONFINITE, nothing written.
+ *
+ * The handle also keeps the API's detection history, /stash/detection (api/stash/detection.js, api/server.js:99-100):
+ * every fetched document enters it with its timestamp; after each one the API drops documents more than 300 s older
+ * than the new one with its own loop, which tests only every other document from the front and removes one from the
+ * front per stale test, so stale documents can stay.  The history is sent as JSON.stringify of
+ * {"timestamp":[..],"delay":[..],"doppler":[..],"snr":[..]}: the detections of the held documents in order, each
+ * with its document's timestamp, every number as Number::toString (see b200dd_maxhold_*); "[]" before the first
+ * document.  Every delay, Doppler and SNR text is k/100 for an integer k, so the history is a device ring of int32
+ * triples holding max_held detections.  Not reproduced: the API loses its first document after start and its 100 ms
+ * polling skips documents that arrive faster; every fetched document is taken here.
+ *
+ * Limits: a value whose hundredths lie outside int32 (|v| >= 21474836.48) cannot enter the history: its fetch writes
+ * the document and returns B200DD_ERR_ARG without committing it.  When committing a document would hold more than
+ * max_held detections, its fetch writes the document and returns B200DD_ERR_CAPACITY, and the history is lost:
+ * b200dd_detjson_fetch_stash returns B200DD_ERR_CAPACITY from then on, for the life of the handle (for a pipeline's
+ * stage, until the stage is enabled again); later documents are still written and return B200DD_OK.
+ * Device memory: about 20 MB for the document, plus max_held * 72 bytes for the history.
+ */
+typedef struct b200dd_detjson b200dd_detjson;
+
+/* fs in Hz (the delay's km scale); max_held in [1, 2^25] detections held by the history. */
+B200DD_API int b200dd_detjson_create(uint32_t fs, uint32_t max_held, int32_t device, b200dd_detjson **out);
+/* Upper bound of a detection document's size in bytes (2^18 detections, every value's text at most 24 bytes). */
+B200DD_API size_t b200dd_detjson_max_bytes(const b200dd_detjson *h);
+/* Upper bound of the /stash/detection document's size in bytes. */
+B200DD_API size_t b200dd_detjson_stash_max_bytes(const b200dd_detjson *h);
+B200DD_API void b200dd_detjson_destroy(b200dd_detjson *h);
+/* Renders the document body of a device detection list: d_delay (bins), d_doppler (Hz), d_snr (dB) doubles whose
+ * length is the device word *d_count, read when the kernels run (at most 2^18 entries are read).  Asynchronous on
+ * `stream` (NULL = the handle's stream); the launch shape does not depend on the count, so the call can be recorded
+ * in a CUDA graph.  Also writes the values' hundredths into the history's ring, where the next commit takes them. */
+B200DD_API int b200dd_detjson_render_device(b200dd_detjson *h, const double *d_delay, const double *d_doppler,
+                                            const double *d_snr, const uint32_t *d_count, void *stream);
+/* Writes the last render's document with `timestamp` into out (*n_bytes = its length), then commits it to the
+ * history and prunes it.  Synchronises `stream` (the render's stream).  Each render is fetched once; B200DD_ERR_ARG
+ * when nothing was rendered since the last fetch.  B200DD_ERR_CAPACITY, nothing written or committed: the count
+ * exceeds 2^18 (*n_bytes = 0), or cap < *n_bytes (the same render may be fetched again).  B200DD_ERR_NONFINITE:
+ * nothing written or committed.  See the limits above for B200DD_ERR_ARG / B200DD_ERR_CAPACITY with the document
+ * written (*n_bytes <= cap). */
+B200DD_API int b200dd_detjson_fetch(b200dd_detjson *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
+                                    void *stream);
+/* Writes the /stash/detection document into out; *n_bytes = its length.  Synchronises `stream`.
+ * B200DD_ERR_CAPACITY: cap < *n_bytes, or the history overflowed. */
+B200DD_API int b200dd_detjson_fetch_stash(b200dd_detjson *h, char *out, size_t cap, size_t *n_bytes, void *stream);
+/* The detection document of n HOST detections, without a handle or a device.  B200DD_ERR_NONFINITE: a value has no
+ * text, nothing written.  B200DD_ERR_CAPACITY: cap < *n_bytes. */
+B200DD_API int b200dd_detjson_render_host(const double *delay, const double *doppler, const double *snr, uint32_t n,
+                                          uint64_t timestamp, uint32_t fs, char *out, size_t cap, size_t *n_bytes);
+
 /* ------------------------------------------------------------------ whole CPI pipeline
  *
  * One coherent-processing interval through the body of the reference's process thread
@@ -534,6 +596,24 @@ B200DD_API int b200dd_pipeline_fetch_map_json(b200dd_pipeline *h, uint64_t times
 B200DD_API int b200dd_pipeline_enable_maxhold(b200dd_pipeline *h, size_t *max_bytes);
 B200DD_API int b200dd_pipeline_fetch_maxhold(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
                                              size_t *n_bytes);
+
+/* Optional last stage (src/blah2.cpp:312-317): renders the detection document (see b200dd_detjson_*) of every CPI
+ * submitted afterwards from the detection list on the device, and keeps the /stash/detection history of up to
+ * max_held detections; works in recorded graphs.  Drops the graphs recorded so far and starts an empty history.
+ * *doc_bytes / *stash_bytes (nullable) = the two documents' size bounds.  B200DD_ERR_ARG when the pipeline has no
+ * detection stage; B200DD_ERR_GEOMETRY when an Interpolate result on the pipeline's axes (delay within one bin of
+ * the delay axis, Doppler within one bin of the Doppler axis) could have hundredths outside int32.  SNR needs no
+ * check: from a float map it lies within about +-1700 dB. */
+B200DD_API int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held, size_t *doc_bytes,
+                                                     size_t *stash_bytes);
+/* Called after b200dd_pipeline_fetch: writes the last CPI's detection document (all its detections, whatever cap
+ * b200dd_pipeline_fetch was given) and commits it to the history, as b200dd_detjson_fetch.  B200DD_FILTER_FAILED,
+ * nothing written or committed, when that CPI's clutter-filter solve failed (blah2.cpp:270-273 skips the CPI);
+ * B200DD_ERR_CAPACITY, nothing written or committed, when CFAR found more detections than the list holds. */
+B200DD_API int b200dd_pipeline_fetch_detection_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
+                                                    size_t *n_bytes);
+/* The /stash/detection document of the pipeline's history (see b200dd_detjson_fetch_stash). */
+B200DD_API int b200dd_pipeline_fetch_detection_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes);
 
 /* ------------------------------------------------------------------------------------------------
  * Inter-GPU exchanges (one process per GPU, NCCL over NVLink / NVSwitch).  The reference has no
