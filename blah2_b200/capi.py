@@ -69,6 +69,11 @@ class WhPlan(C.Structure):
                 ("filter_blocks", C.c_uint32)]
 
 
+class TrackerParams(C.Structure):
+    _fields_ = [("m", C.c_uint32), ("n", C.c_uint32), ("n_delete", C.c_uint32), ("cpi", C.c_double),
+                ("max_acc_init", C.c_double), ("fs", C.c_uint32), ("fc", C.c_uint32)]
+
+
 class CpiResult(C.Structure):
     _fields_ = [("filter_status", C.c_int32), ("n_detections", C.c_uint32), ("noise_power", C.c_double),
                 ("max_power", C.c_double)]
@@ -161,6 +166,9 @@ SIGNATURES = [
                                                         C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_detection_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_detection_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_enable_tracker", C.c_int, [_VP, C.POINTER(TrackerParams), C.c_uint32, C.c_uint32,
+                                                 C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_track_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),
     ("b200dd_mapjson_destroy", None, [_VP]),
@@ -189,6 +197,16 @@ SIGNATURES = [
     ("b200dd_detjson_fetch_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
     ("b200dd_detjson_render_host", C.c_int, [_VP, _VP, _VP, C.c_uint32, C.c_uint64, C.c_uint32, _VP, C.c_size_t,
                                              C.POINTER(C.c_size_t)]),
+    ("b200dd_tracker_plan", C.c_int, [C.POINTER(TrackerParams), C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32),
+                                      C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    ("b200dd_tracker_create", C.c_int, [C.POINTER(TrackerParams), C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
+    ("b200dd_tracker_destroy", None, [_VP]),
+    ("b200dd_tracker_reset", C.c_int, [_VP]),
+    ("b200dd_tracker_max_bytes", C.c_size_t, [_VP]),
+    ("b200dd_tracker_process_device", C.c_int, [_VP, _VP, _VP, _VP, _VP, C.c_uint64, _VP]),
+    ("b200dd_tracker_process_host", C.c_int, [_VP, _VP, _VP, _VP, C.c_uint32, C.c_uint64, _VP]),
+    ("b200dd_tracker_fetch", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
+    ("b200dd_tracker_format_doubles_host", C.c_int, [_VP, C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_comm_get_unique_id", C.c_int, [_VP]),
     ("b200dd_comm_create", C.c_int, [C.c_int32, C.c_int32, _VP, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_comm_destroy", None, [_VP]),
@@ -300,6 +318,27 @@ def format_maxhold_doubles(values, device=None) -> list:
         check(lib.b200dd_maxhold_format_doubles_host(ptr(v), v.size, ptr(out), out.size, C.byref(n)))
     else:
         check(lib.b200dd_maxhold_format_doubles_device(ptr(v), v.size, ptr(out), out.size, C.byref(n), int(device)))
+    return out[:n.value].tobytes().decode("ascii").split(",") if v.size else []
+
+
+def tracker_plan(m, n, nDelete, cpi, maxAcc, fs, fc, max_tracks=1 << 16, max_history=64):
+    """Host-only: (hypotheses per unassociated detection, document size bound, device bytes of the track state)."""
+    lib = load()
+    p = TrackerParams(int(m), int(n), int(nDelete), float(cpi), float(maxAcc), int(fs), int(fc))
+    nh, mb, db = C.c_uint32(), C.c_size_t(), C.c_size_t()
+    check(lib.b200dd_tracker_plan(C.byref(p), int(max_tracks), int(max_history), C.byref(nh), C.byref(mb),
+                                  C.byref(db)))
+    return int(nh.value), int(mb.value), int(db.value)
+
+
+def format_track_doubles(values) -> list:
+    """The text the track document gives each double (Writer::Double at two decimal places, written once), on the
+    host; "" for a non-finite value."""
+    lib = load()
+    v = np.ascontiguousarray(np.asarray(values, dtype=np.float64).ravel())
+    n = C.c_size_t()
+    out = np.empty(v.size * 25 + 1, dtype=np.uint8)
+    check(lib.b200dd_tracker_format_doubles_host(ptr(v), v.size, ptr(out), out.size, C.byref(n)))
     return out[:n.value].tobytes().decode("ascii").split(",") if v.size else []
 
 

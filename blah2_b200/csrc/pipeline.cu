@@ -1,6 +1,6 @@
 // pipeline.cu -- one CPI through WienerHopf -> Ambiguity -> set_metrics -> detection with all
 // intermediates resident in HBM (the body of the reference's process thread, src/blah2.cpp:268-287).
-// Composes the per-class handles of caf.cu / wh.cu / det.cu / mapjson.cu / maxhold.cu / detjson.cu through their C ABI; the only kernels
+// Composes the per-class handles of caf.cu / wh.cu / det.cu / mapjson.cu / maxhold.cu / detjson.cu / tracker.cu through their C ABI; the only kernels
 // defined here are the complex128 <-> complex64 conversions of the host entry point.
 #include "common.cuh"
 
@@ -58,6 +58,9 @@ struct b200dd_pipeline {
   void *mh_stream = nullptr;        // stream of the last submit, where its push was enqueued
   b200dd_detjson *dj = nullptr;     // optional: the detection document (blah2.cpp:312-317) and its stash
   void *dj_stream = nullptr;        // stream of the last submit, where its document was rendered
+  b200dd_tracker *tr = nullptr;     // optional: the tracker (blah2.cpp:291-296), run at fetch time
+  void *tr_stream = nullptr;        // stream of the last submit
+  bool tr_pending = false;          // the last submit's detections have not been given to the tracker yet
   uint32_t spec_bins = 0, spec_nfft = 0;
   b200dd_caf_geometry g;
   std::vector<int32_t> delay;
@@ -138,6 +141,7 @@ void b200dd_pipeline_destroy(b200dd_pipeline *h) {
     b200dd_mapjson_destroy(h->mj);
     b200dd_maxhold_destroy(h->mh);
     b200dd_detjson_destroy(h->dj);
+    b200dd_tracker_destroy(h->tr);
     free_dev(h->d_yf);
     free_dev(h->d_xd);
     free_dev(h->d_yd);
@@ -166,6 +170,8 @@ void *b200dd_pipeline_stream(b200dd_pipeline *h) { return h ? (void *)h->stream 
 
 // the optional stages after set_metrics, on the map `map` of the CPI just enqueued on `st`
 static int pipeline_enqueue_products(b200dd_pipeline *h, float2 *map, void *st) {
+  h->tr_stream = st;
+  h->tr_pending = true;
   if (h->mj) {
     h->mj_stream = st;
     const int rc = mapjson_enqueue_with_metrics(h->mj, map, det_device_metrics(h->det), (cudaStream_t)st);
@@ -243,6 +249,8 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   h->last_had_filter = h->wh != nullptr;
   h->mj_stream = st;
   h->mh_stream = st;
+  h->tr_stream = st;
+  h->tr_pending = true;
   if (h->dj) {
     h->dj_stream = st;
     detjson_mark_rendered(h->dj, true);
@@ -536,6 +544,56 @@ int b200dd_pipeline_fetch_detection_stash(b200dd_pipeline *h, char *out, size_t 
   if (!h->dj) return arg_fail("b200dd_pipeline_fetch_detection_stash: the detection JSON stage is not enabled");
   DeviceGuard guard(h->device);
   return b200dd_detjson_fetch_stash(h->dj, out, cap, n_bytes, h->dj_stream ? h->dj_stream : (void *)h->stream);
+}
+
+int b200dd_pipeline_enable_tracker(b200dd_pipeline *h, const b200dd_tracker_params *params, uint32_t max_tracks,
+                                   uint32_t max_history, size_t *max_bytes) {
+  if (!h || !params) return arg_fail("b200dd_pipeline_enable_tracker: null argument");
+  if (!h->p.detection_enable) return arg_fail("b200dd_pipeline_enable_tracker: detection is not enabled");
+  b200dd_tracker_params tp = *params;
+  tp.cpi = h->g.cpi;  // ambiguity->get_cpi(), blah2.cpp:195
+  tp.fs = h->p.caf.fs;
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  b200dd_tracker_destroy(h->tr);
+  h->tr = nullptr;
+  h->tr_stream = nullptr;
+  h->tr_pending = false;
+  const int rc = b200dd_tracker_create(&tp, max_tracks, max_history, h->device, &h->tr);
+  if (rc != B200DD_OK) return rc;
+  if (max_bytes) *max_bytes = b200dd_tracker_max_bytes(h->tr);
+  return B200DD_OK;
+}
+
+int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_track_json: null argument");
+  if (!h->tr) return arg_fail("b200dd_pipeline_fetch_track_json: the tracker stage is not enabled");
+  if (!h->tr_stream) return arg_fail("b200dd_pipeline_fetch_track_json: no CPI submitted since the stage was enabled");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = (cudaStream_t)h->tr_stream;
+  if (h->tr_pending) {
+    DetDeviceList l;
+    int rc = det_device_list(h->det, &l);
+    if (rc != B200DD_OK) return rc;
+    int fs = 0;
+    uint32_t cfar = 0;
+    if (h->last_had_filter) B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(&cfar, l.cfar_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaStreamSynchronize(st));
+    if (fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273): the tracker does not run
+      set_last_error("b200dd_pipeline_fetch_track_json: the CPI's clutter-filter solve failed; the tracker skips it");
+      return B200DD_FILTER_FAILED;
+    }
+    if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
+      set_last_error("b200dd_pipeline_fetch_track_json: more CFAR detections than the list capacity (2^18)");
+      return B200DD_ERR_CAPACITY;
+    }
+    rc = b200dd_tracker_process_device(h->tr, l.delay, l.doppler, l.snr, l.count, timestamp, st);
+    if (rc != B200DD_OK) return rc;
+    h->tr_pending = false;
+  }
+  return b200dd_tracker_fetch(h->tr, timestamp, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out,

@@ -653,6 +653,71 @@ class DetectionJson:
             pass
 
 
+def _fetch_growing(buf, call):
+    """call(buf) -> (rc, n_bytes); a too-small buffer is grown to the reported size and the call repeated."""
+    rc, n = call(buf)
+    if rc == capi.ERR_CAPACITY and n > buf.size:
+        buf = np.empty(n, dtype=np.uint8)
+        rc, n = call(buf)
+    capi.check(rc)
+    return buf, buf[:n].tobytes()
+
+
+class Tracker:
+    """blah2's Tracker (src/process/tracker/Tracker.cpp) with its tracks on the device, named like the reference's
+    constructor Tracker(m, n, nDelete, cpi, maxAccInit, rangeRes, lambda) with rangeRes = c / fs and lambda = c / fc
+    given as fs and fc (blah2.cpp:193-195).  ``process_device`` / ``process_host`` run Tracker::process on one CPI's
+    detections; ``fetch`` returns Track::to_json(timestamp).  ``max_tracks`` and ``max_history`` bound the state: past
+    them fetch raises ERR_CAPACITY until ``reset``.  A non-finite track value raises ERR_NONFINITE at fetch."""
+
+    def __init__(self, m, n, nDelete, cpi, maxAcc, fs, fc, max_tracks=1 << 16, max_history=64, device=-1):
+        lib = capi.load()
+        self.params = capi.TrackerParams(int(m), int(n), int(nDelete), float(cpi), float(maxAcc), int(fs), int(fc))
+        h = C.c_void_p()
+        capi.check(lib.b200dd_tracker_create(C.byref(self.params), int(max_tracks), int(max_history), int(device),
+                                             C.byref(h)))
+        self._lib, self._h = lib, h
+        self.max_bytes = int(lib.b200dd_tracker_max_bytes(h))
+        self._out = np.empty(1 << 16, dtype=np.uint8)
+
+    def process_device(self, d_delay, d_doppler, d_snr, d_count, timestamp, stream=None):
+        """Asynchronous: the lists are float64 device tensors, d_count a one-word device tensor."""
+        capi.check(self._lib.b200dd_tracker_process_device(self._h, capi.ptr(d_delay), capi.ptr(d_doppler),
+                                                           capi.ptr(d_snr), capi.ptr(d_count), int(timestamp),
+                                                           capi.ptr(stream) if stream else None))
+
+    def process_host(self, delay, doppler, snr, timestamp, stream=None):
+        v = [np.ascontiguousarray(np.asarray(a, dtype=np.float64).ravel()) for a in (delay, doppler, snr)]
+        if not v[0].size == v[1].size == v[2].size:
+            raise ValueError("delay, doppler and snr differ in length")
+        capi.check(self._lib.b200dd_tracker_process_host(self._h, capi.ptr(v[0]), capi.ptr(v[1]), capi.ptr(v[2]),
+                                                         v[0].size, int(timestamp),
+                                                         capi.ptr(stream) if stream else None))
+
+    def fetch(self, timestamp, stream=None) -> bytes:
+        def call(buf):
+            n = C.c_size_t()
+            rc = self._lib.b200dd_tracker_fetch(self._h, int(timestamp), capi.ptr(buf), buf.size, C.byref(n),
+                                                capi.ptr(stream) if stream else None)
+            return rc, n.value
+        self._out, doc = _fetch_growing(self._out, call)
+        return doc
+
+    def reset(self):
+        capi.check(self._lib.b200dd_tracker_reset(self._h))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.b200dd_tracker_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Pipeline:
     """One CPI through the body of the reference's process thread (src/blah2.cpp:268-287):
     [WienerHopf] -> Ambiguity -> Map::set_metrics -> [CfarDetector1D -> Centroid -> Interpolate],
@@ -660,7 +725,8 @@ class Pipeline:
 
     def __init__(self, delayMin, delayMax, dopplerMin, dopplerMax, fs, nSamples, roundHamming=True, clutter=None,
                  detection=None, device=-1, max_detections=4096, spectrum_bandwidth=None, map_json=False,
-                 maxhold=False, detection_json=False, max_held_detections=1 << 20):
+                 maxhold=False, detection_json=False, max_held_detections=1 << 20, tracker=None, max_tracks=1 << 16,
+                 max_track_history=64):
         lib = capi.load()
         p = capi.PipelineParams()
         p.caf = capi.CafParams(int(delayMin), int(delayMax), int(dopplerMin), int(dopplerMax), int(fs),
@@ -711,6 +777,29 @@ class Pipeline:
             self.detection_json_max_bytes, self.detection_stash_max_bytes = int(db.value), int(sb.value)
         self._detjson = np.empty(max(self.detection_json_max_bytes, 1), dtype=np.uint8)
         self._detstash = np.empty(max(self.detection_stash_max_bytes, 1), dtype=np.uint8)
+        self.track_max_bytes = 0
+        if tracker is not None:  # tracker->process + track->to_json, blah2.cpp:291-296 and :324-328
+            t = tracker
+            tp = capi.TrackerParams(int(t.get("M", 3)), int(t.get("N", 5)), int(t.get("delete", 10)), 0.0,
+                                    float(t.get("maxAcc", 10)), 0, int(t["fc"]))  # cpi, fs: the pipeline's
+            mb = C.c_size_t()
+            capi.check(lib.b200dd_pipeline_enable_tracker(h, C.byref(tp), int(max_tracks), int(max_track_history),
+                                                          C.byref(mb)))
+            self.track_max_bytes = int(mb.value)
+        self._track = np.empty(1 << 16, dtype=np.uint8)
+
+    def fetch_track_json(self, timestamp) -> bytes:
+        """The track document after the last fetched CPI (call after fetch()): the first call per CPI runs the tracker
+        on that CPI's detections with `timestamp`.  Raises B200ddError with code FILTER_FAILED when that CPI's
+        clutter-filter solve failed and ERR_CAPACITY when CFAR overflowed the list (the tracker is unchanged), and
+        ERR_CAPACITY / ERR_NONFINITE as Tracker.fetch."""
+        def call(buf):
+            n = C.c_size_t()
+            rc = self._lib.b200dd_pipeline_fetch_track_json(self._h, int(timestamp), capi.ptr(buf), buf.size,
+                                                            C.byref(n))
+            return rc, n.value
+        self._track, doc = _fetch_growing(self._track, call)
+        return doc
 
     def fetch_detection_json(self, timestamp) -> bytes:
         """The detection document of the last fetched CPI (call after fetch()), committed to the /stash/detection

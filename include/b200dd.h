@@ -24,6 +24,8 @@
  *   b200dd_detjson_*    Detection::to_json + Detection::delay_bin_to_km, src/data/Detection.cpp:47-106
  *                       (blah2.cpp:312-317), and the API's detection stash, api/stash/detection.js (served at
  *                       /stash/detection, api/server.js:99-100)
+ *   b200dd_tracker_*    Tracker::process + Track::to_json, src/process/tracker/Tracker.cpp, src/data/Track.cpp
+ *                       (blah2.cpp:291-296, :324-328)
  *
  * Data conventions
  *   host IQ      interleaved complex128 (re, im doubles) -- what IqData holds
@@ -500,6 +502,67 @@ B200DD_API int b200dd_detjson_fetch_stash(b200dd_detjson *h, char *out, size_t c
 B200DD_API int b200dd_detjson_render_host(const double *delay, const double *doppler, const double *snr, uint32_t n,
                                           uint64_t timestamp, uint32_t fs, char *out, size_t cap, size_t *n_bytes);
 
+/* ------------------------------------------------------------------ tracker
+ *
+ * Tracker::process + Track::to_json (src/process/tracker/Tracker.cpp, src/data/Track.cpp; blah2.cpp:291-296 and
+ * :324-328), with the track state kept on the device between CPIs.  The code is reproduced as written, quirks
+ * included (DESIGN.md §9): association tests every detection against delay 0, Doppler 0 rather than against the
+ * prediction, so one detection -- the first inside |delay| < 1, |Doppler| < 1/cpi -- associates with every track
+ * the CPI reaches; the inactivity counters belong to vector positions, not tracks; each removal skips the next track.
+ * The document is {"timestamp":T,"n":..,"nTentative":..,"nAssociated":..,"nActive":..,"nCoasting":..,"data":[..]},
+ * every double written once at two decimals (delays stay in bins).
+ *
+ * Limits: the reference has none.  max_tracks live tracks and max_history entries per track are create-time limits;
+ * a CPI that would exceed either puts the handle in an overflowed state in which process does nothing and fetch
+ * returns B200DD_ERR_CAPACITY with *n_bytes = 0, until b200dd_tracker_reset.  Inactivity counters are 32-bit.
+ * Device memory: 16 max_history + 4 ceil(max_history / 16) + 52 bytes per track slot, plus the document body
+ * (grown to the largest document fetched so far).
+ */
+typedef struct b200dd_tracker b200dd_tracker;
+
+typedef struct {
+  uint32_t m, n;        /* process.tracker.initiate.M / .N: promote when m of the last n states associate */
+  uint32_t n_delete;    /* process.tracker.delete */
+  double cpi;           /* Ambiguity::get_cpi() (s) */
+  double max_acc_init;  /* process.tracker.initiate.maxAcc (Hz/s) */
+  uint32_t fs, fc;      /* capture.fs, capture.fc (Hz): rangeRes = c / fs, lambda = c / fc */
+} b200dd_tracker_params;
+
+/* Host only.  *n_hypotheses = 2 nAcc + 1, the tracks each unassociated detection starts, nAcc =
+ * (uint16_t)((int)max_acc_init / (1 / (cpi cpi))); *max_bytes = the document size bound; *device_bytes = the device
+ * memory of the track state (all nullable).  B200DD_ERR_ARG when a conversion is undefined ((int)max_acc_init outside
+ * int, the uint16 conversion of a NaN or of a value outside (-1, 65536)), nAcc > 4096, fs or fc of 0, max_tracks
+ * outside [1, 2^24], max_history outside [1, 2^16], or a document bound of 2^32 bytes or more. */
+B200DD_API int b200dd_tracker_plan(const b200dd_tracker_params *params, uint32_t max_tracks, uint32_t max_history,
+                                   uint32_t *n_hypotheses, size_t *max_bytes, size_t *device_bytes);
+B200DD_API int b200dd_tracker_create(const b200dd_tracker_params *params, uint32_t max_tracks, uint32_t max_history,
+                                     int32_t device, b200dd_tracker **out);
+B200DD_API void b200dd_tracker_destroy(b200dd_tracker *h);
+/* Back to the constructed state: no tracks, timestamp 0, id counter 0, counters 0, not overflowed.  Synchronous. */
+B200DD_API int b200dd_tracker_reset(b200dd_tracker *h);
+/* The document size bound of the handle's limits. */
+B200DD_API size_t b200dd_tracker_max_bytes(const b200dd_tracker *h);
+/* Tracker::process(detection, timestamp) on a device detection list: d_delay (bins), d_doppler (Hz) doubles whose
+ * length is the device word *d_count (d_snr is accepted for the Detection's shape; the tracker never reads it).
+ * Asynchronous on `stream` (NULL = the handle's stream): no host synchronisation and no count read on the host. */
+B200DD_API int b200dd_tracker_process_device(b200dd_tracker *h, const double *d_delay, const double *d_doppler,
+                                             const double *d_snr, const uint32_t *d_count, uint64_t timestamp,
+                                             void *stream);
+/* The same on n HOST detections: copies them to the device and runs the same kernels (asynchronous; the host
+ * arrays may be reused on return). */
+B200DD_API int b200dd_tracker_process_host(b200dd_tracker *h, const double *delay, const double *doppler,
+                                           const double *snr, uint32_t n, uint64_t timestamp, void *stream);
+/* Track::to_json(timestamp) of the current tracks into out; *n_bytes = its length.  Synchronises `stream`.  May be
+ * called any number of times.  B200DD_ERR_CAPACITY: cap < *n_bytes (nothing written), or the handle overflowed
+ * (*n_bytes = 0).  B200DD_ERR_NONFINITE: a value the document holds is not finite (rapidjson's Writer stops there;
+ * an association with T = 0 makes one), nothing written; the state has advanced as the reference's does. */
+B200DD_API int b200dd_tracker_fetch(b200dd_tracker *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
+                                    void *stream);
+/* Host only: the text Writer::Double gives each of n doubles at two decimal places (the track document's numbers),
+ * comma-separated, an empty text for a non-finite value.  B200DD_ERR_CAPACITY: cap < *n_bytes. */
+B200DD_API int b200dd_tracker_format_doubles_host(const double *v, uint32_t n, char *out, size_t cap,
+                                                  size_t *n_bytes);
+
 /* ------------------------------------------------------------------ whole CPI pipeline
  *
  * One coherent-processing interval through the body of the reference's process thread
@@ -614,6 +677,20 @@ B200DD_API int b200dd_pipeline_fetch_detection_json(b200dd_pipeline *h, uint64_t
                                                     size_t *n_bytes);
 /* The /stash/detection document of the pipeline's history (see b200dd_detjson_fetch_stash). */
 B200DD_API int b200dd_pipeline_fetch_detection_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes);
+
+/* Optional stage (src/blah2.cpp:291-296, :324-328): a tracker (see b200dd_tracker_*) fed with every CPI's device
+ * detection list.  params->cpi and params->fs are replaced by the pipeline's geometry and CAF params.
+ * B200DD_ERR_ARG when the pipeline has no detection stage (blah2.cpp:206-209 disables the tracker then).  Starts a
+ * fresh tracker; the submitted chain does not change.  *max_bytes (nullable) = the document size bound. */
+B200DD_API int b200dd_pipeline_enable_tracker(b200dd_pipeline *h, const b200dd_tracker_params *params,
+                                              uint32_t max_tracks, uint32_t max_history, size_t *max_bytes);
+/* Called after b200dd_pipeline_fetch: the first call after a submit runs Tracker::process on that CPI's device
+ * detection list with `timestamp`; every call then writes the document, as b200dd_tracker_fetch (a call with a
+ * too-small cap can be repeated).  B200DD_FILTER_FAILED when the CPI's clutter-filter solve failed (blah2.cpp:270-273
+ * skips the CPI) and B200DD_ERR_CAPACITY with *n_bytes = 0 when CFAR found more detections than the list holds:
+ * nothing written, the tracker unchanged. */
+B200DD_API int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
+                                                size_t *n_bytes);
 
 /* ------------------------------------------------------------------------------------------------
  * Inter-GPU exchanges (one process per GPU, NCCL over NVLink / NVSwitch).  The reference has no
