@@ -66,7 +66,9 @@ class SpectrumGeometry(C.Structure):
 class WhPlan(C.Structure):
     _fields_ = [("corr_fft_len", C.c_uint32), ("corr_hop", C.c_uint32), ("corr_segments", C.c_uint32),
                 ("corr_ctas", C.c_uint32), ("filter_fft_len", C.c_uint32), ("filter_hop", C.c_uint32),
-                ("filter_blocks", C.c_uint32)]
+                ("filter_blocks", C.c_uint32), ("corr_lag_blocks", C.c_uint32), ("filter_partitions", C.c_uint32),
+                ("filter_partition_taps", C.c_uint32), ("solve_threads", C.c_uint32),
+                ("solve_rows_per_thread", C.c_uint32)]
 
 
 class TrackerParams(C.Structure):

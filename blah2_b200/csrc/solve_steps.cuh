@@ -167,6 +167,113 @@ B2S_HD bool levinson_row_step(const double2 *slot, const double2 *px, double2 *p
   return false;
 }
 
+// ---- the long solve kernel (wh_solve_long_kernel, 2049-4096 taps): one CTA, EPT CONSECUTIVE rows per thread --------
+// Same fraction-free Schur recursion driving the same Levinson accumulation as wh_solve_kernel, with the generator
+// held in registers: row i = EPT tid + e takes a_{i-1} from its own register e - 1, the thread's first row from the
+// boundary slot its left neighbour published (one slot per thread, ping-ponged by the parity of k).  Shared memory
+// holds the predictor phi (mirrored reads, ping-pong), the innovations r (row e of thread t at rr[e NTS + t]) and the
+// boundary slots: (2 n + EPT NTS + 2 NTS) double2 instead of the 6 n that stop wh_solve_kernel at 2048 rows.
+// A row runs the Schur update in the steps k < i and accumulates x_i in the steps k >= i, so one register holds its
+// generator b_i first and x_i afterwards (`bx`: zeroed in step i - 1, after the row's last Schur update).
+
+// the step scalars every thread forms from the published b_k, r_k and the pivot state (as wh_solve_kernel does)
+struct LongStep {
+  double2 rho, q, g, bs;  // b_k / p_k, r_k / p_k, r_k sigma_k, b_k s_k
+  double ps, pnew;        // p_k s_k, p_{k+1} = s_k (p_k^2 - |b_k|^2)
+};
+struct LongState { double p, inv_p, sc, sigma; };
+
+B2S_HD LongStep long_step_scalars(const LongState &st, double2 b, double2 rk) {
+  LongStep s;
+  s.rho = make_double2(b.x * st.inv_p, b.y * st.inv_p);
+  s.ps = st.p * st.sc;
+  s.bs = make_double2(b.x * st.sc, b.y * st.sc);
+  s.pnew = s.ps * st.p - (s.bs.x * b.x + s.bs.y * b.y);
+  s.q = make_double2(rk.x * st.inv_p, rk.y * st.inv_p);
+  s.g = make_double2(rk.x * st.sigma, rk.y * st.sigma);
+  return s;
+}
+
+// after the rows of step k: the state of step k + 1 (called only when s.pnew > 0)
+B2S_HD void long_state_advance(LongState &st, const LongStep &s) {
+  const double inv_pn = 1.0 / s.pnew;
+  st.sigma = st.sigma * st.sc * st.p * st.p * inv_pn;  // sigma / (1 - |rho|^2)
+  st.p = s.pnew;
+  st.inv_p = inv_pn;
+  st.sc = pow2_scale(s.pnew);
+}
+
+// One thread's rows in step k.  bnd_c / bnd_n: the boundary slots read / written in this step (slot t = a of thread
+// t's last row); pc / pn_: phi read / written; rr: the innovations; pub_b / pub_r: where the owners of rows k + 2 /
+// k + 1 publish b_{k+1} / r_{k+1} for the next step.
+template <int EPT>
+B2S_HD void long_rows_step(int k, int n, int tid, int nts, const LongStep &s, const double2 *bnd_c, double2 *bnd_n,
+                           const double2 *pc, double2 *pn_, double2 *rr, double2 *pub_b, double2 *pub_r,
+                           double2 (&al)[EPT], double2 (&bx)[EPT]) {
+  const int i0 = EPT * tid;
+  // ---- (1) Schur, the thread's rows from the last down: row i reads a_{i-1} before the row below rewrites it
+  if (i0 + EPT - 1 > k && i0 < n) {
+    const double2 left = tid > 0 ? bnd_c[tid - 1] : make_double2(0.0, 0.0);
+#pragma unroll
+    for (int e = EPT - 1; e >= 0; e--) {
+      const int i = i0 + e;
+      if (i > k && i < n) {
+        const double2 at = e > 0 ? al[e > 0 ? e - 1 : 0] : left;
+        const double2 be = bx[e];
+        double2 na, nb;
+        na.x = s.ps * at.x - (s.bs.x * be.x + s.bs.y * be.y);   // s (p at - conj(b) be)
+        na.y = s.ps * at.y - (s.bs.x * be.y - s.bs.y * be.x);
+        nb.x = s.ps * be.x - (s.bs.x * at.x - s.bs.y * at.y);   // s (p be - b at)
+        nb.y = s.ps * be.y - (s.bs.x * at.y + s.bs.y * at.x);
+        if (i == k + 2) *pub_b = nb;
+        double2 r = rr[e * nts + tid];
+        r.x -= al[e].x * s.q.x - al[e].y * s.q.y;               // r_i -= a_i (r_k / p_k)
+        r.y -= al[e].x * s.q.y + al[e].y * s.q.x;
+        rr[e * nts + tid] = r;
+        if (i == k + 1) *pub_r = r;
+        al[e] = na;
+        bx[e] = i == k + 1 ? make_double2(0.0, 0.0) : nb;       // the row's last Schur step: x_i starts at 0
+      }
+    }
+    bnd_n[tid] = al[EPT - 1];
+  }
+  // ---- (2) Levinson: x_i += (r_k sigma) conj(phi[k-i]) (i <= k);  phi'[i] = phi[i] (i <= k) - rho conj(phi[k+1-i]) (i >= 1)
+  if (i0 <= k + 1) {
+#pragma unroll
+    for (int e = 0; e < EPT; e++) {
+      const int i = i0 + e;
+      if (i <= k + 1 && i < n) {
+        const double2 ph_i = (i <= k) ? pc[i] : make_double2(0.0, 0.0);
+        const double2 ph_m = (i >= 1) ? pc[k + 1 - i] : make_double2(0.0, 0.0);
+        if (i <= k) {
+          const double2 ph_x = pc[k - i];
+          bx[e].x += s.g.x * ph_x.x + s.g.y * ph_x.y;
+          bx[e].y += s.g.y * ph_x.x - s.g.x * ph_x.y;
+        }
+        double2 np_;
+        np_.x = ph_i.x - (s.rho.x * ph_m.x + s.rho.y * ph_m.y);
+        np_.y = ph_i.y - (s.rho.y * ph_m.x - s.rho.x * ph_m.y);
+        pn_[i] = np_;
+      }
+    }
+  }
+}
+
+// the last innovation, after step n - 2: x_i += (r_{n-1} sigma_{n-1}) conj(phi[n-1-i])
+template <int EPT>
+B2S_HD void long_rows_finish(int n, int tid, const LongState &st, double2 rk, const double2 *pc, double2 (&bx)[EPT]) {
+  const double2 g = make_double2(rk.x * st.sigma, rk.y * st.sigma);
+#pragma unroll
+  for (int e = 0; e < EPT; e++) {
+    const int i = EPT * tid + e;
+    if (i < n) {
+      const double2 ph_x = pc[n - 1 - i];
+      bx[e].x += g.x * ph_x.x + g.y * ph_x.y;
+      bx[e].y += g.y * ph_x.x - g.x * ph_x.y;
+    }
+  }
+}
+
 }  // namespace solve
 }  // namespace b2
 

@@ -21,6 +21,9 @@
 //   K5  wh_apply_kernel<LOG2M>   W5: y'[i] = ys[i] - sum_{k<nBins, k<=i} w[k] xs[i-k]  (:125-160, a
 //                                LINEAR convolution with zero history) by overlap-save with the
 //                                spectrum of w computed once per CPI.
+// Taps: 1-4096.  Above 2048 the solve is wh_solve_long_kernel; above 3585 (where no FFT length <= 4096 leaves M/8
+// new samples per transform) K3 splits the lags and K5 the weights into two blocks on the M = 4096 core
+// (wh_corr_kernel<12, T, true>, wh_apply_part_kernel).
 //
 // Why FP64: the solve amplifies correlation error by cond(A) and the filter output is a small
 // difference of large numbers (30-60 dB of cancellation); SURVEY.md s7 "hard part 3".  Products of
@@ -46,7 +49,10 @@ using namespace b2::solve;
 
 namespace {
 
-constexpr int kMaxBins = 2048;
+constexpr int kMaxBins = 4096;          // filter taps
+constexpr int kMaxBinsOneSweep = 2048;  // the solve kernels with their generator in shared memory (wh_solve_kernel and smaller)
+constexpr int kLongEpt = 4;             // rows per thread of wh_solve_long_kernel (1024 threads)
+constexpr int kPartLog2M = 12;          // FFT length of the lag-block correlations and the partitioned filter
 
 // xs[i] = x[map(i)] reproduces the reference's (((i - delayMin) % N) + N) % N evaluated in uint32
 // arithmetic (WienerHopf.cpp:67) EXACTLY, with no division and no branch on the load path (the first
@@ -98,6 +104,7 @@ struct CorrArgs {
   long long xLo, xHi, yLo, yHi;  // readable element ranges of x / y relative to the pointers above
   XsMap xs;
   int nBins, L, nSegTotal, segPerCta;
+  int lagBlk;  // lag-block kernels: lags per block (block blockIdx.y covers [blockIdx.y lagBlk, + lagBlk) of [0, nBins))
 };
 
 // Variant of dit::transform for kernels at the 128-register bound (two CTAs per SM): the two twiddle bases are
@@ -118,6 +125,7 @@ __device__ __forceinline__ void dit_transform_ld(double2 *A, const double2 *__re
 // elements are loaded directly at the point of use.
 template <class TIN> struct WinDesc {
   const TIN *p;
+  uint32_t base;  // circular index of element 0 before the reference's index map
   uint32_t start, N;
   int lim;
   bool contiguous;
@@ -132,7 +140,10 @@ template <int LOG2M> struct CorrStage { static constexpr int kElems = 15 * dit::
 // cross-spectra W conj(P) and V conj(P) are accumulated over the CTA's segments (shared memory, each thread its
 // own 16 bins), one inverse transform per correlation at the end.  float2 input: the next window is staged into
 // shared memory by a TMA bulk copy while the current one is transformed.
-template <int LOG2M, class TIN>
+// LAGS (above 3585 taps at M = 4096, where one block of lags leaves segments of fewer than M/8 samples): the lag range
+// is split into blocks of at most M/2, one per blockIdx.y; the W and V windows of a block start lag0 samples later and
+// hold len + lagBlk - 1 samples, the segment transform P is recomputed per block.
+template <int LOG2M, class TIN, bool LAGS = false>
 __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrArgs a) {
   using P = dit::Plan3<LOG2M>;
   constexpr int NT = P::NT;
@@ -162,28 +173,37 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
   const int s1 = min(s0 + a.segPerCta, a.nSegTotal);
   const XsMap xs = a.xs;
   const uint32_t N = a.N;
+  const int lag0 = LAGS ? (int)blockIdx.y * a.lagBlk : 0;              // first lag of this CTA
+  const int nLag = LAGS ? min(a.lagBlk, a.nBins - lag0) : a.nBins;     // lags of this CTA
   // window t (0: P, 1: W, 2: V) of segment s
   auto describe = [&](int s, int t) {
     WinDesc<TIN> d;
     const uint32_t n0 = a.nBegin + (uint32_t)s * (uint32_t)a.L;
     const int len = (int)min((uint32_t)a.L, a.nEnd - n0);
     d.N = N;
-    d.lim = t == 0 ? len : len + a.nBins - 1;
+    d.lim = t == 0 ? len : len + nLag - 1;
+    d.base = n0;
+    if constexpr (LAGS) {
+      if (t > 0) {
+        d.base = n0 + (uint32_t)lag0;
+        d.base = d.base >= N ? d.base - N : d.base;
+      }
+    }
     if (t < 2) {
       d.p = x;
-      d.start = xs(n0);
+      d.start = xs(d.base);
       // the shifted reference is a pure rotation of x only for delayMin <= 0 (thr == 0)
       d.contiguous = xs.thr == 0 && (uint64_t)d.start + (uint64_t)d.lim <= (uint64_t)N;
     } else {
       d.p = y;
-      d.start = n0;
-      d.contiguous = (uint64_t)n0 + (uint64_t)d.lim <= (uint64_t)N;
+      d.start = d.base;
+      d.contiguous = (uint64_t)d.base + (uint64_t)d.lim <= (uint64_t)N;
     }
     return d;
   };
   // element m of window d, t < 2 through the reference's index map when the window is not a plain run
-  auto direct = [&](const WinDesc<TIN> &d, int t, uint32_t n0, int m) {
-    uint32_t i = n0 + (uint32_t)min(m, d.lim - 1);
+  auto direct = [&](const WinDesc<TIN> &d, int t, int m) {
+    uint32_t i = d.base + (uint32_t)min(m, d.lim - 1);
     i = i >= N ? i - N : i;
     return d.p[t < 2 ? xs(i) : i];
   };
@@ -203,14 +223,13 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
     if constexpr (kStage) {
       if (tid == 0) tma::issue(stage_window(d), S, mbar);
     }
-    r15 = direct(d, 0, a.nBegin + (uint32_t)s0 * (uint32_t)a.L, tid + 15 * NT);
+    r15 = direct(d, 0, tid + 15 * NT);
   }
   double2 vxp[16];
   double2 za[16];  // a-spectrum accumulator: registers (the b-spectrum's lives in shared memory)
 #pragma unroll
   for (int q = 0; q < 16; q++) za[q] = zero;
   for (int s = s0; s < s1; s++) {
-    const uint32_t n0 = a.nBegin + (uint32_t)s * (uint32_t)a.L;
     // NOT unrolled: three (five with the inverses) copies of the transform overflow the instruction cache
 #pragma unroll 1
     for (int t = 0; t < 3; t++) {
@@ -235,7 +254,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
       }
       if (!staged) {
 #pragma unroll
-        for (int k = 0; k < 15; k++) put(k, direct(d, t, n0, tid + NT * k));
+        for (int k = 0; k < 15; k++) put(k, direct(d, t, tid + NT * k));
       }
       put(15, r15);
       // next window (of this or the next segment): staged while this one is transformed
@@ -247,7 +266,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
           if constexpr (kStage) {
             if (tid == 0) tma::issue(stage_window(dn), S, mbar);
           }
-          r15 = direct(dn, nt, a.nBegin + (uint32_t)ns * (uint32_t)a.L, tid + 15 * NT);
+          r15 = direct(dn, nt, tid + 15 * NT);
         }
       });
       if (t == 0) {
@@ -268,7 +287,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
     }
   }
   const double scale = 1.0 / (double)P::M;
-  double2 *pa = a.partial + (size_t)blockIdx.x * 2 * a.nBins;
+  double2 *pa = a.partial + (size_t)blockIdx.x * 2 * a.nBins + lag0;
   double2 *pb = pa + a.nBins;
   // IFFT gives ra[k] = sum xs[n+k] conj(xs[n]);  a[k] = conj(ra[k])  (WienerHopf.cpp:82-84); b[k] = rb[k]
 #pragma unroll 1
@@ -283,7 +302,7 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_corr_kernel(CorrA
 #pragma unroll
     for (int q = 0; q < 16; q++) {
       const int m = tid + NT * q;
-      if (m < a.nBins) out[m] = make_double2(z[brev<16>(q)].x * scale, z[brev<16>(q)].y * sgn);
+      if (m < nLag) out[m] = make_double2(z[brev<16>(q)].x * scale, z[brev<16>(q)].y * sgn);
     }
     __syncthreads();
   }
@@ -907,6 +926,89 @@ __global__ void __launch_bounds__(1024, 1) wh_solve_split_kernel(SolveArgs s) {
   if (i == 0) *s.status = fine ? 0 : 1;
 }
 
+// ---- long variant (2049-4096 taps; solve_steps.cuh, long_rows_step) ------------------------------------------------
+// wh_solve_kernel<2> stops at 2048 rows (1024 threads x 2) and its 6 n double2 of shared memory pass 227 KB above
+// ~2418 rows.  Here each thread holds EPT = 4 CONSECUTIVE rows and the generator lives in registers: the neighbour
+// shift a_{i-1} -> a_i stays inside a thread except at its first row, which reads the boundary slot of the thread to
+// its left.  Shared memory: phi ping-pong (2 n) + innovations (4 threads) + boundary slots (2 threads) double2,
+// 224 KB at 4096 taps.  Same recursion, same failure verdict and the same fixed-order reduction of the partial
+// correlations as wh_solve_kernel; one __syncthreads per step.
+template <int EPT> __global__ void __launch_bounds__(1024, 1) wh_solve_long_kernel(SolveArgs s) {
+  extern __shared__ __align__(16) double2 sm[];
+  const int n = s.nBins, tid = threadIdx.x, NTS = blockDim.x;
+  double2 *phb0 = sm, *phb1 = sm + n;                 // predictor phi, ping-pong (mirrored access)
+  double2 *rrs = sm + 2 * n;                          // innovations, row EPT t + e at rrs[e NTS + t]
+  double2 *bnd0 = rrs + EPT * NTS, *bnd1 = bnd0 + NTS;  // boundary slots, ping-pong
+  double2 *pub_b = bnd1 + NTS, *pub_r = pub_b + 2;    // b_k / r_k of parity k & 1
+  __shared__ double s_t0;
+  const double2 zero = make_double2(0.0, 0.0);
+  // fixed-order reduction of the per-CTA partial correlations (deterministic), coalesced, staged through phi's buffers
+  for (int i = tid; i < n; i += NTS) {
+    double2 sa = zero, sb = zero;
+    for (int p = 0; p < s.nPartial; p++) {
+      const double2 va = s.partial[((size_t)p * 2) * n + i];
+      const double2 vb = s.partial[((size_t)p * 2 + 1) * n + i];
+      sa.x += va.x; sa.y += va.y;
+      sb.x += vb.x; sb.y += vb.y;
+    }
+    s.a_out[i] = sa;
+    s.b_out[i] = sb;
+    phb0[i] = sa;
+    phb1[i] = sb;
+    if (i == 0) s_t0 = sa.x;
+  }
+  __syncthreads();
+  const double t0 = s_t0;
+  bool ok = (t0 > 0.0) && isfinite(t0);
+  const double inv_t0 = ok ? 1.0 / t0 : 1.0;
+  double2 al[EPT], bx[EPT];  // generator a_i; b_i, then x_i
+#pragma unroll
+  for (int e = 0; e < EPT; e++) {
+    const int i = EPT * tid + e;
+    al[e] = bx[e] = zero;
+    rrs[e * NTS + tid] = zero;
+    if (i < n) {
+      const double2 sa = phb0[i];
+      al[e] = make_double2(sa.x * inv_t0, -sa.y * inv_t0);  // a_i^(0) = conj(a[i]) / t_0  (p_0 = 1)
+      bx[e] = i ? al[e] : zero;
+      rrs[e * NTS + tid] = phb1[i];
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int e = 0; e < EPT; e++) {
+    const int i = EPT * tid + e;
+    if (i < n) {
+      phb0[i] = make_double2(i == 0 ? 1.0 : 0.0, 0.0);  // phi^(1) = [1], sigma = 1 / t_0
+      phb1[i] = zero;
+      if (i == 0) pub_r[0] = rrs[e * NTS + tid];
+      if (i == 1) pub_b[0] = bx[e];
+    }
+  }
+  bnd0[tid] = al[EPT - 1];
+  __syncthreads();
+  LongState st;
+  st.p = 1.0; st.inv_p = 1.0; st.sc = 1.0; st.sigma = inv_t0;
+  if (ok) {
+    for (int k = 0; k < n - 1; k++) {
+      const int par = k & 1;
+      const LongStep ls = long_step_scalars(st, pub_b[par], pub_r[par]);
+      if (!(ls.pnew > 0.0)) { ok = false; break; }  // uniform: every thread read the same published pivot
+      long_rows_step<EPT>(k, n, tid, NTS, ls, par ? bnd1 : bnd0, par ? bnd0 : bnd1, par ? phb1 : phb0, par ? phb0 : phb1,
+                          rrs, pub_b + (par ^ 1), pub_r + (par ^ 1), al, bx);
+      long_state_advance(st, ls);
+      __syncthreads();
+    }
+  }
+  if (ok) long_rows_finish<EPT>(n, tid, st, pub_r[(n - 1) & 1], ((n - 1) & 1) ? phb1 : phb0, bx);
+#pragma unroll
+  for (int e = 0; e < EPT; e++) {
+    const int i = EPT * tid + e;
+    if (i < n) s.w_out[i] = ok ? bx[e] : zero;
+  }
+  if (tid == 0) *s.status = ok ? 0 : 1;
+}
+
 // ---------------------------------------------------------------------------------
 // spectrum of the zero-padded weights, once per CPI: what[q NT + tid] = W^[tid + NT q] (the order in which the
 // filter kernel's threads hold their spectra: coalesced 16-byte loads)
@@ -945,6 +1047,7 @@ struct ApplyArgs {
   XsMap xs;
   int nBins, Lout, nBlocks;
   int *next_block;  // work queue of the persistent CTAs: first block not yet claimed (reset by wh_wspec_kernel)
+  int parts, partLen;  // partitioned filter (wh_apply_part_kernel): weight partitions, taps per partition
 };
 
 template <class TOUT> __device__ __forceinline__ void st_iq(TOUT *p, uint32_t i, double2 v);
@@ -1096,6 +1199,84 @@ __global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, wh_min_ctas<LOG2M>()) w
   }
 }
 
+// K5 above 3585 taps: UNIFORMLY PARTITIONED overlap-save.  The weights are split into `parts` partitions of partLen
+// <= M/2 taps (wh_wspec_kernel, once per partition: spectrum p at what + p M).  Output block b, Lout = M - partLen + 1
+// outputs from i0 on: for each partition p the window of M shifted-reference samples ending partLen p samples before
+// the block's last output is transformed and its spectrum multiplied by partition p's into an accumulator in
+// registers; one inverse transform per block.  Samples more than nBins - 1 before a block's first output only meet
+// zero-padded taps of the last partition and are masked to zero, so the filter reads exactly the samples K5 reads at
+// fewer taps (chunk halos included).  The accumulator keeps 16 double2 more registers live across the forward
+// transforms than wh_apply_kernel: one CTA per SM is guaranteed, more as the compiled register count allows.  Blocks
+// are walked with a fixed stride; direct loads.  y and y_out may be the same buffer (each element is read, then
+// written, by the same thread).
+template <int LOG2M, class TIN>
+__global__ void __launch_bounds__(dit::Plan3<LOG2M>::NT, 1) wh_apply_part_kernel(ApplyArgs a) {
+  using P = dit::Plan3<LOG2M>;
+  constexpr int NT = P::NT;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  double2 *A = reinterpret_cast<double2 *>(smem_raw);
+  const int tid = threadIdx.x;
+  const TIN *__restrict__ x = reinterpret_cast<const TIN *>(a.x);
+  const TIN *y = reinterpret_cast<const TIN *>(a.y);
+  TIN *yo = reinterpret_cast<TIN *>(a.y_out);
+  const int hist = a.partLen - 1;
+  if (*a.status != 0) {  // failed solve: surveillance channel passes through untouched
+    for (int b = blockIdx.x; b < a.nBlocks; b += gridDim.x) {
+      const uint32_t i0 = a.iBegin + (uint32_t)b * (uint32_t)a.Lout;
+      const int nOut = (int)min((uint32_t)a.Lout, a.iEnd - i0);
+      for (int m = tid; m < nOut; m += NT) st_iq<TIN>(yo, i0 + m, ld_iq(y, i0 + m));
+    }
+    return;
+  }
+  const XsMap xs = a.xs;
+  const dit::TwPair<double> tw = dit::load_twiddles<double, LOG2M>(a.tw, tid);
+  for (int b = blockIdx.x; b < a.nBlocks; b += gridDim.x) {
+    const uint32_t i0 = a.iBegin + (uint32_t)b * (uint32_t)a.Lout;
+    const int nOut = (int)min((uint32_t)a.Lout, a.iEnd - i0);
+    const int64_t reach = (int64_t)i0 - (a.nBins - 1);  // the first sample any output of this block needs
+    double2 z[16];
+#pragma unroll
+    for (int q = 0; q < 16; q++) z[q] = make_double2(0.0, 0.0);
+#pragma unroll 1
+    for (int p = 0; p < a.parts; p++) {
+      double2 v[16];
+      const int64_t first = (int64_t)i0 - (int64_t)p * a.partLen - hist;
+#pragma unroll
+      for (int k = 0; k < 16; k++) {
+        const int m = tid + NT * k;
+        const int64_t i = first + m;
+        const bool ok = i >= 0 && i >= reach && i < (int64_t)a.N && m < hist + nOut;
+        const int64_t ic = i < 0 ? 0 : (i >= (int64_t)a.N ? (int64_t)a.N - 1 : i);
+        const long long xi = (long long)xs((uint32_t)ic);
+        const TIN e = x[xi < a.xLo ? a.xLo : (xi >= a.xHi ? a.xHi - 1 : xi)];  // (masked elements only; keeps the address readable)
+        v[k] = make_double2(ok ? (double)e.x : 0.0, ok ? (double)e.y : 0.0);
+      }
+      dit::transform<double, LOG2M, -1>(A, tw, tid, v);
+      const double2 *wp = a.what + (size_t)p * P::M;
+#pragma unroll
+      for (int q = 0; q < 16; q++) {
+        const double2 t = cmul(v[brev<16>(q)], ld_keep(wp + q * NT + tid));
+        z[q].x += t.x;
+        z[q].y += t.y;
+      }
+      __syncthreads();
+    }
+    dit::transform<double, LOG2M, +1>(A, tw, tid, z);
+    const double scale = 1.0 / (double)P::M;
+    // conv[m] valid for m >= hist; output i = i0 + m - hist
+#pragma unroll
+    for (int q = 0; q < 16; q++) {
+      const int o = tid + NT * q - hist;
+      if (o >= 0 && o < nOut) {
+        const double2 cv = z[brev<16>(q)];
+        const TIN yy = ld_stream(y + i0 + o);
+        st_iq<TIN>(yo, i0 + o, make_double2((double)yy.x - cv.x * scale, (double)yy.y - cv.y * scale));
+      }
+    }
+    __syncthreads();  // the buffer is rewritten by the next block's first pass
+  }
+}
+
 std::vector<double2> twiddle_table_f64(int M) {
   std::vector<double2> t(M);
   const long double two_pi = 6.283185307179586476925286766559005768L;
@@ -1126,8 +1307,12 @@ struct b200dd_wh {
   int log2m_c = 12, log2m_a = 12;  // FFT lengths of the correlation / filter stages
   int L = 0, nSeg = 0, segPerCta = 1, gridCorr = 1;  // correlation stage
   int Lout = 0, gridApply = 1, ctasApply = 1;       // filter stage: blocks, persistent CTAs
+  int lagBlocks = 1, lagBlk = 0;                     // correlation stage above 3585 taps: lag blocks, lags per block
+  int parts = 1, partLen = 0;                        // filter stage above 3585 taps: weight partitions, taps per partition
   void (*solve)(SolveArgs) = nullptr;                // the solve kernel of the tap count
   int solveThreads = 0;
+  size_t solveSmem = 0;
+  int partResident = 1;  // resident CTAs per SM of the partitioned filter kernel
   Span span;
   double2 *d_tw_c = nullptr, *d_tw_a = nullptr, *d_partial = nullptr, *d_a = nullptr, *d_b = nullptr, *d_w = nullptr, *d_what = nullptr;
   int *d_status = nullptr;
@@ -1149,6 +1334,10 @@ template <int LOG2M> size_t corr_smem() {
 }
 template <int LOG2M> size_t fft_smem() { return (size_t)dit::Plan3<LOG2M>::MP * sizeof(double2); }
 // FFT buffer + TMA staging of one window (M + 2 float2) + mbarrier
+// phi ping-pong + innovations + boundary slots + published b / r
+inline size_t long_solve_smem(int nBins, int threads) {
+  return ((size_t)2 * nBins + (size_t)(kLongEpt + 2) * threads + 4) * sizeof(double2);
+}
 template <int LOG2M> size_t apply_smem() { return fft_smem<LOG2M>() + (size_t)(dit::Plan3<LOG2M>::M + 2) * sizeof(float2) + 16; }
 
 // Calls f(std::integral_constant<int, LOG2M>) for the FFT length 2^log2m of a stage (512 .. 4096)
@@ -1168,22 +1357,49 @@ template <int LOG2M, class TIN> int wh_launch_corr(b200dd_wh *h, const void *x, 
   ca.x = x; ca.y = y; ca.partial = h->d_partial; ca.tw = h->d_tw_c;
   ca.N = s.N; ca.nBegin = s.begin; ca.nEnd = s.end; ca.xs = s.xs;
   ca.xLo = s.xLo; ca.xHi = s.xHi; ca.yLo = s.yLo; ca.yHi = s.yHi;
-  ca.nBins = h->nBins; ca.L = h->L; ca.nSegTotal = h->nSeg; ca.segPerCta = h->segPerCta;
-  wh_corr_kernel<LOG2M, TIN><<<h->gridCorr, dit::Plan3<LOG2M>::NT, corr_smem<LOG2M>(), st>>>(ca);
+  ca.nBins = h->nBins; ca.L = h->L; ca.nSegTotal = h->nSeg; ca.segPerCta = h->segPerCta; ca.lagBlk = h->lagBlk;
+  if (h->lagBlocks > 1) {
+    if constexpr (LOG2M == kPartLog2M) {
+      wh_corr_kernel<LOG2M, TIN, true><<<dim3(h->gridCorr, h->lagBlocks), dit::Plan3<LOG2M>::NT, corr_smem<LOG2M>(), st>>>(ca);
+    } else {
+      return geom_fail("WienerHopf: lag-block correlation plan without M = 4096");
+    }
+  } else {
+    wh_corr_kernel<LOG2M, TIN><<<h->gridCorr, dit::Plan3<LOG2M>::NT, corr_smem<LOG2M>(), st>>>(ca);
+  }
   B2_LAUNCH_CHECK();
   return B200DD_OK;
 }
 
 template <int LOG2M, class TIN> int wh_launch_apply(b200dd_wh *h, const void *x, const void *y, void *y_out, cudaStream_t st) {
   using P = dit::Plan3<LOG2M>;
-  wh_wspec_kernel<LOG2M><<<1, P::NT, fft_smem<LOG2M>(), st>>>(h->d_w, h->nBins, h->d_what, h->d_tw_a, h->d_next_block, h->ctasApply);
-  B2_LAUNCH_CHECK();
+  if (h->parts > 1) {  // one weight spectrum per partition
+    for (int p = 0; p < h->parts; p++) {
+      const int t0 = p * h->partLen;
+      wh_wspec_kernel<LOG2M><<<1, P::NT, fft_smem<LOG2M>(), st>>>(h->d_w + t0, min(h->partLen, h->nBins - t0),
+                                                                   h->d_what + (size_t)p * P::M, h->d_tw_a,
+                                                                   h->d_next_block, h->ctasApply);
+      B2_LAUNCH_CHECK();
+    }
+  } else {
+    wh_wspec_kernel<LOG2M><<<1, P::NT, fft_smem<LOG2M>(), st>>>(h->d_w, h->nBins, h->d_what, h->d_tw_a, h->d_next_block, h->ctasApply);
+    B2_LAUNCH_CHECK();
+  }
   const Span &s = h->span;
   ApplyArgs aa;
   aa.x = x; aa.y = y; aa.y_out = y_out; aa.what = h->d_what; aa.tw = h->d_tw_a; aa.status = h->d_status;
   aa.N = s.N; aa.iBegin = s.begin; aa.iEnd = s.end; aa.xs = s.xs; aa.xLo = s.xLo; aa.xHi = s.xHi;
   aa.nBins = h->nBins; aa.Lout = h->Lout; aa.nBlocks = h->gridApply; aa.next_block = h->d_next_block;
-  wh_apply_kernel<LOG2M, TIN><<<h->ctasApply, P::NT, apply_smem<LOG2M>(), st>>>(aa);
+  aa.parts = h->parts; aa.partLen = h->partLen;
+  if (h->parts > 1) {
+    if constexpr (LOG2M == kPartLog2M) {
+      wh_apply_part_kernel<LOG2M, TIN><<<h->ctasApply, P::NT, fft_smem<LOG2M>(), st>>>(aa);
+    } else {
+      return geom_fail("WienerHopf: partitioned filter plan without M = 4096");
+    }
+  } else {
+    wh_apply_kernel<LOG2M, TIN><<<h->ctasApply, P::NT, apply_smem<LOG2M>(), st>>>(aa);
+  }
   B2_LAUNCH_CHECK();
   return B200DD_OK;
 }
@@ -1192,7 +1408,7 @@ int wh_launch_solve(b200dd_wh *h, cudaStream_t st) {
   SolveArgs sa;
   sa.partial = h->chunked ? h->d_ab : h->d_partial; sa.nPartial = h->chunked ? 1 : h->gridCorr; sa.nBins = h->nBins;
   sa.a_out = h->d_a; sa.b_out = h->d_b; sa.w_out = h->d_w; sa.status = h->d_status;
-  h->solve<<<1, h->solveThreads, ((size_t)h->nBins * 6 + 16) * sizeof(double2), st>>>(sa);
+  h->solve<<<1, h->solveThreads, h->solveSmem, st>>>(sa);
   B2_LAUNCH_CHECK();
   return B200DD_OK;
 }
@@ -1237,7 +1453,17 @@ int wh_pick_log2m(const b200dd_wh *h, const char *env1, const char *env2, bool f
 void wh_plan(b200dd_wh *h) {
   h->log2m_c = wh_pick_log2m(h, "B200DD_WH_LOG2M", "B200DD_WH_CORR_LOG2M", false);
   h->log2m_a = wh_pick_log2m(h, "B200DD_WH_LOG2M", "B200DD_WH_APPLY_LOG2M", true);
+  // above 3585 taps no single FFT length leaves M/8 new samples per transform: stay on M = 4096 and split the lags
+  // (correlations) and the taps (filter) into blocks of at most M/2
+  constexpr int Mp = 1 << kPartLog2M;
+  if (h->nBins > Mp / 2 && (uint32_t)Mp <= h->N) {
+    const int blocks = (h->nBins + Mp / 2 - 1) / (Mp / 2), per = (h->nBins + blocks - 1) / blocks;
+    if (!h->log2m_c) { h->log2m_c = kPartLog2M; h->lagBlocks = blocks; h->lagBlk = per; }
+    if (!h->log2m_a) { h->log2m_a = kPartLog2M; h->parts = blocks; h->partLen = per; }
+  }
   if (!h->log2m_c || !h->log2m_a) return;
+  if (h->lagBlocks == 1) h->lagBlk = h->nBins;
+  if (h->parts == 1) h->partLen = h->nBins;
   Span &s = h->span;
   if (h->chunked) {
     s.N = 1u << 31; s.begin = h->c0; s.end = h->c0 + h->nc;
@@ -1250,36 +1476,43 @@ void wh_plan(b200dd_wh *h) {
   }
   const uint64_t span = s.end - s.begin;
   const int M = 1 << h->log2m_c;
-  h->L = M - h->nBins + 1;
+  h->L = M - h->lagBlk + 1;
   h->nSeg = (int)((span + h->L - 1) / h->L);
   // CTAs resident at once: shared memory allows 1 (M=4096) or 2 (smaller) per SM
   const size_t smem = (size_t)(M + M / 16 + 2 * M) * sizeof(double2);
   int per_sm = (int)((227 * 1024) / smem);
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 2) per_sm = 2;
-  int slots = h->num_sms * per_sm;
+  int slots = h->num_sms * per_sm / h->lagBlocks;  // the lag blocks of a segment run side by side
   h->segPerCta = (h->nSeg + slots - 1) / slots;
   if (h->segPerCta < 1) h->segPerCta = 1;
   h->gridCorr = (h->nSeg + h->segPerCta - 1) / h->segPerCta;
   const int Ma = 1 << h->log2m_a;
-  h->Lout = Ma - h->nBins + 1;
+  h->Lout = Ma - h->partLen + 1;
   h->gridApply = (int)((span + h->Lout - 1) / h->Lout);
   // persistent filter CTAs: as many as are resident at once (shared memory and the 128-register bound decide)
   h->ctasApply = with_log2m(h->log2m_a, [&](auto l) {
     constexpr int LOG2M = decltype(l)::value;
     int resident = (int)((227 * 1024) / apply_smem<LOG2M>());
     if (resident > wh_min_ctas<LOG2M>()) resident = wh_min_ctas<LOG2M>();
+    if (h->parts > 1) resident = h->partResident;
     if (resident < 1) resident = 1;
     return h->num_sms * resident < h->gridApply ? h->num_sms * resident : h->gridApply;
   });
   // the tap count picks the solve kernel: 1-448 split (includes the reference's 410 taps), 449-480 short<512>,
-  // 481-992 short<1024>, 993-1024 generic<1>, 1025-2048 generic<2>
+  // 481-992 short<1024>, 993-1024 generic<1>, 1025-2048 generic<2>, 2049-4096 long<4>
   const int threads = ((h->nBins + 31) / 32) * 32;
+  h->solveSmem = ((size_t)h->nBins * 6 + 16) * sizeof(double2);
   if (2 * threads + 96 <= 1024) { h->solve = wh_solve_split_kernel; h->solveThreads = 2 * threads + 96; }
   else if (threads + 32 <= 512) { h->solve = wh_solve_short_kernel<512>; h->solveThreads = threads + 32; }
   else if (threads + 32 <= 1024) { h->solve = wh_solve_short_kernel<1024>; h->solveThreads = threads + 32; }
   else if (h->nBins <= 1024) { h->solve = wh_solve_kernel<1>; h->solveThreads = threads; }
-  else { h->solve = wh_solve_kernel<2>; h->solveThreads = 1024; }
+  else if (h->nBins <= kMaxBinsOneSweep) { h->solve = wh_solve_kernel<2>; h->solveThreads = 1024; }
+  else {
+    h->solve = wh_solve_long_kernel<kLongEpt>;
+    h->solveThreads = ((h->nBins + kLongEpt * 32 - 1) / (kLongEpt * 32)) * 32;
+    h->solveSmem = long_solve_smem(h->nBins, h->solveThreads);
+  }
 }
 
 // Shared-memory limits of the kernels the plan launches.  A limit belongs to the function (per device), not to the
@@ -1290,6 +1523,10 @@ int wh_set_smem_limits(const b200dd_wh *h) {
     constexpr int LOG2M = decltype(l)::value;
     B2_CUDA(cudaFuncSetAttribute(wh_corr_kernel<LOG2M, float2>, kLimit, (int)corr_smem<LOG2M>()));
     B2_CUDA(cudaFuncSetAttribute(wh_corr_kernel<LOG2M, double2>, kLimit, (int)corr_smem<LOG2M>()));
+    if constexpr (LOG2M == kPartLog2M) {
+      B2_CUDA(cudaFuncSetAttribute(wh_corr_kernel<LOG2M, float2, true>, kLimit, (int)corr_smem<LOG2M>()));
+      B2_CUDA(cudaFuncSetAttribute(wh_corr_kernel<LOG2M, double2, true>, kLimit, (int)corr_smem<LOG2M>()));
+    }
     return B200DD_OK;
   });
   if (rc != B200DD_OK) return rc;
@@ -1301,7 +1538,14 @@ int wh_set_smem_limits(const b200dd_wh *h) {
     return B200DD_OK;
   });
   if (rc != B200DD_OK) return rc;
-  B2_CUDA(cudaFuncSetAttribute(h->solve, kLimit, (int)(((size_t)kMaxBins * 6 + 16) * sizeof(double2))));
+  if (h->solve == wh_solve_long_kernel<kLongEpt>)
+    B2_CUDA(cudaFuncSetAttribute(h->solve, kLimit, (int)long_solve_smem(kMaxBins, 1024)));
+  else
+    B2_CUDA(cudaFuncSetAttribute(h->solve, kLimit, (int)(((size_t)kMaxBinsOneSweep * 6 + 16) * sizeof(double2))));
+  if (h->parts > 1) {
+    B2_CUDA(cudaFuncSetAttribute(wh_apply_part_kernel<kPartLog2M, float2>, kLimit, (int)fft_smem<kPartLog2M>()));
+    B2_CUDA(cudaFuncSetAttribute(wh_apply_part_kernel<kPartLog2M, double2>, kLimit, (int)fft_smem<kPartLog2M>()));
+  }
   return B200DD_OK;
 }
 
@@ -1331,7 +1575,7 @@ static int wh_create_impl(int32_t delay_min, int32_t delay_max, uint32_t n_sampl
   if (n_samples == 0) return arg_fail("b200dd_wh_create: n_samples must be > 0");
   const int64_t nb = (int64_t)delay_max - (int64_t)delay_min;  // WienerHopf.cpp:12 (no +1)
   if (nb < 1) return geom_fail("b200dd_wh_create: delayMax - delayMin must be >= 1");
-  if (nb > kMaxBins) return geom_fail("b200dd_wh_create: more than 2048 filter taps unsupported");
+  if (nb > kMaxBins) return geom_fail("b200dd_wh_create: more than 4096 filter taps unsupported");
   if ((uint64_t)nb > n_samples) return geom_fail("b200dd_wh_create: more taps than samples");
   b200dd_wh *h = new (std::nothrow) b200dd_wh();
   if (!h) return arg_fail("b200dd_wh_create: out of host memory");
@@ -1359,8 +1603,15 @@ static int wh_create_impl(int32_t delay_min, int32_t delay_max, uint32_t n_sampl
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDeviceProperties", __FILE__, __LINE__));
   h->num_sms = prop.multiProcessorCount;
+  if (h->nBins > 3585) {  // resident CTAs of the partitioned filter: what its compiled register count allows
+    int r = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, wh_apply_part_kernel<kPartLog2M, float2>,
+                                                      dit::Plan3<kPartLog2M>::NT, fft_smem<kPartLog2M>()) != cudaSuccess)
+      return fail(cuda_fail(cudaGetLastError(), "cudaOccupancyMaxActiveBlocksPerMultiprocessor", __FILE__, __LINE__));
+    h->partResident = r < 1 ? 1 : r;
+  }
   wh_plan(h);
-  if (!h->log2m_c || !h->log2m_a) return fail(geom_fail("b200dd_wh_create: no FFT plan (needs nSamples >= 512 and nBins <= 2048)"));
+  if (!h->log2m_c || !h->log2m_a) return fail(geom_fail("b200dd_wh_create: no FFT plan (needs nSamples >= 512, and nSamples >= 4096 above 3585 taps)"));
   auto body = [&]() -> int {
     const int rc = wh_set_smem_limits(h);
     if (rc != B200DD_OK) return rc;
@@ -1375,7 +1626,7 @@ static int wh_create_impl(int32_t delay_min, int32_t delay_max, uint32_t n_sampl
     B2_CUDA(cudaMalloc(&h->d_a, sizeof(double2) * h->nBins));
     B2_CUDA(cudaMalloc(&h->d_b, sizeof(double2) * h->nBins));
     B2_CUDA(cudaMalloc(&h->d_w, sizeof(double2) * h->nBins));
-    B2_CUDA(cudaMalloc(&h->d_what, sizeof(double2) * M));
+    B2_CUDA(cudaMalloc(&h->d_what, sizeof(double2) * M * h->parts));
     B2_CUDA(cudaMalloc(&h->d_status, sizeof(int)));
     B2_CUDA(cudaMemset(h->d_status, 0, sizeof(int)));
     B2_CUDA(cudaMalloc(&h->d_next_block, sizeof(int)));
@@ -1538,6 +1789,11 @@ int b200dd_wh_get_plan(const b200dd_wh *h, b200dd_wh_plan *out) {
   out->filter_fft_len = 1u << h->log2m_a;
   out->filter_hop = (uint32_t)h->Lout;
   out->filter_blocks = (uint32_t)h->gridApply;
+  out->corr_lag_blocks = (uint32_t)h->lagBlocks;
+  out->filter_partitions = (uint32_t)h->parts;
+  out->filter_partition_taps = (uint32_t)h->partLen;
+  out->solve_threads = (uint32_t)h->solveThreads;
+  out->solve_rows_per_thread = h->nBins > kMaxBinsOneSweep ? (uint32_t)kLongEpt : (h->nBins > 1024 ? 2u : 1u);
   return B200DD_OK;
 }
 void *b200dd_wh_stream(b200dd_wh *h) { return h ? (void *)h->stream : nullptr; }

@@ -233,11 +233,17 @@ B200DD_API int b200dd_wh_chunk_corr_device(b200dd_wh *h, const void *d_x_loc, co
 B200DD_API int b200dd_wh_chunk_filter_device(b200dd_wh *h, const void *d_ab, const void *d_x_loc, const void *d_y_loc,
                                              void *d_y_out, void *stream);
 
-/* The FFT plan of the two FFT stages (for measurement: transforms per CPI = 3 corr_segments + 2 corr_ctas in the
- * correlation kernel, 2 filter_blocks + 1 in the filter stage). */
+/* The FFT plan of the two FFT stages (for measurement: transforms per CPI = corr_lag_blocks (3 corr_segments +
+ * 2 corr_ctas) in the correlation kernel, (filter_partitions + 1) filter_blocks + filter_partitions in the filter
+ * stage) and the solve kernel's shape.  Above 3585 taps the correlations split the lags into corr_lag_blocks blocks
+ * and the filter splits the weights into filter_partitions partitions of filter_partition_taps taps (both 1 / nBins
+ * below); the solve runs solve_threads threads of one CTA, solve_rows_per_thread matrix rows each (4 above 2048
+ * taps: the register-resident generator kernel). */
 typedef struct {
   uint32_t corr_fft_len, corr_hop, corr_segments, corr_ctas;
   uint32_t filter_fft_len, filter_hop, filter_blocks;
+  uint32_t corr_lag_blocks, filter_partitions, filter_partition_taps;
+  uint32_t solve_threads, solve_rows_per_thread;
 } b200dd_wh_plan;
 B200DD_API int b200dd_wh_get_plan(const b200dd_wh *h, b200dd_wh_plan *out);
 B200DD_API void *b200dd_wh_stream(b200dd_wh *h);
