@@ -171,6 +171,10 @@ SIGNATURES = [
     ("b200dd_pipeline_enable_tracker", C.c_int, [_VP, C.POINTER(TrackerParams), C.c_uint32, C.c_uint32,
                                                  C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_track_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_enable_iqdata_json", C.c_int, [_VP, C.c_double, C.c_double, C.c_double, C.POINTER(C.c_size_t),
+                                                     C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_iqdata_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_iqdata_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),
     ("b200dd_mapjson_destroy", None, [_VP]),
@@ -199,6 +203,16 @@ SIGNATURES = [
     ("b200dd_detjson_fetch_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
     ("b200dd_detjson_render_host", C.c_int, [_VP, _VP, _VP, C.c_uint32, C.c_uint64, C.c_uint32, _VP, C.c_size_t,
                                              C.POINTER(C.c_size_t)]),
+    ("b200dd_iqjson_create", C.c_int, [C.c_uint32, C.c_double, C.c_double, C.c_double, C.c_int32, C.POINTER(_VP)]),
+    ("b200dd_iqjson_max_bytes", C.c_size_t, [_VP]),
+    ("b200dd_iqjson_stash_max_bytes", C.c_size_t, [_VP]),
+    ("b200dd_iqjson_destroy", None, [_VP]),
+    ("b200dd_iqjson_render_device", C.c_int, [_VP, _VP, _VP]),
+    ("b200dd_iqjson_fetch", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
+    ("b200dd_iqjson_fetch_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),
+    ("b200dd_iqjson_render_host", C.c_int, [_VP, C.c_uint32, C.c_double, C.c_double, C.c_double, C.c_uint64, _VP,
+                                            C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_iqjson_debug_bin_values", C.c_int, [_VP, _VP, _VP, _VP]),
     ("b200dd_tracker_plan", C.c_int, [C.POINTER(TrackerParams), C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32),
                                       C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     ("b200dd_tracker_create", C.c_int, [C.POINTER(TrackerParams), C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(_VP)]),

@@ -87,5 +87,9 @@ void detjson_mark_rendered(b200dd_detjson *h, bool rendered);
 // within one bin of the Doppler axis -- has hundredths outside int32 in the detection document; else
 // B200DD_ERR_GEOMETRY.
 int detjson_check_axes(const int32_t *delay, uint32_t n_del, const double *doppler, uint32_t n_dop, uint32_t fs);
+// spectrum.cu: the handle's own double2[n_spectrum] buffer, where process_device with d_spectrum == NULL writes.
+const void *spectrum_device_output(const b200dd_spectrum *h);
+// iqjson.cu: a render recorded in a graph was replayed (true), or the pipeline dropped the CPI's document (false).
+void iqjson_mark_rendered(b200dd_iqjson *h, bool rendered);
 
 }  // namespace b2

@@ -1,0 +1,509 @@
+// iqjson.cu -- the IQ-data document blah2 sends on its IQ-data socket, and the API's 20-CPI history served at
+// /stash/iqdata, both rendered on the device.
+//
+// blah2 publishes every CPI's spectrum as x->to_json(ts) (src/blah2.cpp:299-300, src/data/IqData.cpp:93-125):
+//   {"timestamp":T,"min":m,"max":M,"mean":u,"frequency":[],"spectrum":[..]}
+// Each spectrum entry is 10 * log10(|s|) of one SpectrumAnalyser bin, written ONCE by Writer::Double at two decimals
+// (jf::fmt_double, no read-back).  frequency is always empty (the analyser's uint32_t loop never runs) and min, max and
+// mean are members nothing in blah2 assigns: here they are constants fixed when the handle is created.  The API
+// (api/stash/iqdata.js) parses every document and keeps the spectrum, frequency and timestamp of the last 20; it
+// serves the newest document with those three members replaced by the arrays,
+//   {"timestamp":[..],"min":m,"max":M,"mean":u,"frequency":[[],..],"spectrum":[[..],..]}
+// each number re-printed by Number::toString.  Every spectrum text is k/100 for an integer k (json_fmt.cuh), so the
+// history is a ring of int32 rows.
+//
+// Per CPI (recordable in a graph: the launch shape depends only on nSpectrum):
+//   ij_len_kernel    formats each bin with its separator (one bin per thread), counts each tile's bytes, and writes
+//                    the bin's hundredths into the ring's uncommitted row and its text code (the hundredths, or a
+//                    mark for "-0.0") into a scratch row;
+//   scan_kernel      turns the tile counts into offsets;
+//   ij_write_kernel  rebuilds each text from its code with integer arithmetic, stages each tile at its 16-byte phase
+//                    and stores it aligned (mapjson.cu).
+// The ring has kDepth + 1 rows: the row a render writes is never a held one, so a render nobody fetches (or one the
+// fetch rejects) leaves the history intact.  The fetch composes the document around the body on the host and then
+// commits the row with its timestamp.  The stash fetch renders the held rows, oldest first, with the same
+// three-kernel pattern; the short head (timestamps, min / max / mean, the empty frequency arrays) is made on the host.
+#include "common.cuh"
+#include "json_fmt.cuh"
+#include "scan.cuh"
+
+#include <math.h>
+#include <stdlib.h>
+
+#include <cstring>
+#include <deque>
+#include <new>
+#include <string>
+#include <vector>
+
+using namespace b2;
+
+namespace {
+
+constexpr uint32_t kMaxBins = 65536;     // the spectrum stage's bound
+constexpr uint32_t kDepth = 20;          // nCpi, api/stash/iqdata.js:3
+constexpr uint32_t kRows = kDepth + 1;   // + the row a render writes
+constexpr int kThreads = 256;
+constexpr int kRounds = 4;                 // stash items per thread
+constexpr int kTile = kThreads * kRounds;  // stash items per CTA
+constexpr int kDocTile = kThreads;         // document bins per CTA: one per thread, the render is latency-bound
+constexpr int32_t kMinusZero = INT32_MIN;  // the text code of "-0.0"
+constexpr int kDocItemMax = jf::kMaxText + 1;                // "," before the value
+constexpr int kStashItemMax = jf::kMaxHundredthsText + 3;   // ",[" before the value, "]" after it
+
+// what a render leaves for the fetch
+struct IjInfo {
+  uint32_t nonfinite;  // a bin has no JSON text
+  uint32_t body;       // body bytes (scan_kernel's total)
+};
+
+// One spectrum entry as IqData::to_json computes it: 10 * log10(std::abs(s)), std::abs being hypot; the product is
+// rounded on its own (nothing is contracted).
+__host__ __device__ __forceinline__ double bin_db(double re, double im) {
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(10.0, log10(hypot(re, im)));
+#else
+  return 10.0 * log10(hypot(re, im));
+#endif
+}
+
+// the document text of a bin's value; -1 when rapidjson's Writer has none (|s| = 0, inf or NaN)
+__host__ __device__ __forceinline__ int bin_text(double v, char *t) {
+  return jf::is_finite(v) ? jf::fmt_double(v, t) : -1;
+}
+
+// A bin's document text from its text code: the hundredths k of the text, or kMinusZero for "-0.0".  fmt_double's
+// text of a value below 10^21 is its sign, the integer part, "." and the first two fraction digits of its shortest
+// digits with trailing zeros dropped keeping one, so k and the sign give it back.
+__device__ __forceinline__ int code_text(int32_t code, char *t) {
+  if (code == kMinusZero) {
+    t[0] = '-'; t[1] = '0'; t[2] = '.'; t[3] = '0';
+    return 4;
+  }
+  const int n = jf::fmt_hundredths(code, t);  // the same digits without ".0" where k % 100 == 0
+  if (code % 100 != 0) return n;
+  t[n] = '.';
+  t[n + 1] = '0';
+  return n + 2;
+}
+
+struct DocArgs {
+  const double2 *spec;
+  uint32_t n;
+  int32_t *ring;        // [kRows][n] sent hundredths
+  const uint32_t *row;  // the uncommitted row, set by the host after every commit
+  int32_t *code;        // [n] text codes, written by ij_len_kernel for ij_write_kernel
+  IjInfo *info;
+  uint32_t *tile_len;        // [tiles]
+  const uint32_t *tile_off;  // [tiles + 1]
+  char *body;
+};
+
+// bin j: its separator and its text (*vlen = the text's length, -1 when it has none)
+__device__ __forceinline__ int doc_item(const DocArgs &a, uint32_t j, char *t, int *vlen) {
+  int n = 0;
+  if (j) t[n++] = ',';
+  const double2 s = a.spec[j];
+  *vlen = bin_text(bin_db(s.x, s.y), t + n);
+  return *vlen < 0 ? n : n + *vlen;
+}
+
+__global__ void __launch_bounds__(kThreads) ij_len_kernel(DocArgs a) {
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const uint32_t j = blockIdx.x * kDocTile + threadIdx.x;
+  uint32_t sum = 0;
+  if (j < a.n) {
+    char t[kDocItemMax];
+    int vlen;
+    sum = (uint32_t)doc_item(a, j, t, &vlen);
+    const char *vt = t + (j ? 1 : 0);
+    int32_t k;
+    // a finite bin lies within [-3233.1, 3082.6] dB: its text always has hundredths
+    if (vlen < 0 || !jf::hundredths_of_text(vt, vlen, &k)) {
+      a.info->nonfinite = 1u;  // every writer stores the same value
+    } else {
+      a.ring[(size_t)(*a.row) * a.n + j] = k;
+      a.code[j] = k == 0 && vt[0] == '-' ? kMinusZero : k;
+    }
+  }
+  uint32_t tot;
+  block_excl_scan<kThreads>(sum, wsum, tot);
+  if (threadIdx.x == 0) a.tile_len[blockIdx.x] = tot;
+}
+
+// Stages a tile's texts at the 16-byte phase of its offset and stores them aligned (mapjson.cu: mj_write_kernel).
+template <int ITEM_MAX, int ROUNDS, class F>
+__device__ __forceinline__ void write_tile(uint32_t off, char *body, char *stage, uint32_t *wsum, F item) {
+  const uint32_t phase = off & 15u;  // stage[phase + i] <-> body[off + i]: same address mod 16
+  char t[ITEM_MAX];
+  uint32_t pos = phase;
+  for (int r = 0; r < ROUNDS; r++) {
+    const int n = item(r, t);
+    uint32_t tot;
+    const uint32_t ex = block_excl_scan<kThreads>((uint32_t)n, wsum, tot);
+    for (int i = 0; i < n; i++) stage[pos + ex + i] = t[i];
+    pos += tot;
+  }
+  __syncthreads();
+  const uint32_t g0 = off, g1 = off + (pos - phase);
+  uint32_t a0 = (g0 + 15u) & ~15u, a1 = g1 & ~15u;
+  if (a0 > g1) a0 = g1;
+  if (a1 < a0) a1 = a0;
+  for (uint32_t g = g0 + threadIdx.x; g < a0; g += kThreads) body[g] = stage[g - off + phase];
+  for (uint32_t g = a1 + threadIdx.x; g < g1; g += kThreads) body[g] = stage[g - off + phase];
+  for (uint32_t g = a0 + 16u * threadIdx.x; g < a1; g += 16u * kThreads)
+    *reinterpret_cast<uint4 *>(body + g) = *reinterpret_cast<const uint4 *>(stage + (g - off + phase));
+}
+
+// Writes the texts ij_len_kernel measured, from their codes (a rejected render's body is never read).
+__global__ void __launch_bounds__(kThreads) ij_write_kernel(DocArgs a) {
+  __shared__ __align__(16) char stage[kDocTile * kDocItemMax + 16];
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  write_tile<kDocItemMax, 1>(a.tile_off[blockIdx.x], a.body, stage, wsum, [&](int, char *t) {
+    const uint32_t j = blockIdx.x * kDocTile + threadIdx.x;
+    if (j >= a.n) return 0;
+    int n = 0;
+    if (j) t[n++] = ',';
+    return n + code_text(a.code[j], t + n);
+  });
+}
+
+__global__ void ij_values_kernel(const double2 *spec, uint32_t n, double *out) {
+  for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+    const double2 s = spec[j];
+    out[j] = bin_db(s.x, s.y);
+  }
+}
+
+struct StashArgs {
+  const int32_t *ring;  // [kRows][n]
+  uint32_t n, head, held;  // held rows from ring row head on
+  uint32_t *tile_len;         // [tiles]
+  const uint32_t *tile_off;   // [tiles + 1]
+  char *body;
+};
+
+// item e = (held row e / n, bin e % n) of the /stash/iqdata spectrum arrays: "[" (",[" after the first row) before a
+// row's first value, "," before the others, "]" after a row's last
+__device__ __forceinline__ int stash_item(const StashArgs &a, uint32_t e, char *t) {
+  const uint32_t r = e / a.n, j = e - r * a.n;
+  int n = 0;
+  if (j == 0) {
+    if (r) t[n++] = ',';
+    t[n++] = '[';
+  } else {
+    t[n++] = ',';
+  }
+  const uint32_t slot = (a.head + r) % kRows;
+  n += jf::fmt_hundredths(a.ring[(size_t)slot * a.n + j], t + n);
+  if (j == a.n - 1) t[n++] = ']';
+  return n;
+}
+
+__global__ void __launch_bounds__(kThreads) is_len_kernel(StashArgs a) {
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const uint32_t base = blockIdx.x * kTile, items = a.held * a.n;
+  char t[kStashItemMax];
+  uint32_t sum = 0;
+  for (int r = 0; r < kRounds; r++) {
+    const uint32_t e = base + r * kThreads + threadIdx.x;
+    if (e < items) sum += (uint32_t)stash_item(a, e, t);
+  }
+  uint32_t tot;
+  block_excl_scan<kThreads>(sum, wsum, tot);
+  if (threadIdx.x == 0) a.tile_len[blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(kThreads) is_write_kernel(StashArgs a) {
+  __shared__ __align__(16) char stage[kTile * kStashItemMax + 16];
+  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  const uint32_t base = blockIdx.x * kTile, items = a.held * a.n;
+  write_tile<kStashItemMax, kRounds>(a.tile_off[blockIdx.x], a.body, stage, wsum, [&](int r, char *t) {
+    const uint32_t e = base + r * kThreads + threadIdx.x;
+    return e < items ? stash_item(a, e, t) : 0;
+  });
+}
+
+// the text Writer::Double gives a metric (written once); false when it has none
+bool metric_text(double v, std::string &out) {
+  char t[jf::kMaxText];
+  if (!jf::is_finite(v)) return false;
+  out.assign(t, (size_t)jf::fmt_double(v, t));
+  return true;
+}
+
+// JSON.stringify of what JSON.parse reads from that text
+std::string js_metric(const std::string &text) { return js_number_text(strtod(text.c_str(), nullptr)); }
+
+// everything of the document before the spectrum's values
+std::string doc_head(uint64_t ts, const std::string *metrics) {
+  return "{\"timestamp\":" + std::to_string((unsigned long long)ts) + ",\"min\":" + metrics[0] + ",\"max\":" +
+         metrics[1] + ",\"mean\":" + metrics[2] + ",\"frequency\":[],\"spectrum\":[";
+}
+
+int check_metrics(const char *who, double mn, double mx, double mean, std::string *texts) {
+  const double v[3] = {mn, mx, mean};
+  for (int i = 0; i < 3; i++)
+    if (!metric_text(v[i], texts[i])) {
+      set_last_error(std::string(who) + ": min, max and mean must be finite (rapidjson's Writer has no text otherwise)");
+      return B200DD_ERR_ARG;
+    }
+  return B200DD_OK;
+}
+
+inline int nonfinite_fail(const char *msg) {
+  set_last_error(msg);
+  return B200DD_ERR_NONFINITE;
+}
+
+}  // namespace
+
+struct b200dd_iqjson {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  uint32_t n = 0, tiles = 0, stash_tiles = 0;
+  std::string metric[3];     // min, max, mean as the document writes them
+  std::string js_metric[3];  // ... and as /stash/iqdata re-prints them
+  size_t max_bytes = 0, stash_max_bytes = 0;
+  // per-CPI render
+  char *d_body = nullptr;
+  uint32_t *d_tile_len = nullptr, *d_tile_off = nullptr;  // [tiles], [tiles + 1]
+  int32_t *d_code = nullptr;                              // [n] text codes
+  IjInfo *d_info = nullptr;
+  uint32_t *d_row = nullptr;  // the uncommitted ring row
+  uint32_t row = 0;           // its host copy, the source of the upload after a commit
+  bool pending = false;       // a render not fetched yet
+  // stash
+  int32_t *d_ring = nullptr;  // [kRows][n]
+  char *d_stash = nullptr;
+  uint32_t *d_stile_len = nullptr, *d_stile_off = nullptr;  // [stash_tiles], [stash_tiles + 1]
+  std::deque<std::string> ts_text;  // Number::toString of each held document's timestamp, oldest first
+  uint32_t head = 0;                // ring row of the oldest held document
+};
+
+namespace {
+
+uint32_t free_row(const b200dd_iqjson *h) { return (h->head + (uint32_t)h->ts_text.size()) % kRows; }
+
+// iqdata.js: push the spectrum, frequency and timestamp, dropping the oldest past nCpi
+int commit(b200dd_iqjson *h, uint64_t ts, cudaStream_t st) {
+  h->ts_text.push_back(js_number_text((double)ts));
+  if (h->ts_text.size() > kDepth) {
+    h->ts_text.pop_front();
+    h->head = (h->head + 1) % kRows;
+  }
+  static_assert(kRows > kDepth, "a render must never write a held row");
+  h->row = free_row(h);
+  B2_CUDA(cudaMemcpyAsync(h->d_row, &h->row, sizeof(h->row), cudaMemcpyHostToDevice, st));
+  return B200DD_OK;
+}
+
+}  // namespace
+
+void b2::iqjson_mark_rendered(b200dd_iqjson *h, bool rendered) { h->pending = rendered; }
+
+extern "C" {
+
+int b200dd_iqjson_create(uint32_t n_spectrum, double min, double max, double mean, int32_t device,
+                         b200dd_iqjson **out) {
+  if (!out) return arg_fail("b200dd_iqjson_create: null argument");
+  *out = nullptr;
+  if (n_spectrum == 0 || n_spectrum > kMaxBins) return arg_fail("b200dd_iqjson_create: n_spectrum must be in [1, 65536]");
+  std::string metric[3];
+  const int rc0 = check_metrics("b200dd_iqjson_create", min, max, mean, metric);
+  if (rc0 != B200DD_OK) return rc0;
+  b200dd_iqjson *h = new (std::nothrow) b200dd_iqjson();
+  if (!h) return arg_fail("b200dd_iqjson_create: out of host memory");
+  auto fail = [&](int rc) { b200dd_iqjson_destroy(h); return rc; };
+  h->n = n_spectrum;
+  h->tiles = (n_spectrum + kDocTile - 1) / kDocTile;
+  h->stash_tiles = (kDepth * n_spectrum + kTile - 1) / kTile;
+  for (int i = 0; i < 3; i++) {
+    h->metric[i] = metric[i];
+    h->js_metric[i] = js_metric(metric[i]);
+  }
+  h->max_bytes = doc_head(~0ull, h->metric).size() + (size_t)n_spectrum * kDocItemMax + 2;
+  // the head: 20 timestamps of at most 20 bytes ("18446744073709552000"), metrics, 20 "[]"
+  const size_t head = strlen("{\"timestamp\":[],\"min\":,\"max\":,\"mean\":,\"frequency\":[],\"spectrum\":[") +
+                      kDepth * 21 + h->js_metric[0].size() + h->js_metric[1].size() + h->js_metric[2].size() +
+                      kDepth * 3;
+  h->stash_max_bytes = head + (size_t)kDepth * n_spectrum * kStashItemMax + 2;
+  int dev = device;
+  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
+  h->device = dev;
+  DeviceGuard guard(dev);
+  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
+  auto body = [&]() -> int {
+    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    B2_CUDA(cudaMalloc(&h->d_body, ((size_t)n_spectrum * kDocItemMax + 15) & ~(size_t)15));
+    B2_CUDA(cudaMalloc(&h->d_tile_len, sizeof(uint32_t) * h->tiles));
+    B2_CUDA(cudaMalloc(&h->d_tile_off, sizeof(uint32_t) * (h->tiles + 1)));
+    B2_CUDA(cudaMalloc(&h->d_code, sizeof(int32_t) * n_spectrum));
+    B2_CUDA(cudaMalloc(&h->d_info, sizeof(IjInfo)));
+    B2_CUDA(cudaMalloc(&h->d_row, sizeof(uint32_t)));
+    B2_CUDA(cudaMalloc(&h->d_ring, sizeof(int32_t) * kRows * (size_t)n_spectrum));
+    B2_CUDA(cudaMalloc(&h->d_stash, ((size_t)kDepth * n_spectrum * kStashItemMax + 15) & ~(size_t)15));
+    B2_CUDA(cudaMalloc(&h->d_stile_len, sizeof(uint32_t) * h->stash_tiles));
+    B2_CUDA(cudaMalloc(&h->d_stile_off, sizeof(uint32_t) * (h->stash_tiles + 1)));
+    B2_CUDA(cudaMemsetAsync(h->d_row, 0, sizeof(uint32_t), h->stream));
+    B2_CUDA(cudaStreamSynchronize(h->stream));  // the row is set before a render on another stream
+    return B200DD_OK;
+  };
+  const int rc = body();
+  if (rc != B200DD_OK) return fail(rc);
+  *out = h;
+  return B200DD_OK;
+}
+
+size_t b200dd_iqjson_max_bytes(const b200dd_iqjson *h) { return h ? h->max_bytes : 0; }
+size_t b200dd_iqjson_stash_max_bytes(const b200dd_iqjson *h) { return h ? h->stash_max_bytes : 0; }
+
+void b200dd_iqjson_destroy(b200dd_iqjson *h) {
+  if (!h) return;
+  {
+    DeviceGuard guard(h->device);
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    free_dev(h->d_body);
+    free_dev(h->d_tile_len);
+    free_dev(h->d_tile_off);
+    free_dev(h->d_code);
+    free_dev(h->d_info);
+    free_dev(h->d_row);
+    free_dev(h->d_ring);
+    free_dev(h->d_stash);
+    free_dev(h->d_stile_len);
+    free_dev(h->d_stile_off);
+    if (h->stream) cudaStreamDestroy(h->stream);
+  }
+  delete h;
+}
+
+int b200dd_iqjson_render_device(b200dd_iqjson *h, const void *d_spectrum, void *stream) {
+  if (!h || !d_spectrum) return arg_fail("b200dd_iqjson_render_device: null argument");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  DocArgs a;
+  a.spec = (const double2 *)d_spectrum; a.n = h->n; a.ring = h->d_ring; a.row = h->d_row; a.code = h->d_code; a.info = h->d_info;
+  a.tile_len = h->d_tile_len; a.tile_off = h->d_tile_off; a.body = h->d_body;
+  B2_CUDA(cudaMemsetAsync(h->d_info, 0, sizeof(IjInfo), st));
+  ij_len_kernel<<<h->tiles, kThreads, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)h->tiles, &h->d_info->body);
+  B2_LAUNCH_CHECK();
+  ij_write_kernel<<<h->tiles, kThreads, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  h->pending = true;
+  return B200DD_OK;
+}
+
+int b200dd_iqjson_fetch(b200dd_iqjson *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes, void *stream) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_iqjson_fetch: null argument");
+  if (!h->pending) return arg_fail("b200dd_iqjson_fetch: nothing rendered since the last fetch");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  IjInfo info;
+  B2_CUDA(cudaMemcpyAsync(&info, h->d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  if (info.nonfinite) {
+    h->pending = false;
+    return nonfinite_fail("b200dd_iqjson_fetch: a spectrum bin is zero, infinite or NaN (rapidjson's Writer has no "
+                          "text for its value): no document");
+  }
+  const std::string hdr = doc_head(timestamp, h->metric);
+  const size_t total = hdr.size() + info.body + 2;
+  if (n_bytes) *n_bytes = total;
+  if (total > cap) {
+    set_last_error("b200dd_iqjson_fetch: output capacity too small (see b200dd_iqjson_max_bytes)");
+    return B200DD_ERR_CAPACITY;
+  }
+  memcpy(out, hdr.data(), hdr.size());
+  B2_CUDA(cudaMemcpyAsync(out + hdr.size(), h->d_body, info.body, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  out[total - 2] = ']';
+  out[total - 1] = '}';
+  h->pending = false;
+  return commit(h, timestamp, st);
+}
+
+int b200dd_iqjson_fetch_stash(b200dd_iqjson *h, char *out, size_t cap, size_t *n_bytes, void *stream) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_iqjson_fetch_stash: null argument");
+  if (h->ts_text.empty()) {  // iqdata.js:8, output = []
+    if (n_bytes) *n_bytes = 2;
+    if (cap < 2) return B200DD_ERR_CAPACITY;
+    out[0] = '[';
+    out[1] = ']';
+    return B200DD_OK;
+  }
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  const uint32_t held = (uint32_t)h->ts_text.size();
+  std::string hdr = "{\"timestamp\":[";
+  for (uint32_t i = 0; i < held; i++) hdr += (i ? "," : "") + h->ts_text[i];
+  hdr += "],\"min\":" + h->js_metric[0] + ",\"max\":" + h->js_metric[1] + ",\"mean\":" + h->js_metric[2] +
+         ",\"frequency\":[";
+  for (uint32_t i = 0; i < held; i++) hdr += i ? ",[]" : "[]";
+  hdr += "],\"spectrum\":[";
+  StashArgs a;
+  a.ring = h->d_ring; a.n = h->n; a.head = h->head; a.held = held;
+  a.tile_len = h->d_stile_len; a.tile_off = h->d_stile_off; a.body = h->d_stash;
+  const uint32_t tiles = (held * h->n + kTile - 1) / kTile;
+  is_len_kernel<<<tiles, kThreads, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  scan_kernel<<<1, 1024, 0, st>>>(h->d_stile_len, h->d_stile_off, (int)tiles, h->d_stile_off + tiles);
+  B2_LAUNCH_CHECK();
+  is_write_kernel<<<tiles, kThreads, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  uint32_t body = 0;
+  B2_CUDA(cudaMemcpyAsync(&body, h->d_stile_off + tiles, sizeof(body), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  const size_t total = hdr.size() + body + 2;
+  if (n_bytes) *n_bytes = total;
+  if (total > cap) {
+    set_last_error("b200dd_iqjson_fetch_stash: output capacity too small (see b200dd_iqjson_stash_max_bytes)");
+    return B200DD_ERR_CAPACITY;
+  }
+  memcpy(out, hdr.data(), hdr.size());
+  B2_CUDA(cudaMemcpyAsync(out + hdr.size(), h->d_stash, body, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  out[total - 2] = ']';
+  out[total - 1] = '}';
+  return B200DD_OK;
+}
+
+int b200dd_iqjson_render_host(const double *spectrum, uint32_t n, double min, double max, double mean,
+                              uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if ((n && !spectrum) || !out) return arg_fail("b200dd_iqjson_render_host: null argument");
+  std::string metric[3];
+  const int rc = check_metrics("b200dd_iqjson_render_host", min, max, mean, metric);
+  if (rc != B200DD_OK) return rc;
+  std::string doc = doc_head(timestamp, metric);
+  char t[jf::kMaxText];
+  for (uint32_t j = 0; j < n; j++) {
+    const int len = bin_text(bin_db(spectrum[2 * (size_t)j], spectrum[2 * (size_t)j + 1]), t);
+    if (len < 0) return nonfinite_fail("b200dd_iqjson_render_host: a spectrum bin is zero, infinite or NaN");
+    if (j) doc += ',';
+    doc.append(t, (size_t)len);
+  }
+  doc += "]}";
+  if (n_bytes) *n_bytes = doc.size();
+  if (doc.size() > cap) {
+    set_last_error("b200dd_iqjson_render_host: output capacity too small");
+    return B200DD_ERR_CAPACITY;
+  }
+  memcpy(out, doc.data(), doc.size());
+  return B200DD_OK;
+}
+
+int b200dd_iqjson_debug_bin_values(b200dd_iqjson *h, const void *d_spectrum, void *d_out, void *stream) {
+  if (!h || !d_spectrum || !d_out) return arg_fail("b200dd_iqjson_debug_bin_values: null argument");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  ij_values_kernel<<<(h->n + 255) / 256, 256, 0, st>>>((const double2 *)d_spectrum, h->n, (double *)d_out);
+  B2_LAUNCH_CHECK();
+  return B200DD_OK;
+}
+
+}  // extern "C"

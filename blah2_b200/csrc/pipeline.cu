@@ -1,6 +1,7 @@
 // pipeline.cu -- one CPI through WienerHopf -> Ambiguity -> set_metrics -> detection with all
 // intermediates resident in HBM (the body of the reference's process thread, src/blah2.cpp:268-287).
-// Composes the per-class handles of caf.cu / wh.cu / det.cu / mapjson.cu / maxhold.cu / detjson.cu / tracker.cu through their C ABI; the only kernels
+// Composes the per-class handles of caf.cu / wh.cu / det.cu / spectrum.cu / iqjson.cu / mapjson.cu / maxhold.cu / detjson.cu /
+// tracker.cu through their C ABI; the only kernels
 // defined here are the complex128 <-> complex64 conversions of the host entry point.
 #include "common.cuh"
 
@@ -52,6 +53,8 @@ struct b200dd_pipeline {
   b200dd_wh *wh = nullptr;
   b200dd_det *det = nullptr;
   b200dd_spectrum *spec = nullptr;  // optional first stage (blah2.cpp:263-265)
+  b200dd_iqjson *ij = nullptr;      // optional, after the spectrum: the IQ-data document (blah2.cpp:299-300) and its stash
+  void *ij_stream = nullptr;        // stream of the last submit, where its document was rendered
   b200dd_mapjson *mj = nullptr;     // optional last stage: the map document (blah2.cpp:303-304)
   void *mj_stream = nullptr;        // stream of the last submit, where its document was rendered
   b200dd_maxhold *mh = nullptr;     // optional: the API's max-hold window (api/stash/maxhold.js)
@@ -138,6 +141,7 @@ void b200dd_pipeline_destroy(b200dd_pipeline *h) {
     pipeline_drop_graphs(h);
     b200dd_det_destroy(h->det);
     b200dd_spectrum_destroy(h->spec);
+    b200dd_iqjson_destroy(h->ij);
     b200dd_mapjson_destroy(h->mj);
     b200dd_maxhold_destroy(h->mh);
     b200dd_detjson_destroy(h->dj);
@@ -193,6 +197,13 @@ static int pipeline_enqueue_products(b200dd_pipeline *h, float2 *map, void *st) 
   return B200DD_OK;
 }
 
+// the IQ-data document of the spectrum the spectrum stage just enqueued on `st`, from its own buffer
+static int pipeline_enqueue_iqdata(b200dd_pipeline *h, void *st) {
+  if (!h->ij) return B200DD_OK;
+  h->ij_stream = st;
+  return b200dd_iqjson_render_device(h->ij, spectrum_device_output(h->spec), st);
+}
+
 // the kernels of one CPI on device-resident IQ, enqueued on `st` (also what a graph capture records)
 static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map, void *st) {
   const void *y = d_y;
@@ -200,6 +211,8 @@ static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const vo
   if (h->spec) {  // spectrumAnalyser->process(x), blah2.cpp:264, before the filter touches anything
     if (n < h->spec_nfft) return arg_fail("b200dd_pipeline_submit_device: the spectrum stage needs nfft samples");
     rc = b200dd_spectrum_process_device(h->spec, d_x, n, nullptr, st);
+    if (rc != B200DD_OK) return rc;
+    rc = pipeline_enqueue_iqdata(h, st);
     if (rc != B200DD_OK) return rc;
   }
   if (h->wh) {
@@ -254,6 +267,10 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   if (h->dj) {
     h->dj_stream = st;
     detjson_mark_rendered(h->dj, true);
+  }
+  if (h->ij) {
+    h->ij_stream = st;
+    iqjson_mark_rendered(h->ij, true);
   }
   B2_CUDA(cudaGraphLaunch(g->exec, (cudaStream_t)st));
   return B200DD_OK;
@@ -345,6 +362,8 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   if (h->spec) {  // on the caller's doubles, unrounded
     rc = b200dd_spectrum_process_device_f64(h->spec, h->d_xd, need_x, nullptr, st);
     if (rc != B200DD_OK) return rc;
+    rc = pipeline_enqueue_iqdata(h, st);
+    if (rc != B200DD_OK) return rc;
   }
   if (h->wh) {
     // the filter sees the caller's complex128 samples unrounded (FP64 kernels, in place)
@@ -412,6 +431,9 @@ int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32
   DeviceGuard guard(h->device);
   B2_CUDA(cudaStreamSynchronize(h->stream));
   pipeline_drop_graphs(h);  // the chain changes
+  b200dd_iqjson_destroy(h->ij);  // its bin count may change: the IQ-data stage is enabled again after this
+  h->ij = nullptr;
+  h->ij_stream = nullptr;
   b200dd_spectrum_destroy(h->spec);
   h->spec = nullptr;
   h->spec_bins = h->spec_nfft = 0;
@@ -594,6 +616,51 @@ int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, cha
     h->tr_pending = false;
   }
   return b200dd_tracker_fetch(h->tr, timestamp, out, cap, n_bytes, st);
+}
+
+int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double max, double mean, size_t *doc_bytes,
+                                       size_t *stash_bytes) {
+  if (!h) return arg_fail("b200dd_pipeline_enable_iqdata_json: null handle");
+  if (!h->spec) return arg_fail("b200dd_pipeline_enable_iqdata_json: the spectrum stage is not enabled");
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  pipeline_drop_graphs(h);  // the chain changes
+  b200dd_iqjson_destroy(h->ij);
+  h->ij = nullptr;
+  h->ij_stream = nullptr;
+  const int rc = b200dd_iqjson_create(h->spec_bins, min, max, mean, h->device, &h->ij);
+  if (rc != B200DD_OK) return rc;
+  if (doc_bytes) *doc_bytes = b200dd_iqjson_max_bytes(h->ij);
+  if (stash_bytes) *stash_bytes = b200dd_iqjson_stash_max_bytes(h->ij);
+  return B200DD_OK;
+}
+
+int b200dd_pipeline_fetch_iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_iqdata_json: null argument");
+  if (!h->ij) return arg_fail("b200dd_pipeline_fetch_iqdata_json: the IQ-data JSON stage is not enabled");
+  if (!h->ij_stream) return arg_fail("b200dd_pipeline_fetch_iqdata_json: no CPI submitted since the stage was enabled");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = (cudaStream_t)h->ij_stream;
+  if (h->last_had_filter) {
+    int fs = 0;
+    B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaStreamSynchronize(st));
+    if (fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273): no IQ-data document is sent
+      iqjson_mark_rendered(h->ij, false);
+      set_last_error("b200dd_pipeline_fetch_iqdata_json: the CPI's clutter-filter solve failed; it has no document");
+      return B200DD_FILTER_FAILED;
+    }
+  }
+  return b200dd_iqjson_fetch(h->ij, timestamp, out, cap, n_bytes, st);
+}
+
+int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_iqdata_stash: null argument");
+  if (!h->ij) return arg_fail("b200dd_pipeline_fetch_iqdata_stash: the IQ-data JSON stage is not enabled");
+  DeviceGuard guard(h->device);
+  return b200dd_iqjson_fetch_stash(h->ij, out, cap, n_bytes, h->ij_stream ? h->ij_stream : (void *)h->stream);
 }
 
 int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out,

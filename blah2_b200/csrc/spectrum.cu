@@ -289,6 +289,8 @@ template <class TIN> int run_spectrum(b200dd_spectrum *h, const TIN *d_x, double
 
 }  // namespace
 
+const void *b2::spectrum_device_output(const b200dd_spectrum *h) { return h->d_out; }
+
 extern "C" {
 
 // host half of b200dd_spectrum_create: the constructor's geometry (SpectrumAnalyser.cpp:16-18), the frequency vector

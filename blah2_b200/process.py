@@ -653,6 +653,75 @@ class DetectionJson:
             pass
 
 
+class IqDataJson:
+    """The IQ-data document of blah2.cpp:299-300 (IqData::to_json of the spectrum) and the API's /stash/iqdata history
+    of the last 20 documents (api/stash/iqdata.js).  ``min``, ``max`` and ``mean`` are the IqData members the document
+    carries (blah2 never assigns them); they must be finite.  ``render_device`` renders a device spectrum (a complex128
+    tensor of ``n_spectrum`` bins); ``fetch`` writes its document and commits it to the history; ``fetch_stash`` writes
+    the history.  ``render_host`` needs no handle and no device.  Raises B200ddError with code ERR_NONFINITE for a
+    bin that is zero, infinite or NaN (see include/b200dd.h)."""
+
+    def __init__(self, n_spectrum, min, max, mean, device=-1):
+        lib = capi.load()
+        h = C.c_void_p()
+        capi.check(lib.b200dd_iqjson_create(int(n_spectrum), float(min), float(max), float(mean), int(device),
+                                            C.byref(h)))
+        self._lib, self._h = lib, h
+        self.n_spectrum = int(n_spectrum)
+        self.metrics = (float(min), float(max), float(mean))
+        self.max_bytes = int(lib.b200dd_iqjson_max_bytes(h))
+        self.stash_max_bytes = int(lib.b200dd_iqjson_stash_max_bytes(h))
+        self._out = np.empty(self.max_bytes, dtype=np.uint8)
+        self._stash = np.empty(self.stash_max_bytes, dtype=np.uint8)
+
+    def render_device(self, d_spectrum, stream=None):
+        """Asynchronous: d_spectrum is a complex128 device tensor of n_spectrum bins."""
+        capi.check(self._lib.b200dd_iqjson_render_device(self._h, capi.ptr(d_spectrum),
+                                                         capi.ptr(stream) if stream else None))
+
+    def fetch(self, timestamp, stream=None) -> bytes:
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_iqjson_fetch(self._h, int(timestamp), capi.ptr(self._out), self._out.size,
+                                                 C.byref(n), capi.ptr(stream) if stream else None))
+        return self._out[:n.value].tobytes()
+
+    def fetch_stash(self, stream=None) -> bytes:
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_iqjson_fetch_stash(self._h, capi.ptr(self._stash), self._stash.size, C.byref(n),
+                                                       capi.ptr(stream) if stream else None))
+        return self._stash[:n.value].tobytes()
+
+    def bin_values(self, d_spectrum):
+        """The double of every bin, 10 log10|s| as the device render computes it (a test aid)."""
+        import torch
+        out = torch.empty(self.n_spectrum, dtype=torch.float64, device=d_spectrum.device)
+        capi.check(self._lib.b200dd_iqjson_debug_bin_values(self._h, capi.ptr(d_spectrum), capi.ptr(out), None))
+        torch.cuda.synchronize(d_spectrum.device)
+        return out.cpu().numpy()
+
+    @staticmethod
+    def render_host(spectrum, min, max, mean, timestamp) -> bytes:
+        """IqData::to_json(timestamp) of host complex bins, on the CPU."""
+        lib = capi.load()
+        s = np.ascontiguousarray(np.asarray(spectrum, dtype=np.complex128).ravel())
+        out = np.empty(160 + 25 * s.size, dtype=np.uint8)
+        n = C.c_size_t()
+        capi.check(lib.b200dd_iqjson_render_host(capi.ptr(s), s.size, float(min), float(max), float(mean),
+                                                 int(timestamp), capi.ptr(out), out.size, C.byref(n)))
+        return out[:n.value].tobytes()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.b200dd_iqjson_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def _fetch_growing(buf, call):
     """call(buf) -> (rc, n_bytes); a too-small buffer is grown to the reported size and the call repeated."""
     rc, n = call(buf)
@@ -787,6 +856,8 @@ class Pipeline:
                                                           C.byref(mb)))
             self.track_max_bytes = int(mb.value)
         self._track = np.empty(1 << 16, dtype=np.uint8)
+        self.iqdata_json_max_bytes = self.iqdata_stash_max_bytes = 0  # see enable_iqdata_json
+        self._iqjson = self._iqstash = np.empty(1, dtype=np.uint8)
 
     def fetch_track_json(self, timestamp) -> bytes:
         """The track document after the last fetched CPI (call after fetch()): the first call per CPI runs the tracker
@@ -833,6 +904,34 @@ class Pipeline:
         capi.check(self._lib.b200dd_pipeline_fetch_map_json(self._h, int(timestamp), capi.ptr(self._json),
                                                             self._json.size, C.byref(n)))
         return self._json[:n.value].tobytes()
+
+    def enable_iqdata_json(self, min, max, mean):
+        """Renders the IQ-data document of every CPI submitted from now on (blah2.cpp:299-300), right after the spectrum
+        stage, and keeps the /stash/iqdata history of the last 20 fetched documents, starting empty.  min, max and mean
+        are the IqData members the document carries.  Needs ``spectrum_bandwidth``; enabling the spectrum stage again
+        disables this stage."""
+        db, sb = C.c_size_t(), C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_enable_iqdata_json(self._h, float(min), float(max), float(mean),
+                                                                C.byref(db), C.byref(sb)))
+        self.iqdata_json_max_bytes, self.iqdata_stash_max_bytes = int(db.value), int(sb.value)
+        self._iqjson = np.empty(self.iqdata_json_max_bytes, dtype=np.uint8)
+        self._iqstash = np.empty(self.iqdata_stash_max_bytes, dtype=np.uint8)
+
+    def fetch_iqdata_json(self, timestamp) -> bytes:
+        """The IQ-data document of the last fetched CPI (call after fetch()), committed to the /stash/iqdata history.
+        Raises B200ddError with code FILTER_FAILED when that CPI's clutter-filter solve failed (nothing is sent, the
+        history is unchanged), ERR_NONFINITE when a spectrum bin has no text."""
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_fetch_iqdata_json(self._h, int(timestamp), capi.ptr(self._iqjson),
+                                                               self._iqjson.size, C.byref(n)))
+        return self._iqjson[:n.value].tobytes()
+
+    def fetch_iqdata_stash(self) -> bytes:
+        """The /stash/iqdata document of the documents fetched so far."""
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_fetch_iqdata_stash(self._h, capi.ptr(self._iqstash), self._iqstash.size,
+                                                                C.byref(n)))
+        return self._iqstash[:n.value].tobytes()
 
     def fetch_spectrum(self):
         """Spectrum of the reference channel of the last submitted CPI (complex128, nSpectrum bins)."""

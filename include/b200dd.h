@@ -26,6 +26,8 @@
  *                       /stash/detection, api/server.js:99-100)
  *   b200dd_tracker_*    Tracker::process + Track::to_json, src/process/tracker/Tracker.cpp, src/data/Track.cpp
  *                       (blah2.cpp:291-296, :324-328)
+ *   b200dd_iqjson_*     IqData::to_json, src/data/IqData.cpp:93-125 (blah2.cpp:299-300), and the API's IQ-data
+ *                       stash, api/stash/iqdata.js (served at /stash/iqdata, api/server.js:102-103)
  *
  * Data conventions
  *   host IQ      interleaved complex128 (re, im doubles) -- what IqData holds
@@ -72,8 +74,8 @@ extern "C" {
 #define B200DD_ERR_GEOMETRY 2    /* geometry outside the supported range (see DESIGN.md "limits") */
 #define B200DD_ERR_CUDA 3        /* CUDA runtime error; b200dd_last_error() has the text */
 #define B200DD_ERR_CAPACITY 4    /* output capacity too small (detections, map JSON) */
-#define B200DD_ERR_NONFINITE 5   /* map / detection JSON: a value rapidjson cannot write (a map cell with |z| = 0,
-                                    inf or NaN; a detection that is not finite) */
+#define B200DD_ERR_NONFINITE 5   /* map / detection / IQ-data JSON: a value rapidjson cannot write (a map cell or
+                                    spectrum bin with |z| = 0, inf or NaN; a detection that is not finite) */
 #define B200DD_FILTER_FAILED 10  /* WienerHopf: matrix not positive definite -> y left untouched
                                     (reference returns false, WienerHopf.cpp:111-122) */
 
@@ -508,6 +510,57 @@ B200DD_API int b200dd_detjson_fetch_stash(b200dd_detjson *h, char *out, size_t c
 B200DD_API int b200dd_detjson_render_host(const double *delay, const double *doppler, const double *snr, uint32_t n,
                                           uint64_t timestamp, uint32_t fs, char *out, size_t cap, size_t *n_bytes);
 
+/* ------------------------------------------------------------------ IQ-data JSON
+ *
+ * The document blah2 sends on its IQ-data socket for every CPI: the std::string returned by x->to_json(timestamp)
+ * (src/blah2.cpp:299-300, src/data/IqData.cpp:93-125), byte for byte:
+ *   {"timestamp":T,"min":m,"max":M,"mean":u,"frequency":[],"spectrum":[..]}
+ * Each spectrum entry is 10 log10(hypot(re, im)) of one SpectrumAnalyser bin, written once by rapidjson's Writer at two
+ * decimal places (no read-back); min, max and mean are written the same way.  frequency is always empty: the
+ * analyser's uint32_t loop never runs.  blah2 never assigns IqData's min, max and mean, so here they are the values
+ * the caller's IqData holds, fixed when the handle is created; a non-finite one is rejected with B200DD_ERR_ARG.  A bin
+ * with |s| = 0, inf or NaN makes rapidjson's Writer stop mid-document: B200DD_ERR_NONFINITE, nothing written.
+ *
+ * The handle also keeps the API's history, /stash/iqdata (api/stash/iqdata.js, api/server.js:102-103): the spectrum,
+ * frequency and timestamp of the last 20 fetched documents, sent as JSON.stringify of the newest document with those
+ * three members replaced by the arrays, {"timestamp":[..],"min":m,"max":M,"mean":u,"frequency":[[],..],
+ * "spectrum":[[..],..]}, every number as Number::toString (see b200dd_maxhold_*); "[]" before the first document.
+ * Every spectrum text is k/100 for an integer k, so the history is a device ring of 21 int32 rows.  Not reproduced:
+ * the API loses its first document after start, its 100 ms polling skips documents that arrive faster, and after a
+ * truncated document blah2's socket text runs into the next one, which the API then loses too; every fetched document
+ * is taken here.  Device memory: n_spectrum * 413 bytes.
+ */
+typedef struct b200dd_iqjson b200dd_iqjson;
+
+/* n_spectrum in [1, 65536] bins; min, max, mean finite (else B200DD_ERR_ARG). */
+B200DD_API int b200dd_iqjson_create(uint32_t n_spectrum, double min, double max, double mean, int32_t device,
+                                    b200dd_iqjson **out);
+/* Upper bound of an IQ-data document's size in bytes. */
+B200DD_API size_t b200dd_iqjson_max_bytes(const b200dd_iqjson *h);
+/* Upper bound of the /stash/iqdata document's size in bytes. */
+B200DD_API size_t b200dd_iqjson_stash_max_bytes(const b200dd_iqjson *h);
+B200DD_API void b200dd_iqjson_destroy(b200dd_iqjson *h);
+/* Renders the document body of a device spectrum d_spectrum = double2[n_spectrum], asynchronously on `stream` (NULL =
+ * the handle's stream); the launch shape depends only on n_spectrum, so the call can be recorded in a CUDA graph.
+ * Also writes the bins' hundredths into the history's free row, where the next commit takes them. */
+B200DD_API int b200dd_iqjson_render_device(b200dd_iqjson *h, const void *d_spectrum, void *stream);
+/* Writes the last render's document with `timestamp` into out (*n_bytes = its length), then commits it to the
+ * history.  Synchronises `stream` (the render's stream).  Each render is fetched once; B200DD_ERR_ARG when nothing was
+ * rendered since the last fetch.  B200DD_ERR_NONFINITE: nothing written or committed.  B200DD_ERR_CAPACITY: cap <
+ * *n_bytes, nothing written or committed (the same render may be fetched again). */
+B200DD_API int b200dd_iqjson_fetch(b200dd_iqjson *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
+                                   void *stream);
+/* Writes the /stash/iqdata document into out; *n_bytes = its length.  Synchronises `stream`.
+ * B200DD_ERR_CAPACITY: cap < *n_bytes. */
+B200DD_API int b200dd_iqjson_fetch_stash(b200dd_iqjson *h, char *out, size_t cap, size_t *n_bytes, void *stream);
+/* The IQ-data document of n HOST bins (complex128), without a handle or a device.  B200DD_ERR_ARG: a non-finite
+ * min, max or mean.  B200DD_ERR_NONFINITE: a bin has no text, nothing written.  B200DD_ERR_CAPACITY: cap < *n_bytes. */
+B200DD_API int b200dd_iqjson_render_host(const double *spectrum, uint32_t n, double min, double max, double mean,
+                                         uint64_t timestamp, char *out, size_t cap, size_t *n_bytes);
+/* Test entry point: the double of every bin, 10 log10|s| as the render computes it, into d_out[n_spectrum] (device
+ * memory).  Asynchronous on `stream`. */
+B200DD_API int b200dd_iqjson_debug_bin_values(b200dd_iqjson *h, const void *d_spectrum, void *d_out, void *stream);
+
 /* ------------------------------------------------------------------ tracker
  *
  * Tracker::process + Track::to_json (src/process/tracker/Tracker.cpp, src/data/Track.cpp; blah2.cpp:291-296 and
@@ -697,6 +750,22 @@ B200DD_API int b200dd_pipeline_enable_tracker(b200dd_pipeline *h, const b200dd_t
  * nothing written, the tracker unchanged. */
 B200DD_API int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
                                                 size_t *n_bytes);
+
+/* Optional stage after the spectrum (src/blah2.cpp:299-300): renders the IQ-data document (see b200dd_iqjson_*) of
+ * every CPI submitted afterwards from the spectrum stage's device buffer, right after the spectrum kernels, and keeps
+ * the /stash/iqdata history; works in recorded graphs.  min, max and mean are the IqData members the document
+ * carries.  Drops the graphs recorded so far and starts an empty history.  *doc_bytes / *stash_bytes (nullable) =
+ * the two documents' size bounds.  B200DD_ERR_ARG when the spectrum stage is not enabled or a metric is not finite.
+ * b200dd_pipeline_enable_spectrum disables this stage (it may change the number of bins): enable it again after. */
+B200DD_API int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double max, double mean,
+                                                  size_t *doc_bytes, size_t *stash_bytes);
+/* Called after b200dd_pipeline_fetch: writes the last CPI's IQ-data document and commits it to the history, as
+ * b200dd_iqjson_fetch.  B200DD_FILTER_FAILED, nothing written or committed, when that CPI's clutter-filter solve
+ * failed (blah2.cpp:270-273 skips the CPI). */
+B200DD_API int b200dd_pipeline_fetch_iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
+                                                 size_t *n_bytes);
+/* The /stash/iqdata document of the pipeline's history (see b200dd_iqjson_fetch_stash). */
+B200DD_API int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes);
 
 /* ------------------------------------------------------------------------------------------------
  * Inter-GPU exchanges (one process per GPU, NCCL over NVLink / NVSwitch).  The reference has no
