@@ -175,6 +175,7 @@ SIGNATURES = [
                                                      C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_iqdata_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_iqdata_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_share_history", C.c_int, [_VP, C.c_uint32]),
     ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),
     ("b200dd_mapjson_destroy", None, [_VP]),

@@ -91,5 +91,10 @@ int detjson_check_axes(const int32_t *delay, uint32_t n_del, const double *doppl
 const void *spectrum_device_output(const b200dd_spectrum *h);
 // iqjson.cu: a render recorded in a graph was replayed (true), or the pipeline dropped the CPI's document (false).
 void iqjson_mark_rendered(b200dd_iqjson *h, bool rendered);
+// detjson.cu / iqjson.cu: makes h a member render of a share set whose history is `hist` (a handle of the same
+// parameters): h's own history is emptied and its stash buffers freed, its renders stage in its own ring, and its
+// fetch copies the staged values into hist's ring and commits there; its stash fetch renders hist's.  Synchronous.
+int detjson_share(b200dd_detjson *h, b200dd_detjson *hist);
+int iqjson_share(b200dd_iqjson *h, b200dd_iqjson *hist);
 
 }  // namespace b2

@@ -175,6 +175,18 @@ __global__ void __launch_bounds__(kThreads) dj_write_kernel(DocArgs a) {
   });
 }
 
+// A share-set member's commit: copies the triples its render staged at [0, count) of its own ring into the shared
+// ring from `tail` on.  The count is the list's, read here, so the host need not know it.
+__global__ void dj_commit_kernel(const int32_t *__restrict__ stage, uint32_t stage_cap, const uint32_t *count,
+                                 int32_t *__restrict__ ring, uint32_t ring_cap, uint32_t tail) {
+  const uint32_t raw = *count, n = raw < kListCap ? raw : kListCap;
+  for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+    const uint32_t slot = (uint32_t)(((uint64_t)tail + j) % ring_cap);
+#pragma unroll
+    for (int arr = 0; arr < 3; arr++) ring[(size_t)arr * ring_cap + slot] = stage[(size_t)arr * stage_cap + j];
+  }
+}
+
 struct StashArgs {
   const int32_t *ring;  // [3][ring_cap]
   uint32_t ring_cap, head, held;
@@ -268,6 +280,9 @@ struct b200dd_detjson {
   uint64_t head = 0, tail = 0;  // absolute entry numbers: [head, tail) held
   bool overflowed = false;
   DjRing ring_state{0, 0};
+  // a share-set member (detjson_share): its renders stage at [0, n) of d_ring (its ring state stays {0, ring_cap})
+  // and its fetches commit into hist, the set's history
+  b200dd_detjson *hist = nullptr;
 };
 
 namespace {
@@ -302,6 +317,18 @@ int commit(b200dd_detjson *h, uint64_t ts, uint32_t n, cudaStream_t st) {
   return upload_ring_state(h, st);
 }
 
+// a member's commit: the staged triples go to the set's ring, then the set's history takes the document
+int commit_shared(b200dd_detjson *h, uint64_t ts, uint32_t n, cudaStream_t st) {
+  b200dd_detjson *H = h->hist;
+  if (!H->overflowed && (H->tail - H->head) + n <= H->ring_cap && n) {
+    const uint32_t want = (n + 255) / 256;
+    dj_commit_kernel<<<want < 132 ? want : 132, 256, 0, st>>>(h->d_ring, h->ring_cap, &h->d_info->count, H->d_ring,
+                                                              H->ring_cap, (uint32_t)(H->tail % H->ring_cap));
+    B2_LAUNCH_CHECK();
+  }
+  return commit(H, ts, n, st);
+}
+
 // device array p of `have` elements grown to at least `need` (doubling), contents not kept
 template <class T> int grow(T *&p, size_t &have, size_t need) {
   if (need <= have) return B200DD_OK;
@@ -316,6 +343,27 @@ template <class T> int grow(T *&p, size_t &have, size_t need) {
 }  // namespace
 
 void b2::detjson_mark_rendered(b200dd_detjson *h, bool rendered) { h->pending = rendered; }
+
+int b2::detjson_share(b200dd_detjson *h, b200dd_detjson *hist) {
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  h->records.clear();
+  h->head = h->tail = 0;
+  h->overflowed = false;
+  h->pending = false;
+  const int rc = upload_ring_state(h, h->stream);  // {0, ring_cap}: every render stages at [0, n)
+  if (rc != B200DD_OK) return rc;
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  free_dev(h->d_stash);  // the stash is rendered from hist
+  free_dev(h->d_stile_len);
+  free_dev(h->d_stile_off);
+  free_dev(h->d_doc_first);
+  free_dev(h->d_doc_text);
+  free_dev(h->d_texts);
+  h->first_alloc = h->toff_alloc = h->texts_alloc = 0;
+  h->hist = hist;
+  return B200DD_OK;
+}
 
 int b2::detjson_check_axes(const int32_t *delay, uint32_t n_del, const double *doppler, uint32_t n_dop, uint32_t fs) {
   char t[jf::kMaxText];
@@ -472,12 +520,13 @@ int b200dd_detjson_fetch(b200dd_detjson *h, uint64_t timestamp, char *out, size_
                    "stash does not take it");
     return B200DD_ERR_ARG;
   }
-  return commit(h, timestamp, info.count, st);
+  return h->hist ? commit_shared(h, timestamp, info.count, st) : commit(h, timestamp, info.count, st);
 }
 
 int b200dd_detjson_fetch_stash(b200dd_detjson *h, char *out, size_t cap, size_t *n_bytes, void *stream) {
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_detjson_fetch_stash: null argument");
+  if (h->hist) h = h->hist;
   if (h->overflowed) {
     set_last_error("b200dd_detjson_fetch_stash: the stash's ring overflowed (see max_held)");
     return B200DD_ERR_CAPACITY;

@@ -279,6 +279,8 @@ struct b200dd_iqjson {
   uint32_t *d_stile_len = nullptr, *d_stile_off = nullptr;  // [stash_tiles], [stash_tiles + 1]
   std::deque<std::string> ts_text;  // Number::toString of each held document's timestamp, oldest first
   uint32_t head = 0;                // ring row of the oldest held document
+  // a share-set member (iqjson_share): its renders write ring row 0, its fetches commit into hist, the set's history
+  b200dd_iqjson *hist = nullptr;
 };
 
 namespace {
@@ -298,9 +300,33 @@ int commit(b200dd_iqjson *h, uint64_t ts, cudaStream_t st) {
   return B200DD_OK;
 }
 
+// a member's commit: its row joins the set's history at the history's free row
+int commit_shared(b200dd_iqjson *h, uint64_t ts, cudaStream_t st) {
+  b200dd_iqjson *H = h->hist;
+  B2_CUDA(cudaMemcpyAsync(H->d_ring + (size_t)free_row(H) * H->n, h->d_ring, sizeof(int32_t) * h->n,
+                          cudaMemcpyDeviceToDevice, st));
+  return commit(H, ts, st);
+}
+
 }  // namespace
 
 void b2::iqjson_mark_rendered(b200dd_iqjson *h, bool rendered) { h->pending = rendered; }
+
+int b2::iqjson_share(b200dd_iqjson *h, b200dd_iqjson *hist) {
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  h->ts_text.clear();
+  h->head = 0;
+  h->row = 0;
+  h->pending = false;
+  B2_CUDA(cudaMemcpyAsync(h->d_row, &h->row, sizeof(h->row), cudaMemcpyHostToDevice, h->stream));
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  free_dev(h->d_stash);  // the stash is rendered from hist
+  free_dev(h->d_stile_len);
+  free_dev(h->d_stile_off);
+  h->hist = hist;
+  return B200DD_OK;
+}
 
 extern "C" {
 
@@ -423,12 +449,13 @@ int b200dd_iqjson_fetch(b200dd_iqjson *h, uint64_t timestamp, char *out, size_t 
   out[total - 2] = ']';
   out[total - 1] = '}';
   h->pending = false;
-  return commit(h, timestamp, st);
+  return h->hist ? commit_shared(h, timestamp, st) : commit(h, timestamp, st);
 }
 
 int b200dd_iqjson_fetch_stash(b200dd_iqjson *h, char *out, size_t cap, size_t *n_bytes, void *stream) {
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_iqjson_fetch_stash: null argument");
+  if (h->hist) h = h->hist;
   if (h->ts_text.empty()) {  // iqdata.js:8, output = []
     if (n_bytes) *n_bytes = 2;
     if (cap < 2) return B200DD_ERR_CAPACITY;

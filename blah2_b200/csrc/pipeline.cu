@@ -5,6 +5,7 @@
 // defined here are the complex128 <-> complex64 conversions of the host entry point.
 #include "common.cuh"
 
+#include <algorithm>
 #include <new>
 #include <vector>
 
@@ -44,6 +45,23 @@ inline int grid_for(uint32_t n) {
 }
 
 }  // namespace
+
+// The stateful stages of a share set (b200dd_pipeline_share_history): one max-hold window, one detection history,
+// one IQ-data history and one tracker for all members, each null when the members do not enable it.  Every
+// operation on them is enqueued on the stream of the member that makes it, after the set's event, and records the
+// event again: so they run in the order the host calls them, whatever streams the members use.
+struct ShareSet {
+  int device = 0;
+  std::vector<b200dd_pipeline *> members;
+  int64_t next_cpi = 0;  // the number the next submit to any member gets
+  b200dd_maxhold *mh = nullptr;
+  b200dd_detjson *dj = nullptr;
+  b200dd_iqjson *ij = nullptr;
+  b200dd_tracker *tr = nullptr;
+  int64_t mh_last = -1, dj_last = -1, ij_last = -1, tr_last = -1;  // the CPI each one took last
+  cudaEvent_t ev = nullptr;
+  bool ev_recorded = false;
+};
 
 struct b200dd_pipeline {
   b200dd_pipeline_params p;
@@ -85,6 +103,18 @@ struct b200dd_pipeline {
   };
   std::vector<GraphEntry> graphs;
   bool eager_only = false;  // the chain could not be captured: every submit eager, prepare is a no-op
+  // the stateful stages' parameters, compared by b200dd_pipeline_share_history
+  double spec_bandwidth = 0.0;
+  double ij_metrics[3] = {0.0, 0.0, 0.0};
+  uint32_t dj_max_held = 0;
+  b200dd_tracker_params tr_params{};
+  uint32_t tr_max_tracks = 0, tr_max_history = 0;
+  // share-set membership: the stateful stages above are null and the set's are used
+  ShareSet *set = nullptr;
+  int64_t cpi = -1;             // the set's number of the last CPI submitted here
+  bool unfetched = false;       // ... and b200dd_pipeline_fetch has not taken it yet
+  void *cpi_stream = nullptr;   // the stream it was submitted on
+  const void *cpi_map = nullptr;  // its float2 map, pushed into the set's max-hold window at fetch
 };
 
 extern "C" {
@@ -131,11 +161,14 @@ int b200dd_pipeline_create(const b200dd_pipeline_params *params, b200dd_pipeline
   return B200DD_OK;
 }
 
+static void set_leave(b200dd_pipeline *h);
+
 void b200dd_pipeline_destroy(b200dd_pipeline *h) {
   if (!h) return;
   {
     DeviceGuard guard(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
+    set_leave(h);
     b200dd_caf_destroy(h->caf);
     b200dd_wh_destroy(h->wh);
     pipeline_drop_graphs(h);
@@ -246,15 +279,27 @@ static const b200dd_pipeline::GraphEntry *pipeline_find_graph(const b200dd_pipel
   return nullptr;
 }
 
+// A share-set member takes one CPI at a time: B200DD_ERR_ARG while its last one is not fetched.
+static int member_may_submit(const b200dd_pipeline *h, const char *msg) {
+  return h->set && h->unfetched ? arg_fail(msg) : B200DD_OK;
+}
+
+// a share-set member numbers the CPI just enqueued on `st` with map `map`
+static void member_submitted(b200dd_pipeline *h, void *st, const void *map) {
+  if (!h->set) return;
+  h->cpi = h->set->next_cpi++;
+  h->unfetched = true;
+  h->cpi_stream = st;
+  h->cpi_map = map ? map : h->d_map;
+}
+
 // A CPI is 12+ kernel launches on the single submitting thread.  The chain's arguments only depend on the caller's
 // three device pointers, so a triple can be recorded by stream capture (everything below runs on `st`; no
 // allocation, attribute call or host copy after the first eager run) and replayed with ONE cudaGraphLaunch.
 // Replay pays off in a submit -> fetch -> submit loop; in a deep queue of CPIs enqueued ahead eager launches can be
 // faster, so replay is opt-in per triple (b200dd_pipeline_prepare_device).
-int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
+static int pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
                                   void *stream) {
-  if (!h || !d_x || !d_y) return arg_fail("b200dd_pipeline_submit_device: null argument");
-  if (h->wh && n != h->p.caf.n_samples) return arg_fail("b200dd_pipeline_submit_device: the clutter filter needs exactly n_samples");
   DeviceGuard guard(h->device);
   void *st = stream ? stream : (void *)h->stream;
   const b200dd_pipeline::GraphEntry *g = pipeline_find_graph(h, d_x, d_y, n, d_map);
@@ -276,6 +321,17 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   return B200DD_OK;
 }
 
+int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
+                                  void *stream) {
+  if (!h || !d_x || !d_y) return arg_fail("b200dd_pipeline_submit_device: null argument");
+  if (h->wh && n != h->p.caf.n_samples) return arg_fail("b200dd_pipeline_submit_device: the clutter filter needs exactly n_samples");
+  int rc = member_may_submit(h, "b200dd_pipeline_submit_device: the share-set member's last CPI is not fetched yet");
+  if (rc != B200DD_OK) return rc;
+  rc = pipeline_submit_device(h, d_x, d_y, n, d_map, stream);
+  if (rc == B200DD_OK) member_submitted(h, stream ? stream : (void *)h->stream, d_map);
+  return rc;
+}
+
 int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
                                    void *stream) {
   if (!h || !d_x || !d_y) return arg_fail("b200dd_pipeline_prepare_device: null argument");
@@ -284,9 +340,12 @@ int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const vo
   DeviceGuard guard(h->device);
   void *st = stream ? stream : (void *)h->stream;
   if (!pipeline_find_graph(h, d_x, d_y, n, d_map)) {
-    // the eager run sets up what a capture must not do (uploads the axes, sizes scratch buffers)
-    int rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
+    // the eager run sets up what a capture must not do (uploads the axes, sizes scratch buffers); it is a CPI
+    int rc = member_may_submit(h, "b200dd_pipeline_prepare_device: the share-set member's last CPI is not fetched yet");
     if (rc != B200DD_OK) return rc;
+    rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
+    if (rc != B200DD_OK) return rc;
+    member_submitted(h, st, d_map);
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     if (cudaStreamBeginCapture((cudaStream_t)st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -308,11 +367,49 @@ int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const vo
   return B200DD_OK;
 }
 
+// the set's operations run after the previous one (see ShareSet)
+static int set_wait(ShareSet *s, void *st) {
+  if (s->ev_recorded) B2_CUDA(cudaStreamWaitEvent((cudaStream_t)st, s->ev, 0));
+  return B200DD_OK;
+}
+
+static int set_record(ShareSet *s, void *st) {
+  B2_CUDA(cudaEventRecord(s->ev, (cudaStream_t)st));
+  s->ev_recorded = true;
+  return B200DD_OK;
+}
+
+// b200dd_pipeline_fetch of a share-set member: its CPI must be the set's oldest unfetched one; it enters the
+// max-hold window now, on the stream it was submitted on
+static int member_fetch(b200dd_pipeline *h) {
+  ShareSet *s = h->set;
+  if (!h->unfetched) return arg_fail("b200dd_pipeline_fetch: the share-set member has no unfetched CPI");
+  for (const b200dd_pipeline *m : s->members)
+    if (m != h && m->unfetched && m->cpi < h->cpi)
+      return arg_fail("b200dd_pipeline_fetch: an older CPI of the share set is not fetched yet (fetch in submit order)");
+  if (s->mh) {
+    int rc = set_wait(s, h->cpi_stream);
+    if (rc != B200DD_OK) return rc;
+    rc = maxhold_enqueue_with_metrics(s->mh, h->cpi_map, det_device_metrics(h->det),
+                                      h->wh ? b200dd_wh_device_status(h->wh) : nullptr, (cudaStream_t)h->cpi_stream);
+    if (rc != B200DD_OK) return rc;
+    rc = set_record(s, h->cpi_stream);
+    if (rc != B200DD_OK) return rc;
+    s->mh_last = h->cpi;
+  }
+  h->unfetched = false;
+  return B200DD_OK;
+}
+
 int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double *o_delay, double *o_doppler,
                           double *o_snr, uint32_t cap, void *stream) {
   if (!h || !result) return arg_fail("b200dd_pipeline_fetch: null argument");
   DeviceGuard guard(h->device);
   void *st = stream ? stream : (void *)h->stream;
+  if (h->set) {
+    const int rc = member_fetch(h);
+    if (rc != B200DD_OK) return rc;
+  }
   result->filter_status = B200DD_OK;
   result->n_detections = 0;
   result->noise_power = 0.0;
@@ -340,6 +437,8 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   const uint32_t N = h->p.caf.n_samples;
   const uint32_t need = h->wh ? N : h->g.n_used;
   if (h->wh ? (n != N) : (n < need)) return arg_fail("b200dd_pipeline_submit_host: wrong number of samples");
+  int rc = member_may_submit(h, "b200dd_pipeline_submit_host: the share-set member's last CPI is not fetched yet");
+  if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
   if (!h->d_xd) {
@@ -358,7 +457,6 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   }
   B2_CUDA(cudaMemcpyAsync(h->d_xd, x, sizeof(double2) * need_x, cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemcpyAsync(h->d_yd, y, sizeof(double2) * need, cudaMemcpyHostToDevice, st));
-  int rc;
   if (h->spec) {  // on the caller's doubles, unrounded
     rc = b200dd_spectrum_process_device_f64(h->spec, h->d_xd, need_x, nullptr, st);
     if (rc != B200DD_OK) return rc;
@@ -388,6 +486,7 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
     B2_LAUNCH_CHECK();
     B2_CUDA(cudaMemcpyAsync(map_out, h->d_mapd, sizeof(double2) * cells, cudaMemcpyDeviceToHost, st));
   }
+  member_submitted(h, st, h->d_map);
   return B200DD_OK;
 }
 
@@ -396,6 +495,8 @@ int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, ui
   const uint32_t N = h->p.caf.n_samples;
   uint32_t need = h->wh ? N : h->g.n_used;
   if (h->wh ? (n != N) : (n < need)) return arg_fail("b200dd_pipeline_submit_host_rspduo: wrong number of samples");
+  int rc = member_may_submit(h, "b200dd_pipeline_submit_host_rspduo: the share-set member's last CPI is not fetched yet");
+  if (rc != B200DD_OK) return rc;
   if (h->spec && h->spec_nfft > need) {
     if (n < h->spec_nfft) return arg_fail("b200dd_pipeline_submit_host_rspduo: the spectrum stage needs nfft samples");
     need = h->spec_nfft;  // <= n_samples; the CAF still consumes n_used of them
@@ -415,7 +516,7 @@ int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, ui
   B2_LAUNCH_CHECK();
   // int16 samples are exact in float32, so the float2 device path gives the same result as the
   // complex128 host path
-  int rc = b200dd_pipeline_submit_device(h, h->d_xf, h->d_yf2, need, h->d_map, st);
+  rc = pipeline_submit_device(h, h->d_xf, h->d_yf2, need, h->d_map, st);
   if (rc != B200DD_OK) return rc;
   if (map_out) {
     const uint32_t cells = h->g.n_doppler_bins * h->g.n_delay_bins;
@@ -423,11 +524,14 @@ int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, ui
     B2_LAUNCH_CHECK();
     B2_CUDA(cudaMemcpyAsync(map_out, h->d_mapd, sizeof(double2) * cells, cudaMemcpyDeviceToHost, st));
   }
+  member_submitted(h, st, h->d_map);
   return B200DD_OK;
 }
 
 int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32_t *n_spectrum) {
   if (!h) return arg_fail("b200dd_pipeline_enable_spectrum: null handle");
+  if (h->set && h->set->ij)
+    return arg_fail("b200dd_pipeline_enable_spectrum: the member's share set keeps an IQ-data history of its spectra");
   DeviceGuard guard(h->device);
   B2_CUDA(cudaStreamSynchronize(h->stream));
   pipeline_drop_graphs(h);  // the chain changes
@@ -443,6 +547,7 @@ int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32
   b200dd_spectrum_get_geometry(h->spec, &sg);
   h->spec_bins = sg.n_spectrum;
   h->spec_nfft = sg.nfft;
+  h->spec_bandwidth = bandwidth;
   if (n_spectrum) *n_spectrum = sg.n_spectrum;
   return B200DD_OK;
 }
@@ -490,6 +595,7 @@ int b200dd_pipeline_fetch_map_json(b200dd_pipeline *h, uint64_t timestamp, char 
 
 int b200dd_pipeline_enable_maxhold(b200dd_pipeline *h, size_t *max_bytes) {
   if (!h) return arg_fail("b200dd_pipeline_enable_maxhold: null handle");
+  if (h->set) return arg_fail("b200dd_pipeline_enable_maxhold: a share-set member's stateful stages are the set's");
   DeviceGuard guard(h->device);
   B2_CUDA(cudaStreamSynchronize(h->stream));
   pipeline_drop_graphs(h);  // the chain changes
@@ -506,6 +612,16 @@ int b200dd_pipeline_enable_maxhold(b200dd_pipeline *h, size_t *max_bytes) {
 int b200dd_pipeline_fetch_maxhold(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_maxhold: null argument");
+  if (ShareSet *s = h->set) {
+    if (!s->mh) return arg_fail("b200dd_pipeline_fetch_maxhold: the max-hold stage is not enabled");
+    if (h->cpi < 0 || h->unfetched || h->cpi != s->mh_last)
+      return arg_fail("b200dd_pipeline_fetch_maxhold: the share-set member's CPI is not the last one the window took "
+                      "(call after b200dd_pipeline_fetch, before the next CPI of the set is fetched)");
+    DeviceGuard guard(h->device);
+    const int rc = set_wait(s, h->cpi_stream);
+    if (rc != B200DD_OK) return rc;
+    return b200dd_maxhold_fetch(s->mh, timestamp, out, cap, n_bytes, h->cpi_stream);
+  }
   if (!h->mh) return arg_fail("b200dd_pipeline_fetch_maxhold: the max-hold stage is not enabled");
   if (!h->mh_stream) return arg_fail("b200dd_pipeline_fetch_maxhold: no CPI submitted since the stage was enabled");
   DeviceGuard guard(h->device);
@@ -515,6 +631,7 @@ int b200dd_pipeline_fetch_maxhold(b200dd_pipeline *h, uint64_t timestamp, char *
 int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held, size_t *doc_bytes,
                                           size_t *stash_bytes) {
   if (!h) return arg_fail("b200dd_pipeline_enable_detection_json: null handle");
+  if (h->set) return arg_fail("b200dd_pipeline_enable_detection_json: a share-set member's stateful stages are the set's");
   if (!h->p.detection_enable) return arg_fail("b200dd_pipeline_enable_detection_json: detection is not enabled");
   int rc = detjson_check_axes(h->delay.data(), h->g.n_delay_bins, h->doppler.data(), h->g.n_doppler_bins, h->p.caf.fs);
   if (rc != B200DD_OK) return rc;
@@ -526,6 +643,7 @@ int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held,
   h->dj_stream = nullptr;
   rc = b200dd_detjson_create(h->p.caf.fs, max_held, h->device, &h->dj);
   if (rc != B200DD_OK) return rc;
+  h->dj_max_held = max_held;
   if (doc_bytes) *doc_bytes = b200dd_detjson_max_bytes(h->dj);
   if (stash_bytes) *stash_bytes = b200dd_detjson_stash_max_bytes(h->dj);
   return B200DD_OK;
@@ -539,9 +657,16 @@ int b200dd_pipeline_fetch_detection_json(b200dd_pipeline *h, uint64_t timestamp,
   if (!h->dj_stream) return arg_fail("b200dd_pipeline_fetch_detection_json: no CPI submitted since the stage was enabled");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)h->dj_stream;
+  ShareSet *s = h->set;
+  if (s && h->cpi < s->dj_last)
+    return arg_fail("b200dd_pipeline_fetch_detection_json: the share set's history has taken a later CPI");
   DetDeviceList l;
   int rc = det_device_list(h->det, &l);
   if (rc != B200DD_OK) return rc;
+  if (s) {
+    rc = set_wait(s, st);
+    if (rc != B200DD_OK) return rc;
+  }
   int fs = 0;
   uint32_t cfar = 0;
   if (h->last_had_filter) B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -557,7 +682,13 @@ int b200dd_pipeline_fetch_detection_json(b200dd_pipeline *h, uint64_t timestamp,
     set_last_error("b200dd_pipeline_fetch_detection_json: more CFAR detections than the list capacity (2^18)");
     return B200DD_ERR_CAPACITY;
   }
-  return b200dd_detjson_fetch(h->dj, timestamp, out, cap, n_bytes, st);
+  rc = b200dd_detjson_fetch(h->dj, timestamp, out, cap, n_bytes, st);
+  if (s) {
+    const int rr = set_record(s, st);
+    if (rr != B200DD_OK) return rr;
+    if (rc == B200DD_OK) s->dj_last = h->cpi;
+  }
+  return rc;
 }
 
 int b200dd_pipeline_fetch_detection_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes) {
@@ -565,12 +696,18 @@ int b200dd_pipeline_fetch_detection_stash(b200dd_pipeline *h, char *out, size_t 
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_detection_stash: null argument");
   if (!h->dj) return arg_fail("b200dd_pipeline_fetch_detection_stash: the detection JSON stage is not enabled");
   DeviceGuard guard(h->device);
-  return b200dd_detjson_fetch_stash(h->dj, out, cap, n_bytes, h->dj_stream ? h->dj_stream : (void *)h->stream);
+  void *st = h->dj_stream ? h->dj_stream : (void *)h->stream;
+  if (h->set) {
+    const int rc = set_wait(h->set, st);
+    if (rc != B200DD_OK) return rc;
+  }
+  return b200dd_detjson_fetch_stash(h->dj, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_enable_tracker(b200dd_pipeline *h, const b200dd_tracker_params *params, uint32_t max_tracks,
                                    uint32_t max_history, size_t *max_bytes) {
   if (!h || !params) return arg_fail("b200dd_pipeline_enable_tracker: null argument");
+  if (h->set) return arg_fail("b200dd_pipeline_enable_tracker: a share-set member's stateful stages are the set's");
   if (!h->p.detection_enable) return arg_fail("b200dd_pipeline_enable_tracker: detection is not enabled");
   b200dd_tracker_params tp = *params;
   tp.cpi = h->g.cpi;  // ambiguity->get_cpi(), blah2.cpp:195
@@ -583,17 +720,39 @@ int b200dd_pipeline_enable_tracker(b200dd_pipeline *h, const b200dd_tracker_para
   h->tr_pending = false;
   const int rc = b200dd_tracker_create(&tp, max_tracks, max_history, h->device, &h->tr);
   if (rc != B200DD_OK) return rc;
+  h->tr_params = tp;
+  h->tr_max_tracks = max_tracks;
+  h->tr_max_history = max_history;
   if (max_bytes) *max_bytes = b200dd_tracker_max_bytes(h->tr);
   return B200DD_OK;
 }
 
+static int track_json(b200dd_pipeline *h, b200dd_tracker *tr, uint64_t timestamp, char *out, size_t cap,
+                      size_t *n_bytes, cudaStream_t st);
+
 int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_track_json: null argument");
-  if (!h->tr) return arg_fail("b200dd_pipeline_fetch_track_json: the tracker stage is not enabled");
+  ShareSet *s = h->set;
+  b200dd_tracker *tr = s ? s->tr : h->tr;
+  if (!tr) return arg_fail("b200dd_pipeline_fetch_track_json: the tracker stage is not enabled");
   if (!h->tr_stream) return arg_fail("b200dd_pipeline_fetch_track_json: no CPI submitted since the stage was enabled");
+  if (s && h->unfetched) return arg_fail("b200dd_pipeline_fetch_track_json: the share-set member's CPI is not fetched yet");
+  if (s && h->cpi < s->tr_last) return arg_fail("b200dd_pipeline_fetch_track_json: the share set's tracker has taken a later CPI");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)h->tr_stream;
+  if (s) {
+    int rc = set_wait(s, st);
+    if (rc == B200DD_OK) rc = track_json(h, tr, timestamp, out, cap, n_bytes, st);
+    const int rr = set_record(s, st);
+    return rc != B200DD_OK ? rc : rr;
+  }
+  return track_json(h, tr, timestamp, out, cap, n_bytes, st);
+}
+
+// the tracker update of the last CPI, once, then the document
+static int track_json(b200dd_pipeline *h, b200dd_tracker *tr, uint64_t timestamp, char *out, size_t cap,
+                      size_t *n_bytes, cudaStream_t st) {
   if (h->tr_pending) {
     DetDeviceList l;
     int rc = det_device_list(h->det, &l);
@@ -611,16 +770,18 @@ int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, cha
       set_last_error("b200dd_pipeline_fetch_track_json: more CFAR detections than the list capacity (2^18)");
       return B200DD_ERR_CAPACITY;
     }
-    rc = b200dd_tracker_process_device(h->tr, l.delay, l.doppler, l.snr, l.count, timestamp, st);
+    rc = b200dd_tracker_process_device(tr, l.delay, l.doppler, l.snr, l.count, timestamp, st);
     if (rc != B200DD_OK) return rc;
     h->tr_pending = false;
+    if (h->set) h->set->tr_last = h->cpi;
   }
-  return b200dd_tracker_fetch(h->tr, timestamp, out, cap, n_bytes, st);
+  return b200dd_tracker_fetch(tr, timestamp, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double max, double mean, size_t *doc_bytes,
                                        size_t *stash_bytes) {
   if (!h) return arg_fail("b200dd_pipeline_enable_iqdata_json: null handle");
+  if (h->set) return arg_fail("b200dd_pipeline_enable_iqdata_json: a share-set member's stateful stages are the set's");
   if (!h->spec) return arg_fail("b200dd_pipeline_enable_iqdata_json: the spectrum stage is not enabled");
   DeviceGuard guard(h->device);
   B2_CUDA(cudaStreamSynchronize(h->stream));
@@ -630,18 +791,40 @@ int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double ma
   h->ij_stream = nullptr;
   const int rc = b200dd_iqjson_create(h->spec_bins, min, max, mean, h->device, &h->ij);
   if (rc != B200DD_OK) return rc;
+  h->ij_metrics[0] = min;
+  h->ij_metrics[1] = max;
+  h->ij_metrics[2] = mean;
   if (doc_bytes) *doc_bytes = b200dd_iqjson_max_bytes(h->ij);
   if (stash_bytes) *stash_bytes = b200dd_iqjson_stash_max_bytes(h->ij);
   return B200DD_OK;
 }
+
+// the last CPI's IQ-data document, committed to the history
+static int iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
+                       cudaStream_t st);
 
 int b200dd_pipeline_fetch_iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_iqdata_json: null argument");
   if (!h->ij) return arg_fail("b200dd_pipeline_fetch_iqdata_json: the IQ-data JSON stage is not enabled");
   if (!h->ij_stream) return arg_fail("b200dd_pipeline_fetch_iqdata_json: no CPI submitted since the stage was enabled");
+  ShareSet *s = h->set;
+  if (s && h->cpi < s->ij_last)
+    return arg_fail("b200dd_pipeline_fetch_iqdata_json: the share set's history has taken a later CPI");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)h->ij_stream;
+  if (s) {
+    int rc = set_wait(s, st);
+    if (rc == B200DD_OK) rc = iqdata_json(h, timestamp, out, cap, n_bytes, st);
+    const int rr = set_record(s, st);
+    if (rc == B200DD_OK) s->ij_last = h->cpi;
+    return rc != B200DD_OK ? rc : rr;
+  }
+  return iqdata_json(h, timestamp, out, cap, n_bytes, st);
+}
+
+static int iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
+                       cudaStream_t st) {
   if (h->last_had_filter) {
     int fs = 0;
     B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -660,7 +843,12 @@ int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_iqdata_stash: null argument");
   if (!h->ij) return arg_fail("b200dd_pipeline_fetch_iqdata_stash: the IQ-data JSON stage is not enabled");
   DeviceGuard guard(h->device);
-  return b200dd_iqjson_fetch_stash(h->ij, out, cap, n_bytes, h->ij_stream ? h->ij_stream : (void *)h->stream);
+  void *st = h->ij_stream ? h->ij_stream : (void *)h->stream;
+  if (h->set) {
+    const int rc = set_wait(h->set, st);
+    if (rc != B200DD_OK) return rc;
+  }
+  return b200dd_iqjson_fetch_stash(h->ij, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out,
@@ -670,6 +858,119 @@ int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const doub
   int rc = b200dd_pipeline_submit_host(h, x, y, n, map_out);
   if (rc != B200DD_OK) return rc;
   return b200dd_pipeline_fetch(h, result, o_delay, o_doppler, o_snr, cap, h->stream);
+}
+
+
+static bool same_params(const b200dd_pipeline *a, const b200dd_pipeline *b) {
+  const b200dd_caf_params &c = a->p.caf, &e = b->p.caf;  // devices compared as resolved at create
+  const b200dd_det_params &d = a->p.det, &f = b->p.det;
+  return c.delay_min == e.delay_min && c.delay_max == e.delay_max && c.doppler_min == e.doppler_min &&
+         c.doppler_max == e.doppler_max && c.fs == e.fs && c.n_samples == e.n_samples &&
+         c.round_hamming == e.round_hamming && a->p.clutter_enable == b->p.clutter_enable &&
+         a->p.clutter_delay_min == b->p.clutter_delay_min && a->p.clutter_delay_max == b->p.clutter_delay_max &&
+         a->p.detection_enable == b->p.detection_enable && d.pfa == f.pfa && d.n_guard == f.n_guard &&
+         d.n_train == f.n_train && d.min_delay == f.min_delay && d.min_doppler == f.min_doppler &&
+         d.n_centroid_delay == f.n_centroid_delay && d.n_centroid_doppler == f.n_centroid_doppler &&
+         d.resolution_doppler == f.resolution_doppler && d.interp_delay == f.interp_delay &&
+         d.interp_doppler == f.interp_doppler;
+}
+
+// the spectrum and the four stateful stages are enabled alike, with the same parameters
+static bool same_stages(const b200dd_pipeline *a, const b200dd_pipeline *b) {
+  if (!a->spec != !b->spec || !a->ij != !b->ij || !a->mh != !b->mh || !a->dj != !b->dj || !a->tr != !b->tr) return false;
+  if (a->spec && a->spec_bandwidth != b->spec_bandwidth) return false;
+  if (a->ij && (a->ij_metrics[0] != b->ij_metrics[0] || a->ij_metrics[1] != b->ij_metrics[1] ||
+                a->ij_metrics[2] != b->ij_metrics[2]))
+    return false;
+  if (a->dj && a->dj_max_held != b->dj_max_held) return false;
+  if (a->tr) {
+    const b200dd_tracker_params &t = a->tr_params, &u = b->tr_params;
+    if (t.m != u.m || t.n != u.n || t.n_delete != u.n_delete || t.cpi != u.cpi || t.max_acc_init != u.max_acc_init ||
+        t.fs != u.fs || t.fc != u.fc || a->tr_max_tracks != b->tr_max_tracks || a->tr_max_history != b->tr_max_history)
+      return false;
+  }
+  return true;
+}
+
+static void set_free(ShareSet *s) {
+  DeviceGuard guard(s->device);
+  b200dd_maxhold_destroy(s->mh);
+  b200dd_detjson_destroy(s->dj);
+  b200dd_iqjson_destroy(s->ij);
+  b200dd_tracker_destroy(s->tr);
+  if (s->ev) cudaEventDestroy(s->ev);
+  delete s;
+}
+
+// a member being destroyed leaves its set; the last one frees it (its stream is synchronised: nothing is in flight)
+static void set_leave(b200dd_pipeline *h) {
+  ShareSet *s = h->set;
+  if (!s) return;
+  h->set = nullptr;
+  s->members.erase(std::find(s->members.begin(), s->members.end(), h));
+  if (s->members.empty()) set_free(s);
+}
+
+int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
+  if (!members || n == 0) return arg_fail("b200dd_pipeline_share_history: no members");
+  for (uint32_t i = 0; i < n; i++) {
+    const b200dd_pipeline *m = members[i];
+    if (!m) return arg_fail("b200dd_pipeline_share_history: null member");
+    for (uint32_t j = 0; j < i; j++)
+      if (members[j] == m) return arg_fail("b200dd_pipeline_share_history: a pipeline is given twice");
+    if (m->set) return arg_fail("b200dd_pipeline_share_history: a pipeline is in a share set already");
+    if (m->device != members[0]->device) return arg_fail("b200dd_pipeline_share_history: members on different devices");
+    if (!same_params(m, members[0])) return arg_fail("b200dd_pipeline_share_history: the members' parameters differ");
+    if (!same_stages(m, members[0]))
+      return arg_fail("b200dd_pipeline_share_history: the members' spectrum or stateful stages differ");
+  }
+  b200dd_pipeline *h0 = members[0];
+  DeviceGuard guard(h0->device);
+  ShareSet *s = new (std::nothrow) ShareSet();
+  if (!s) return arg_fail("b200dd_pipeline_share_history: out of host memory");
+  s->device = h0->device;
+  auto body = [&]() -> int {
+    for (uint32_t i = 0; i < n; i++) B2_CUDA(cudaStreamSynchronize(members[i]->stream));
+    B2_CUDA(cudaEventCreateWithFlags(&s->ev, cudaEventDisableTiming));
+    int rc = B200DD_OK;
+    if (h0->mh)
+      rc = b200dd_maxhold_create(h0->g.n_doppler_bins, h0->g.n_delay_bins, h0->delay.data(), h0->doppler.data(),
+                                 h0->p.caf.fs, h0->device, &s->mh);
+    if (rc == B200DD_OK && h0->dj) rc = b200dd_detjson_create(h0->p.caf.fs, h0->dj_max_held, h0->device, &s->dj);
+    if (rc == B200DD_OK && h0->ij)
+      rc = b200dd_iqjson_create(h0->spec_bins, h0->ij_metrics[0], h0->ij_metrics[1], h0->ij_metrics[2], h0->device,
+                                &s->ij);
+    if (rc == B200DD_OK && h0->tr)
+      rc = b200dd_tracker_create(&h0->tr_params, h0->tr_max_tracks, h0->tr_max_history, h0->device, &s->tr);
+    return rc;
+  };
+  const int rc = body();
+  if (rc != B200DD_OK) {
+    set_free(s);
+    return rc;
+  }
+  // from here on the members change: each one's renders stage for the set's histories, its own window and tracker go
+  int first = B200DD_OK;  // only a CUDA error can fail here; every member joins all the same
+  for (uint32_t i = 0; i < n; i++) {
+    b200dd_pipeline *m = members[i];
+    int r = m->dj ? detjson_share(m->dj, s->dj) : B200DD_OK;
+    if (r == B200DD_OK && m->ij) r = iqjson_share(m->ij, s->ij);
+    if (first == B200DD_OK) first = r;
+    pipeline_drop_graphs(m);  // they record the window's push
+    b200dd_maxhold_destroy(m->mh);
+    m->mh = nullptr;
+    m->mh_stream = nullptr;
+    b200dd_tracker_destroy(m->tr);
+    m->tr = nullptr;
+    m->tr_stream = nullptr;
+    m->tr_pending = false;
+    m->dj_stream = m->ij_stream = nullptr;
+    m->cpi = -1;
+    m->unfetched = false;
+    m->set = s;
+    s->members.push_back(m);
+  }
+  return first;
 }
 
 }  // extern "C"

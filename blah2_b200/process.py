@@ -933,6 +933,18 @@ class Pipeline:
                                                                 C.byref(n)))
         return self._iqstash[:n.value].tobytes()
 
+    @staticmethod
+    def share_history(pipes):
+        """Makes the max-hold window, the detection and IQ-data histories and the tracker of ``pipes`` one object
+        (b200dd_pipeline_share_history), for pipelines used alternately: after every fetch their stash and track
+        documents are those of one pipeline given the same CPIs in submit order.  Each member then holds one unfetched
+        CPI at a time, fetch() follows submit order across the set, and a member's CPI enters the max-hold window at
+        its fetch().  The pipelines must have equal parameters and stages; the histories start empty.  Raises
+        B200ddError (ERR_ARG) otherwise."""
+        pipes = list(pipes)
+        arr = (C.c_void_p * max(len(pipes), 1))(*[p._h for p in pipes])
+        capi.check(capi.load().b200dd_pipeline_share_history(arr, len(pipes)))
+
     def fetch_spectrum(self):
         """Spectrum of the reference channel of the last submitted CPI (complex128, nSpectrum bins)."""
         out = np.empty(self.n_spectrum, dtype=np.complex128)

@@ -767,6 +767,34 @@ B200DD_API int b200dd_pipeline_fetch_iqdata_json(b200dd_pipeline *h, uint64_t ti
 /* The /stash/iqdata document of the pipeline's history (see b200dd_iqjson_fetch_stash). */
 B200DD_API int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes);
 
+/* Share set: makes the stateful stages of n pipelines -- the max-hold window, the detection and IQ-data histories
+ * and the tracker -- one object, so that pipelines used alternately (to overlap one CPI's transfers with another's
+ * kernels) keep blah2's "last 20 CPIs", "last 300 s" and "the tracker sees every CPI".  The set's CPIs are numbered
+ * in submit order across its members.  After every fetch, the /stash/map, /stash/detection, /stash/iqdata and track
+ * documents equal those of one unshared pipeline given the same CPIs one after another (fetching every product after
+ * every CPI).  Per-CPI products (fetch's results, the spectrum, the map, detection and IQ-data documents) stay per
+ * member.
+ *  - A member holds at most one unfetched CPI: submit (and prepare_device when it runs the chain, which is a CPI)
+ *    returns B200DD_ERR_ARG, nothing enqueued, while its last CPI is not fetched.
+ *  - b200dd_pipeline_fetch must follow submit order across the set: B200DD_ERR_ARG, nothing consumed, for any CPI
+ *    other than the oldest unfetched one.  A member's CPI enters the max-hold window at that fetch (an unshared
+ *    pipeline pushes it at submit): a CPI that is never fetched never enters the window.  Its float2 map buffer must
+ *    stay untouched until then.
+ *  - The histories take a CPI at its document fetch, the tracker at the first b200dd_pipeline_fetch_track_json after
+ *    b200dd_pipeline_fetch.  A product fetch for a CPI older than the one that product took last returns
+ *    B200DD_ERR_ARG and commits nothing; so does fetch_maxhold on any CPI but the window's last, and fetch_track_json
+ *    before the member's fetch.  B200DD_FILTER_FAILED, B200DD_ERR_NONFINITE and B200DD_ERR_CAPACITY commit nothing.
+ *  - The existing fetch entry points of any member read and commit the shared state.
+ * B200DD_ERR_ARG, nothing changed, when n is 0, a member is null, given twice or in a set already, the members sit on
+ * different devices, or their b200dd_pipeline_params, spectrum stages (enabled, bandwidth) or stateful stages
+ * (enabled, IQ-data min / max / mean, max_held, tracker params and limits) differ.  Histories start empty; the
+ * members' recorded graphs are dropped.  On a member, enabling a stateful stage returns B200DD_ERR_ARG, and so does
+ * b200dd_pipeline_enable_spectrum when the set keeps an IQ-data history (it would disable the member's IQ-data
+ * render); the map document and the spectrum stay per member.  Destroying a member leaves the set; the last one
+ * frees the shared state.  Every operation on the shared state is ordered after the previous one by a CUDA event,
+ * whichever member's stream it runs on; nothing synchronises the host beyond what each call already does. */
+B200DD_API int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n);
+
 /* ------------------------------------------------------------------------------------------------
  * Inter-GPU exchanges (one process per GPU, NCCL over NVLink / NVSwitch).  The reference has no
  * distributed code; these serve the two shardings of SURVEY.md s8(e): independent CPIs round-robin
