@@ -175,6 +175,14 @@ SIGNATURES = [
                                                      C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_iqdata_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_fetch_iqdata_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_enable_timing_json", C.c_int, [_VP, C.c_uint64, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_timing_json", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_fetch_timing_stash", C.c_int, [_VP, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_debug_timing_values", C.c_int, [_VP, C.POINTER(C.c_char_p), _VP, C.c_uint32,
+                                                      C.POINTER(C.c_uint32)]),
+    ("b200dd_timing_render_host", C.c_int, [C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(C.c_char_p), _VP,
+                                            C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("b200dd_timing_max_bytes", C.c_size_t, []),
     ("b200dd_pipeline_share_history", C.c_int, [_VP, C.c_uint32]),
     ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),

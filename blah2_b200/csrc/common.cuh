@@ -96,5 +96,21 @@ void iqjson_mark_rendered(b200dd_iqjson *h, bool rendered);
 // fetch copies the staged values into hist's ring and commits there; its stash fetch renders hist's.  Synchronous.
 int detjson_share(b200dd_detjson *h, b200dd_detjson *hist);
 int iqjson_share(b200dd_iqjson *h, b200dd_iqjson *hist);
+// timing.cu: enqueues one thread writing %globaltimer (ns) into *d_slot on `st`.
+int timing_stamp(uint64_t *d_slot, cudaStream_t st);
+// det.cu: b200dd_det_chain_device_async also stamps *d_slot (nullable) between set_metrics and CFAR.
+void det_set_metrics_stamp(b200dd_det *h, uint64_t *d_slot);
+// timing.cu: Timing's state (tStart, n) and the API's /stash/timing history.  timing_history_fetch writes the
+// document of the next CPI (nCpi = n + 1) and commits it: B200DD_ERR_CAPACITY, nothing written or committed, when
+// cap is too small; B200DD_ERR_ARG, written but not committed, when a value cannot enter the history exactly.
+struct TimingHistory;
+TimingHistory *timing_history_create(uint64_t t_start);
+void timing_history_destroy(TimingHistory *t);
+uint64_t timing_history_t_start(const TimingHistory *t);
+size_t timing_doc_max_bytes();
+size_t timing_stash_max_bytes();
+int timing_history_fetch(TimingHistory *t, uint64_t t_now, const char *const *names, const double *values,
+                         uint32_t count, char *out, size_t cap, size_t *n_bytes);
+int timing_history_stash(const TimingHistory *t, char *out, size_t cap, size_t *n_bytes);
 
 }  // namespace b2

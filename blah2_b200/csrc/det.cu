@@ -412,7 +412,10 @@ struct b200dd_det {
   std::vector<int32_t> axes_delay;   // host copies of what d_delay / d_doppler hold
   std::vector<double> axes_doppler;
   int chain_buf = 0, chain_slot = 0;  // where the last async chain left its results
+  uint64_t *metrics_stamp = nullptr;  // the pipeline's timing stamp between set_metrics and CFAR (nullable)
 };
+
+void b2::det_set_metrics_stamp(b200dd_det *h, uint64_t *d_slot) { h->metrics_stamp = d_slot; }
 
 namespace {
 
@@ -665,6 +668,10 @@ int b200dd_det_chain_device_async(b200dd_det *h, int last_stage, const void *d_m
   B2_LAUNCH_CHECK();
   metrics_final_kernel<<<1, kBlock, 0, st>>>(h->d_part, h->d_part + h->nPart, grid, (double)cells, h->d_metrics);
   B2_LAUNCH_CHECK();
+  if (h->metrics_stamp) {
+    rc = timing_stamp(h->metrics_stamp, st);
+    if (rc != B200DD_OK) return rc;
+  }
   if (last_stage == 0) {  // Map::set_metrics only (blah2.cpp:279 runs it whether or not detection is enabled)
     h->chain_buf = 0;
     h->chain_slot = -1;

@@ -1,7 +1,7 @@
 // pipeline.cu -- one CPI through WienerHopf -> Ambiguity -> set_metrics -> detection with all
 // intermediates resident in HBM (the body of the reference's process thread, src/blah2.cpp:268-287).
 // Composes the per-class handles of caf.cu / wh.cu / det.cu / spectrum.cu / iqjson.cu / mapjson.cu / maxhold.cu / detjson.cu /
-// tracker.cu through their C ABI; the only kernels
+// tracker.cu through their C ABI, and timing.cu's stamps and history; the only kernels
 // defined here are the complex128 <-> complex64 conversions of the host entry point.
 #include "common.cuh"
 
@@ -44,12 +44,30 @@ inline int grid_for(uint32_t n) {
   return b > 132 * 8 ? 132 * 8 : (b < 1 ? 1 : b);
 }
 
+// The timing stage's device stamps, one slot per stage boundary (timing.cu).  Each stage's time is its closing stamp
+// minus the stamp before it in the chain.
+enum TmSlot {
+  kTmExtract0,  // host submits: before the H2D copy
+  kTmChain,     // the device chain's first stamp; host submits: after the H2D copy
+  kTmSpectrum,  // after the spectrum kernels and the IQ-data render
+  kTmClutter,   // after the WienerHopf kernels
+  kTmNarrow,    // b200dd_pipeline_submit_host: after the complex128 -> complex64 conversion
+  kTmAmbiguity, // after CAF and set_metrics (det.cu, inside b200dd_det_chain_device_async)
+  kTmDetector,  // after CFAR -> Centroid -> Interpolate
+  kTmOutput,    // after the map document, the max-hold push and the detection document
+  kTmTracker0,  // around b200dd_tracker_process_device at the first track fetch
+  kTmTracker1,
+  kTmSlots
+};
+enum TmPath { kTmNone, kTmHost, kTmRspduo, kTmDevice };
+
 }  // namespace
 
 // The stateful stages of a share set (b200dd_pipeline_share_history): one max-hold window, one detection history,
-// one IQ-data history and one tracker for all members, each null when the members do not enable it.  Every
-// operation on them is enqueued on the stream of the member that makes it, after the set's event, and records the
-// event again: so they run in the order the host calls them, whatever streams the members use.
+// one IQ-data history, one tracker and one timing history for all members, each null when the members do not enable
+// it.  Every device operation on them is enqueued on the stream of the member that makes it, after the set's event,
+// and records the event again: so they run in the order the host calls them, whatever streams the members use.  The
+// timing history lives on the host and changes in that order too.
 struct ShareSet {
   int device = 0;
   std::vector<b200dd_pipeline *> members;
@@ -58,7 +76,8 @@ struct ShareSet {
   b200dd_detjson *dj = nullptr;
   b200dd_iqjson *ij = nullptr;
   b200dd_tracker *tr = nullptr;
-  int64_t mh_last = -1, dj_last = -1, ij_last = -1, tr_last = -1;  // the CPI each one took last
+  TimingHistory *tm = nullptr;  // host state: its commits need no event
+  int64_t mh_last = -1, dj_last = -1, ij_last = -1, tr_last = -1, tm_last = -1;  // the CPI each one took last
   cudaEvent_t ev = nullptr;
   bool ev_recorded = false;
 };
@@ -82,6 +101,21 @@ struct b200dd_pipeline {
   b200dd_tracker *tr = nullptr;     // optional: the tracker (blah2.cpp:291-296), run at fetch time
   void *tr_stream = nullptr;        // stream of the last submit
   bool tr_pending = false;          // the last submit's detections have not been given to the tracker yet
+  // optional: the timing document (blah2.cpp:331-345) from device stamps at the chain's stage boundaries, and its
+  // /stash/timing history (null for a share-set member: the set's)
+  bool tm_on = false;               // the submits enqueue stamps
+  TimingHistory *tm = nullptr;
+  uint64_t tm_t_start = 0;
+  uint64_t *d_tm = nullptr;         // the last submit's stamps, TmSlot
+  void *tm_stream = nullptr;        // ... enqueued on this stream
+  int tm_path = kTmNone;            // how the last submit came in
+  bool tm_spec = false;             // it ran the spectrum stage
+  bool tm_fetched = false;          // b200dd_pipeline_fetch took it ...
+  int tm_fs = 0;                    // ... and read this clutter-filter status
+  int tm_track = 0;                 // a track fetch ran the tracker on it (1, stamped) or skipped it (2, CFAR overflow)
+  bool tm_done = false;             // its document was committed
+  std::vector<const char *> tm_names;  // behind the last document written
+  std::vector<double> tm_values;
   uint32_t spec_bins = 0, spec_nfft = 0;
   b200dd_caf_geometry g;
   std::vector<int32_t> delay;
@@ -179,6 +213,8 @@ void b200dd_pipeline_destroy(b200dd_pipeline *h) {
     b200dd_maxhold_destroy(h->mh);
     b200dd_detjson_destroy(h->dj);
     b200dd_tracker_destroy(h->tr);
+    timing_history_destroy(h->tm);
+    free_dev(h->d_tm);
     free_dev(h->d_yf);
     free_dev(h->d_xd);
     free_dev(h->d_yd);
@@ -237,21 +273,50 @@ static int pipeline_enqueue_iqdata(b200dd_pipeline *h, void *st) {
   return b200dd_iqjson_render_device(h->ij, spectrum_device_output(h->spec), st);
 }
 
+// the timing stage's stamp closing the stage that ends at `slot`, on `st` (nothing when the stage is off)
+static int tm_stamp(b200dd_pipeline *h, int slot, void *st) {
+  return h->tm_on ? timing_stamp(h->d_tm + slot, (cudaStream_t)st) : B200DD_OK;
+}
+
+// after a submit: its stamps are the ones the next timing document reads
+static void tm_submitted(b200dd_pipeline *h, int path, void *st) {
+  if (!h->tm_on) return;
+  h->tm_path = path;
+  h->tm_stream = st;
+  h->tm_spec = h->spec != nullptr;
+  h->tm_fetched = h->tm_done = false;
+  h->tm_fs = 0;
+  h->tm_track = 0;
+}
+
+// the detection stage's closing stamp and the products after it, closed by the output stamp
+static int pipeline_enqueue_outputs(b200dd_pipeline *h, float2 *map, void *st) {
+  int rc = h->p.detection_enable ? tm_stamp(h, kTmDetector, st) : B200DD_OK;
+  if (rc == B200DD_OK) rc = pipeline_enqueue_products(h, map, st);
+  if (rc == B200DD_OK) rc = tm_stamp(h, kTmOutput, st);
+  return rc;
+}
+
 // the kernels of one CPI on device-resident IQ, enqueued on `st` (also what a graph capture records)
 static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map, void *st) {
   const void *y = d_y;
-  int rc;
+  int rc = tm_stamp(h, kTmChain, st);
+  if (rc != B200DD_OK) return rc;
   if (h->spec) {  // spectrumAnalyser->process(x), blah2.cpp:264, before the filter touches anything
     if (n < h->spec_nfft) return arg_fail("b200dd_pipeline_submit_device: the spectrum stage needs nfft samples");
     rc = b200dd_spectrum_process_device(h->spec, d_x, n, nullptr, st);
     if (rc != B200DD_OK) return rc;
     rc = pipeline_enqueue_iqdata(h, st);
     if (rc != B200DD_OK) return rc;
+    rc = tm_stamp(h, kTmSpectrum, st);
+    if (rc != B200DD_OK) return rc;
   }
   if (h->wh) {
     rc = b200dd_wh_process_device(h->wh, d_x, d_y, h->d_yf, st);  // failed solve -> y passes through
     if (rc != B200DD_OK) return rc;
     y = h->d_yf;
+    rc = tm_stamp(h, kTmClutter, st);
+    if (rc != B200DD_OK) return rc;
   }
   h->last_had_filter = h->wh != nullptr;
   float2 *map = d_map ? (float2 *)d_map : h->d_map;
@@ -262,7 +327,7 @@ static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const vo
   rc = b200dd_det_chain_device_async(h->det, last, map, h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(),
                                      h->doppler.data(), st);
   if (rc != B200DD_OK) return rc;
-  return pipeline_enqueue_products(h, map, st);
+  return pipeline_enqueue_outputs(h, map, st);
 }
 
 
@@ -328,7 +393,10 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   int rc = member_may_submit(h, "b200dd_pipeline_submit_device: the share-set member's last CPI is not fetched yet");
   if (rc != B200DD_OK) return rc;
   rc = pipeline_submit_device(h, d_x, d_y, n, d_map, stream);
-  if (rc == B200DD_OK) member_submitted(h, stream ? stream : (void *)h->stream, d_map);
+  if (rc == B200DD_OK) {
+    member_submitted(h, stream ? stream : (void *)h->stream, d_map);
+    tm_submitted(h, kTmDevice, stream ? stream : (void *)h->stream);
+  }
   return rc;
 }
 
@@ -346,6 +414,7 @@ int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const vo
     rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
     if (rc != B200DD_OK) return rc;
     member_submitted(h, st, d_map);
+    tm_submitted(h, kTmDevice, st);
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     if (cudaStreamBeginCapture((cudaStream_t)st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -419,6 +488,10 @@ int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double 
   double metrics[2] = {0.0, 0.0};
   uint32_t n = 0;
   const int rc = b200dd_det_chain_fetch(h->det, metrics, o_delay, o_doppler, o_snr, cap, &n, st);  // synchronises st
+  if (h->tm_path != kTmNone && (rc == B200DD_OK || rc == B200DD_ERR_CAPACITY)) {
+    h->tm_fetched = true;
+    h->tm_fs = fs;
+  }
   if (fs != 0) {
     // The reference skips the whole CPI when the Cholesky solve fails: `if (!filter->process(x, y)) continue;`
     // (blah2.cpp:270-273) -- no map, no metrics, no detections are published.  The kernels downstream of the
@@ -455,17 +528,25 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
     if (n < h->spec_nfft) return arg_fail("b200dd_pipeline_submit_host: the spectrum stage needs nfft samples");
     need_x = h->spec_nfft;
   }
+  rc = tm_stamp(h, kTmExtract0, st);
+  if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaMemcpyAsync(h->d_xd, x, sizeof(double2) * need_x, cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemcpyAsync(h->d_yd, y, sizeof(double2) * need, cudaMemcpyHostToDevice, st));
+  rc = tm_stamp(h, kTmChain, st);
+  if (rc != B200DD_OK) return rc;
   if (h->spec) {  // on the caller's doubles, unrounded
     rc = b200dd_spectrum_process_device_f64(h->spec, h->d_xd, need_x, nullptr, st);
     if (rc != B200DD_OK) return rc;
     rc = pipeline_enqueue_iqdata(h, st);
     if (rc != B200DD_OK) return rc;
+    rc = tm_stamp(h, kTmSpectrum, st);
+    if (rc != B200DD_OK) return rc;
   }
   if (h->wh) {
     // the filter sees the caller's complex128 samples unrounded (FP64 kernels, in place)
     rc = b200dd_wh_process_device_f64(h->wh, h->d_xd, h->d_yd, h->d_yd, st);
+    if (rc != B200DD_OK) return rc;
+    rc = tm_stamp(h, kTmClutter, st);
     if (rc != B200DD_OK) return rc;
   }
   h->last_had_filter = h->wh != nullptr;
@@ -473,12 +554,14 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   B2_LAUNCH_CHECK();
   pl_narrow_kernel<<<grid_for(need), 256, 0, st>>>(h->d_yd, h->d_yf2, need);
   B2_LAUNCH_CHECK();
+  rc = tm_stamp(h, kTmNarrow, st);
+  if (rc != B200DD_OK) return rc;
   rc = b200dd_caf_process_device(h->caf, h->d_xf, h->d_yf2, need, h->d_map, st);
   if (rc != B200DD_OK) return rc;
   rc = b200dd_det_chain_device_async(h->det, h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0, h->d_map,
                                      h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(), st);
   if (rc != B200DD_OK) return rc;
-  rc = pipeline_enqueue_products(h, h->d_map, st);
+  rc = pipeline_enqueue_outputs(h, h->d_map, st);
   if (rc != B200DD_OK) return rc;
   if (map_out) {
     const uint32_t cells = h->g.n_doppler_bins * h->g.n_delay_bins;
@@ -487,6 +570,7 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
     B2_CUDA(cudaMemcpyAsync(map_out, h->d_mapd, sizeof(double2) * cells, cudaMemcpyDeviceToHost, st));
   }
   member_submitted(h, st, h->d_map);
+  tm_submitted(h, kTmHost, st);
   return B200DD_OK;
 }
 
@@ -511,6 +595,8 @@ int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, ui
     }
   }
   if (map_out && !h->d_mapd) B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * (size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
+  rc = tm_stamp(h, kTmExtract0, st);  // the device chain's first stamp closes extract_buffer
+  if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaMemcpyAsync(h->d_iq16, iq, sizeof(short4) * need, cudaMemcpyHostToDevice, st));
   pl_ingest_rspduo_kernel<<<grid_for(need), 256, 0, st>>>(h->d_iq16, h->d_xf, h->d_yf2, need);
   B2_LAUNCH_CHECK();
@@ -525,6 +611,7 @@ int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, ui
     B2_CUDA(cudaMemcpyAsync(map_out, h->d_mapd, sizeof(double2) * cells, cudaMemcpyDeviceToHost, st));
   }
   member_submitted(h, st, h->d_map);
+  tm_submitted(h, kTmRspduo, st);
   return B200DD_OK;
 }
 
@@ -767,11 +854,17 @@ static int track_json(b200dd_pipeline *h, b200dd_tracker *tr, uint64_t timestamp
       return B200DD_FILTER_FAILED;
     }
     if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
+      if (h->tm_on) h->tm_track = 2;  // the tracker did not run: its time is 0
       set_last_error("b200dd_pipeline_fetch_track_json: more CFAR detections than the list capacity (2^18)");
       return B200DD_ERR_CAPACITY;
     }
+    rc = tm_stamp(h, kTmTracker0, st);
+    if (rc != B200DD_OK) return rc;
     rc = b200dd_tracker_process_device(tr, l.delay, l.doppler, l.snr, l.count, timestamp, st);
     if (rc != B200DD_OK) return rc;
+    rc = tm_stamp(h, kTmTracker1, st);
+    if (rc != B200DD_OK) return rc;
+    if (h->tm_on) h->tm_track = 1;
     h->tr_pending = false;
     if (h->set) h->set->tr_last = h->cpi;
   }
@@ -851,6 +944,129 @@ int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap
   return b200dd_iqjson_fetch_stash(h->ij, out, cap, n_bytes, st);
 }
 
+int b200dd_pipeline_enable_timing_json(b200dd_pipeline *h, uint64_t t_start, size_t *doc_bytes, size_t *stash_bytes) {
+  if (!h) return arg_fail("b200dd_pipeline_enable_timing_json: null handle");
+  if (h->set) return arg_fail("b200dd_pipeline_enable_timing_json: a share-set member's stateful stages are the set's");
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  pipeline_drop_graphs(h);  // the chain changes
+  if (!h->d_tm) {
+    B2_CUDA(cudaMalloc(&h->d_tm, sizeof(uint64_t) * kTmSlots));
+    B2_CUDA(cudaMemset(h->d_tm, 0, sizeof(uint64_t) * kTmSlots));
+  }
+  TimingHistory *t = timing_history_create(t_start);
+  if (!t) return arg_fail("b200dd_pipeline_enable_timing_json: out of host memory");
+  timing_history_destroy(h->tm);
+  h->tm = t;
+  h->tm_t_start = t_start;
+  h->tm_on = true;
+  h->tm_path = kTmNone;
+  h->tm_names.clear();
+  h->tm_values.clear();
+  det_set_metrics_stamp(h->det, h->d_tm + kTmAmbiguity);
+  if (doc_bytes) *doc_bytes = timing_doc_max_bytes();
+  if (stash_bytes) *stash_bytes = timing_stash_max_bytes();
+  return B200DD_OK;
+}
+
+// blah2's stage names and values of the last submit (blah2.cpp:251-338), from its device stamps
+static void timing_values(b200dd_pipeline *h, const uint64_t *t, bool tracker) {
+  auto ms = [](uint64_t to, uint64_t from) { return (double)(int64_t)(to - from) / 1e6; };
+  h->tm_names.clear();
+  h->tm_values.clear();
+  auto put = [&](const char *name, double v) {
+    h->tm_names.push_back(name);
+    h->tm_values.push_back(v);
+  };
+  const bool host = h->tm_path == kTmHost;
+  const uint64_t first = h->tm_path == kTmDevice ? t[kTmChain] : t[kTmExtract0];
+  uint64_t prev = t[kTmChain];
+  double extract = h->tm_path == kTmDevice ? 0.0 : ms(t[kTmChain], t[kTmExtract0]);
+  double spectrum = 0.0, clutter = 0.0;
+  if (h->tm_spec) {
+    spectrum = ms(t[kTmSpectrum], prev);
+    prev = t[kTmSpectrum];
+  }
+  if (h->wh) {
+    clutter = ms(t[kTmClutter], prev);
+    prev = t[kTmClutter];
+  }
+  if (host) {  // the conversion to complex64 runs after the filter here: it counts as extract_buffer
+    extract += ms(t[kTmNarrow], prev);
+    prev = t[kTmNarrow];
+  }
+  put("extract_buffer", extract);
+  if (h->tm_spec) put("spectrum", spectrum);
+  if (h->wh) put("clutter_filter", clutter);
+  put("ambiguity_processing", ms(t[kTmAmbiguity], prev));
+  prev = t[kTmAmbiguity];
+  if (h->p.detection_enable) {
+    put("detector", ms(t[kTmDetector], prev));
+    prev = t[kTmDetector];
+  }
+  const double track = h->tm_track == 1 ? ms(t[kTmTracker1], t[kTmTracker0]) : 0.0;
+  if (tracker) put("tracker", track);
+  put("output_radar_data", ms(t[kTmOutput], prev));
+  put("cpi", ms(t[kTmOutput], first) + track);
+}
+
+int b200dd_pipeline_fetch_timing_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_timing_json: null argument");
+  ShareSet *s = h->set;
+  TimingHistory *tm = s ? s->tm : h->tm;
+  if (!h->tm_on || !tm) return arg_fail("b200dd_pipeline_fetch_timing_json: the timing JSON stage is not enabled");
+  if (h->tm_path == kTmNone) return arg_fail("b200dd_pipeline_fetch_timing_json: no CPI submitted since the stage was enabled");
+  if (!h->tm_fetched) return arg_fail("b200dd_pipeline_fetch_timing_json: call after the CPI's b200dd_pipeline_fetch");
+  if (h->tm_done) return arg_fail("b200dd_pipeline_fetch_timing_json: the CPI's document was fetched already");
+  if (h->tm_fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273) skips Timing::update
+    set_last_error("b200dd_pipeline_fetch_timing_json: the CPI's clutter-filter solve failed; it has no document");
+    return B200DD_FILTER_FAILED;
+  }
+  const bool tracker = (s ? s->tr : h->tr) != nullptr;
+  if (tracker && h->tm_track == 0)
+    return arg_fail("b200dd_pipeline_fetch_timing_json: with the tracker enabled, call after the CPI's track fetch");
+  if (s && h->cpi < s->tm_last)
+    return arg_fail("b200dd_pipeline_fetch_timing_json: the share set's history has taken a later CPI");
+  DeviceGuard guard(h->device);
+  uint64_t t[kTmSlots];
+  B2_CUDA(cudaMemcpyAsync(t, h->d_tm, sizeof(t), cudaMemcpyDeviceToHost, (cudaStream_t)h->tm_stream));
+  B2_CUDA(cudaStreamSynchronize((cudaStream_t)h->tm_stream));
+  timing_values(h, t, tracker);
+  const int rc = timing_history_fetch(tm, timestamp, h->tm_names.data(), h->tm_values.data(),
+                                      (uint32_t)h->tm_names.size(), out, cap, n_bytes);
+  if (rc == B200DD_OK) {
+    h->tm_done = true;
+    if (s) s->tm_last = h->cpi;
+  }
+  return rc;
+}
+
+int b200dd_pipeline_fetch_timing_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_timing_stash: null argument");
+  const TimingHistory *tm = h->set ? h->set->tm : h->tm;
+  if (!h->tm_on || !tm) return arg_fail("b200dd_pipeline_fetch_timing_stash: the timing JSON stage is not enabled");
+  return timing_history_stash(tm, out, cap, n_bytes);
+}
+
+int b200dd_pipeline_debug_timing_values(b200dd_pipeline *h, const char **names, double *values, uint32_t cap,
+                                        uint32_t *count) {
+  if (count) *count = 0;
+  if (!h || !count || (cap && (!names || !values))) return arg_fail("b200dd_pipeline_debug_timing_values: null argument");
+  if (h->tm_names.empty()) return arg_fail("b200dd_pipeline_debug_timing_values: no timing document written yet");
+  *count = (uint32_t)h->tm_names.size();
+  if (cap < *count) {
+    set_last_error("b200dd_pipeline_debug_timing_values: capacity too small");
+    return B200DD_ERR_CAPACITY;
+  }
+  for (uint32_t i = 0; i < *count; i++) {
+    names[i] = h->tm_names[i];
+    values[i] = h->tm_values[i];
+  }
+  return B200DD_OK;
+}
+
 int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out,
                                  b200dd_cpi_result *result, double *o_delay, double *o_doppler, double *o_snr,
                                  uint32_t cap) {
@@ -883,6 +1099,7 @@ static bool same_stages(const b200dd_pipeline *a, const b200dd_pipeline *b) {
                 a->ij_metrics[2] != b->ij_metrics[2]))
     return false;
   if (a->dj && a->dj_max_held != b->dj_max_held) return false;
+  if (a->tm_on != b->tm_on || (a->tm_on && a->tm_t_start != b->tm_t_start)) return false;
   if (a->tr) {
     const b200dd_tracker_params &t = a->tr_params, &u = b->tr_params;
     if (t.m != u.m || t.n != u.n || t.n_delete != u.n_delete || t.cpi != u.cpi || t.max_acc_init != u.max_acc_init ||
@@ -898,6 +1115,7 @@ static void set_free(ShareSet *s) {
   b200dd_detjson_destroy(s->dj);
   b200dd_iqjson_destroy(s->ij);
   b200dd_tracker_destroy(s->tr);
+  timing_history_destroy(s->tm);
   if (s->ev) cudaEventDestroy(s->ev);
   delete s;
 }
@@ -942,6 +1160,8 @@ int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
                                 &s->ij);
     if (rc == B200DD_OK && h0->tr)
       rc = b200dd_tracker_create(&h0->tr_params, h0->tr_max_tracks, h0->tr_max_history, h0->device, &s->tr);
+    if (rc == B200DD_OK && h0->tm_on && !(s->tm = timing_history_create(h0->tm_t_start)))
+      rc = arg_fail("b200dd_pipeline_share_history: out of host memory");
     return rc;
   };
   const int rc = body();
@@ -964,6 +1184,9 @@ int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
     m->tr = nullptr;
     m->tr_stream = nullptr;
     m->tr_pending = false;
+    timing_history_destroy(m->tm);
+    m->tm = nullptr;
+    m->tm_path = kTmNone;
     m->dj_stream = m->ij_stream = nullptr;
     m->cpi = -1;
     m->unfetched = false;

@@ -722,6 +722,21 @@ class IqDataJson:
             pass
 
 
+def timing_render_host(t_start, t_now, n, names, values) -> bytes:
+    """blah2's Timing(t_start), update(t_now, values, names) after n - 1 earlier updates, then to_json(), on the CPU
+    (b200dd_timing_render_host).  Raises B200ddError (ERR_ARG) for a name written unescaped or a non-finite value."""
+    lib = capi.load()
+    v = np.ascontiguousarray(np.asarray(values, dtype=np.float64).ravel())
+    if len(names) != v.size:
+        raise ValueError("names and values differ in length")
+    arr = (C.c_char_p * max(v.size, 1))(*[s.encode() if isinstance(s, str) else s for s in names])
+    out = np.empty(int(lib.b200dd_timing_max_bytes()), dtype=np.uint8)
+    nb = C.c_size_t()
+    capi.check(lib.b200dd_timing_render_host(int(t_start), int(t_now), int(n), arr, capi.ptr(v), v.size,
+                                             capi.ptr(out), out.size, C.byref(nb)))
+    return out[:nb.value].tobytes()
+
+
 def _fetch_growing(buf, call):
     """call(buf) -> (rc, n_bytes); a too-small buffer is grown to the reported size and the call repeated."""
     rc, n = call(buf)
@@ -932,6 +947,42 @@ class Pipeline:
         capi.check(self._lib.b200dd_pipeline_fetch_iqdata_stash(self._h, capi.ptr(self._iqstash), self._iqstash.size,
                                                                 C.byref(n)))
         return self._iqstash[:n.value].tobytes()
+
+    def enable_timing_json(self, t_start):
+        """Stamps every CPI submitted from now on at its stage boundaries on the device and builds blah2's timing
+        document (blah2.cpp:331-345) from those stamps; keeps the /stash/timing history of the last 20 committed
+        documents.  ``t_start`` is Timing's tStart (POSIX ms); nCpi and the history start at 0 and empty."""
+        db, sb = C.c_size_t(), C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_enable_timing_json(self._h, int(t_start), C.byref(db), C.byref(sb)))
+        self.timing_json_max_bytes, self.timing_stash_max_bytes = int(db.value), int(sb.value)
+        self._tmjson = np.empty(self.timing_json_max_bytes, dtype=np.uint8)
+        self._tmstash = np.empty(self.timing_stash_max_bytes, dtype=np.uint8)
+
+    def fetch_timing_json(self, timestamp) -> bytes:
+        """The timing document of the last fetched CPI with tNow = ``timestamp`` (call after fetch() and, with the
+        tracker, after fetch_track_json()), committed to the /stash/timing history.  Raises B200ddError with code
+        FILTER_FAILED when that CPI's clutter-filter solve failed (nothing is sent, nCpi and the history are
+        unchanged), ERR_ARG when called too early or twice, or when a value has more than 15 significant digits (the
+        document is then written but not committed; ``last_timing_doc`` holds it)."""
+        n = C.c_size_t()
+        rc = self._lib.b200dd_pipeline_fetch_timing_json(self._h, int(timestamp), capi.ptr(self._tmjson),
+                                                         self._tmjson.size, C.byref(n))
+        self.last_timing_doc = self._tmjson[:n.value].tobytes()
+        capi.check(rc)
+        return self.last_timing_doc
+
+    def fetch_timing_stash(self) -> bytes:
+        """The /stash/timing document of the documents committed so far."""
+        n = C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_fetch_timing_stash(self._h, capi.ptr(self._tmstash), self._tmstash.size,
+                                                                C.byref(n)))
+        return self._tmstash[:n.value].tobytes()
+
+    def timing_values(self):
+        """The stage names and times (ms) behind the last timing document written (a test aid)."""
+        names, values, count = (C.c_char_p * 16)(), np.empty(16, dtype=np.float64), C.c_uint32()
+        capi.check(self._lib.b200dd_pipeline_debug_timing_values(self._h, names, capi.ptr(values), 16, C.byref(count)))
+        return [names[i].decode() for i in range(count.value)], values[:count.value].copy()
 
     @staticmethod
     def share_history(pipes):

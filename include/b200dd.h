@@ -561,6 +561,24 @@ B200DD_API int b200dd_iqjson_render_host(const double *spectrum, uint32_t n, dou
  * memory).  Asynchronous on `stream`. */
 B200DD_API int b200dd_iqjson_debug_bin_values(b200dd_iqjson *h, const void *d_spectrum, void *d_out, void *stream);
 
+/* ------------------------------------------------------------------ timing JSON
+ *
+ * The document blah2 sends on its timing socket after every CPI (src/blah2.cpp:331-345, Timing::to_json in
+ * src/data/meta/Timing.cpp), byte for byte:
+ *   {"timestamp":T,"nCpi":n,"uptime_s":u/1000.0,"uptime_days":u/1000.0/60/60/24,"<stage>":ms,...}
+ * T = t_now, n and u = t_now - t_start (uint64, wrapping when t_now < t_start) are written as integers / doubles by
+ * rapidjson's Writer at two decimal places; each stage is a name and a time in ms.  In the pipeline (see
+ * b200dd_pipeline_enable_timing_json) the times come from device stamps at the chain's stage boundaries.
+ */
+/* The document of `count` (<= 16) stages, without a handle or a device.  B200DD_ERR_ARG: a null pointer, a name
+ * that is null, 64 bytes or longer or not printable ASCII without '"' and '\\' (names are written unescaped), or a
+ * non-finite time (the Writer has no text for it).  B200DD_ERR_CAPACITY: cap < *n_bytes. */
+B200DD_API int b200dd_timing_render_host(uint64_t t_start, uint64_t t_now, uint64_t n, const char *const *names,
+                                         const double *values, uint32_t count, char *out, size_t cap,
+                                         size_t *n_bytes);
+/* Upper bound of a timing document's size in bytes (16 stages of 63-byte names). */
+B200DD_API size_t b200dd_timing_max_bytes(void);
+
 /* ------------------------------------------------------------------ tracker
  *
  * Tracker::process + Track::to_json (src/process/tracker/Tracker.cpp, src/data/Track.cpp; blah2.cpp:291-296 and
@@ -767,6 +785,44 @@ B200DD_API int b200dd_pipeline_fetch_iqdata_json(b200dd_pipeline *h, uint64_t ti
 /* The /stash/iqdata document of the pipeline's history (see b200dd_iqjson_fetch_stash). */
 B200DD_API int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes);
 
+/* Optional stage (src/blah2.cpp:251-345): every CPI submitted afterwards stamps %globaltimer on the device at its
+ * stage boundaries, on the submit stream (so recorded graphs stamp too), and its timing document (see
+ * b200dd_timing_render_host) is built from those stamps; the API's /stash/timing history is kept.  Timing(t_start):
+ * enabling resets nCpi and the history and drops the graphs recorded so far.  Stages, in blah2's order and under
+ * blah2's conditions, each the time between two device stamps in ms (ns / 1e6):
+ *   extract_buffer        host submits: the H2D copy plus the conversion to complex64 (for b200dd_pipeline_submit_host
+ *                         that conversion runs after the filter); device submits: 0
+ *   spectrum              the spectrum kernels and the IQ-data render (when the spectrum stage is enabled)
+ *   clutter_filter        the WienerHopf kernels (when the clutter filter is enabled)
+ *   ambiguity_processing  CAF and set_metrics
+ *   detector              CFAR -> Centroid -> Interpolate (when detection is enabled)
+ *   tracker               the tracker run at the CPI's first track fetch (when the tracker is enabled; 0 when CFAR
+ *                         overflowed and the tracker skipped the CPI)
+ *   output_radar_data     the map document, the max-hold push and the detection document enqueued after detection
+ *   cpi                   the CPI's first stamp to its last, plus tracker
+ * *doc_bytes / *stash_bytes (nullable) = the two documents' size bounds.  With the stage off nothing is stamped. */
+B200DD_API int b200dd_pipeline_enable_timing_json(b200dd_pipeline *h, uint64_t t_start, size_t *doc_bytes,
+                                                  size_t *stash_bytes);
+/* Called after b200dd_pipeline_fetch (and, when the tracker is enabled, after the CPI's track fetch): writes the
+ * last CPI's timing document with t_now = timestamp and commits it -- nCpi steps and the history takes it.  Each CPI
+ * is committed once.  B200DD_ERR_ARG, nothing written or committed: called too early, or again.
+ * B200DD_FILTER_FAILED, nothing written or committed: the CPI's clutter-filter solve failed (blah2.cpp:270-273 skips
+ * Timing::update).  A CFAR overflow does not stop the document.  B200DD_ERR_CAPACITY: cap < *n_bytes, nothing
+ * written or committed.  The history holds every value as int64 hundredths: a value whose text has more than 15
+ * significant digits (a wrapped uptime, a timestamp of 10^15 ms or more) cannot enter it exactly, so the document is
+ * written and B200DD_ERR_ARG returned, nothing committed. */
+B200DD_API int b200dd_pipeline_fetch_timing_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
+                                                 size_t *n_bytes);
+/* The /stash/timing document (api/stash/timing.js, api/server.js:105-106): JSON.stringify of an object holding, for
+ * every key of the committed documents but "uptime" and "nCpi", the array of its last 20 values (keys in first-seen
+ * order, numbers as Number::toString); "{}" before the first document.  B200DD_ERR_CAPACITY: cap < *n_bytes. */
+B200DD_API int b200dd_pipeline_fetch_timing_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes);
+/* Test entry point: the stage names (static strings) and times behind the last timing document written into
+ * names[cap] / values[cap]; *count = their number.  B200DD_ERR_ARG: no document yet.  B200DD_ERR_CAPACITY: cap <
+ * *count. */
+B200DD_API int b200dd_pipeline_debug_timing_values(b200dd_pipeline *h, const char **names, double *values,
+                                                   uint32_t cap, uint32_t *count);
+
 /* Share set: makes the stateful stages of n pipelines -- the max-hold window, the detection and IQ-data histories
  * and the tracker -- one object, so that pipelines used alternately (to overlap one CPI's transfers with another's
  * kernels) keep blah2's "last 20 CPIs", "last 300 s" and "the tracker sees every CPI".  The set's CPIs are numbered
@@ -792,7 +848,9 @@ B200DD_API int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out,
  * b200dd_pipeline_enable_spectrum when the set keeps an IQ-data history (it would disable the member's IQ-data
  * render); the map document and the spectrum stay per member.  Destroying a member leaves the set; the last one
  * frees the shared state.  Every operation on the shared state is ordered after the previous one by a CUDA event,
- * whichever member's stream it runs on; nothing synchronises the host beyond what each call already does. */
+ * whichever member's stream it runs on; nothing synchronises the host beyond what each call already does.
+ * The timing stage, when enabled alike with the same t_start, shares one Timing (nCpi, uptime) and one /stash/timing
+ * history; its stamps stay per member, and its documents follow the same commit rule as the histories. */
 B200DD_API int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n);
 
 /* ------------------------------------------------------------------------------------------------
