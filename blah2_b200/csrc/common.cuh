@@ -41,6 +41,16 @@ inline int geom_fail(const std::string &msg) {
   set_last_error(msg);
   return B200DD_ERR_GEOMETRY;
 }
+inline int nonfinite_fail(const char *msg) {
+  set_last_error(msg);
+  return B200DD_ERR_NONFINITE;
+}
+
+// element i of a complex map of float2 or double2, widened to double2
+template <class TMAP> __device__ __forceinline__ double2 ld_cell(const TMAP *m, size_t i) {
+  const TMAP v = m[i];
+  return make_double2((double)v.x, (double)v.y);
+}
 
 // RAII device switch (handles remember their device; callers may sit on another one)
 struct DeviceGuard {
@@ -70,8 +80,20 @@ int mapjson_enqueue_with_metrics(b200dd_mapjson *h, const void *d_map, const dou
 // time; the CPI is rejected with B200DD_FILTER_FAILED when *d_filter_status (nullable) is non-zero.
 int maxhold_enqueue_with_metrics(b200dd_maxhold *h, const void *d_map, const double *d_metrics,
                                  const int *d_filter_status, cudaStream_t st);
-// maxhold.cu: ECMAScript Number::toString (radix 10) of a finite double, as JSON.stringify prints numbers.
+// jsontext.cu: ECMAScript Number::toString (radix 10) of a finite double, as JSON.stringify prints numbers.
 std::string js_number_text(double d);
+// jsontext.cu: the text of v as a document carries it: rapidjson's Writer text (written once, jf::fmt_double), or
+// with `twice` that text read back and written again (jf::fmt_double_twice); with `reprint`, JSON.stringify of what
+// JSON.parse reads from that text, as the API's stashes serve it.  False when v has no text.
+bool number_text(double v, bool twice, bool reprint, std::string &out);
+// jsontext.cu: "[a,b,..]" of number_text of v[0..n); false when a value has no text.
+bool numbers_text(const double *v, size_t n, bool twice, bool reprint, std::string &out);
+// jsontext.cu: writes a fetched document into out: head, then each of n_sec sections -- its heading (headings null:
+// none) and its bytes, which lie back to back in the device body d_body and end at ends[i] -- then "]}", which closes
+// the last section's array and the document; with no sections, head alone.  *n_bytes = the document's size.
+// B200DD_ERR_CAPACITY with cap_msg, nothing written, when that exceeds cap.  Synchronises st after the copies.
+int write_document(const std::string &head, int n_sec, const char *const *headings, const uint32_t *ends,
+                   const char *d_body, char *out, size_t cap, size_t *n_bytes, const char *cap_msg, cudaStream_t st);
 // det.cu: the detection list the last async chain left, the one b200dd_det_chain_fetch reads: its three device
 // arrays, the device word holding its length, the device word holding CFAR's count (the list is invalid when that
 // exceeds cap) and the list capacity.  B200DD_ERR_ARG when that chain ran no detection stage.

@@ -36,11 +36,6 @@ namespace {
 constexpr int kBlock = 256;
 constexpr uint32_t kMaxDetections = 1u << 18;
 
-template <class TMAP> __device__ __forceinline__ double2 ld_cell(const TMAP *m, size_t i) {
-  TMAP v = m[i];
-  return make_double2((double)v.x, (double)v.y);
-}
-
 // 10 log10 |z|  (Map.cpp:198, CfarDetector1D.cpp:48, Interpolate.cpp:50)
 __device__ __forceinline__ double db_abs(double2 z) { return 10.0 * log10(hypot(z.x, z.y)); }
 

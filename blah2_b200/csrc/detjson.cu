@@ -16,14 +16,14 @@
 //   dj_len_kernel    formats each value with its separator, counts each tile's bytes, and writes the value's sent
 //                    hundredths to the ring position the stash will hold it at;
 //   scan_kernel      turns the tile counts of the three arrays into offsets in one body;
-//   dj_write_kernel  formats again, stages each tile at its 16-byte phase and stores it aligned (mapjson.cu).
+//   dj_write_kernel  formats again and stores each tile (text_tiles.cuh).
 // The fetch composes the document around the three sections on the host, then commits the CPI's entries to the
 // stash with the timestamp and prunes as detection.js does.  The per-document records (timestamp, first entry,
 // count) stay on the host; the stash fetch renders the four arrays with the same three-kernel pattern, with the
 // timestamp texts made on the host once per document.
 #include "common.cuh"
 #include "json_fmt.cuh"
-#include "scan.cuh"
+#include "text_tiles.cuh"
 
 #include <math.h>
 
@@ -38,9 +38,8 @@ using namespace b2;
 namespace {
 
 constexpr uint32_t kListCap = 1u << 18;  // the detection lists' capacity (det.cu)
-constexpr int kThreads = 256;
 constexpr int kRounds = 4;
-constexpr int kTile = kThreads * kRounds;
+constexpr int kTile = kTextThreads * kRounds;
 constexpr uint32_t kDocTiles = kListCap / kTile;  // per array
 constexpr int kDocItemMax = jf::kMaxText + 1;     // "," before the value
 constexpr int kTsText = 20;                        // Number::toString of a uint64 as a double: "18446744073709552000"
@@ -98,7 +97,7 @@ __device__ __forceinline__ int doc_item(const DocArgs &a, int arr, uint32_t j, c
 
 // __maxnreg__(64): at ptxas's own choice of 32 registers the formatting spills here
 __global__ void __maxnreg__(64) dj_len_kernel(DocArgs a) {
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const int arr = blockIdx.y;
   const uint32_t tile = arr * kDocTiles + blockIdx.x;
   const uint32_t raw = *a.count, n = raw < kListCap ? raw : kListCap;
@@ -114,9 +113,9 @@ __global__ void __maxnreg__(64) dj_len_kernel(DocArgs a) {
   char t[kDocItemMax];
   bool bad = false, range = false;
   uint32_t sum = 0;
-#pragma unroll 1
+#pragma unroll 1  // count_tile's unrolled loop takes more registers here
   for (int r = 0; r < kRounds; r++) {
-    const uint32_t j = base + r * kThreads + threadIdx.x;
+    const uint32_t j = base + r * kTextThreads + threadIdx.x;
     if (j >= n) continue;
     int vlen;
     sum += (uint32_t)doc_item(a, arr, j, t, &vlen);
@@ -131,44 +130,19 @@ __global__ void __maxnreg__(64) dj_len_kernel(DocArgs a) {
   }
   if (bad) a.info->nonfinite = 1u;  // every writer stores the same value
   if (range) a.info->range = 1u;
-  uint32_t tot;
-  block_excl_scan<kThreads>(sum, wsum, tot);
-  if (threadIdx.x == 0) a.tile_len[tile] = tot;
+  store_tile_len(a.tile_len, tile, wsum, sum);
 }
 
-// Stages a tile's texts at the 16-byte phase of its offset and stores them aligned (mapjson.cu: mj_write_kernel).
-template <int ITEM_MAX, class F>
-__device__ __forceinline__ void write_tile(uint32_t off, char *body, char *stage, uint32_t *wsum, F item) {
-  const uint32_t phase = off & 15u;  // stage[phase + i] <-> body[off + i]: same address mod 16
-  char t[ITEM_MAX];
-  uint32_t pos = phase;
-  for (int r = 0; r < kRounds; r++) {
-    const int n = item(r, t);
-    uint32_t tot;
-    const uint32_t ex = block_excl_scan<kThreads>((uint32_t)n, wsum, tot);
-    for (int i = 0; i < n; i++) stage[pos + ex + i] = t[i];
-    pos += tot;
-  }
-  __syncthreads();
-  const uint32_t g0 = off, g1 = off + (pos - phase);
-  uint32_t a0 = (g0 + 15u) & ~15u, a1 = g1 & ~15u;
-  if (a0 > g1) a0 = g1;
-  if (a1 < a0) a1 = a0;
-  for (uint32_t g = g0 + threadIdx.x; g < a0; g += kThreads) body[g] = stage[g - off + phase];
-  for (uint32_t g = a1 + threadIdx.x; g < g1; g += kThreads) body[g] = stage[g - off + phase];
-  for (uint32_t g = a0 + 16u * threadIdx.x; g < a1; g += 16u * kThreads)
-    *reinterpret_cast<uint4 *>(body + g) = *reinterpret_cast<const uint4 *>(stage + (g - off + phase));
-}
-
-__global__ void __launch_bounds__(kThreads) dj_write_kernel(DocArgs a) {
+__global__ void __launch_bounds__(kTextThreads) dj_write_kernel(DocArgs a) {
   __shared__ __align__(16) char stage[kTile * kDocItemMax + 16];
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const int arr = blockIdx.y;
   const uint32_t raw = *a.count, n = raw < kListCap ? raw : kListCap;
   const uint32_t base = blockIdx.x * kTile;
   if (base >= n) return;
-  write_tile<kDocItemMax>(a.tile_off[arr * kDocTiles + blockIdx.x], a.body, stage, wsum, [&](int r, char *t) {
-    const uint32_t j = base + r * kThreads + threadIdx.x;
+  const uint32_t off = a.tile_off[arr * kDocTiles + blockIdx.x];
+  write_tile<kDocItemMax, kRounds>(off, a.body, stage, wsum, [&](int r, char *t) {
+    const uint32_t j = base + r * kTextThreads + threadIdx.x;
     if (j >= n) return 0;
     int vlen;
     return doc_item(a, arr, j, t, &vlen);
@@ -217,35 +191,25 @@ __device__ __forceinline__ int stash_item(const StashArgs &a, int arr, uint32_t 
   return n + jf::fmt_hundredths(a.ring[(size_t)(arr - 1) * a.ring_cap + slot], t + n);
 }
 
-__global__ void __launch_bounds__(kThreads) ds_len_kernel(StashArgs a) {
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+__global__ void __launch_bounds__(kTextThreads) ds_len_kernel(StashArgs a) {
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const int arr = blockIdx.y;
   const uint32_t base = blockIdx.x * kTile;
   char t[kStashItemMax];
-  uint32_t sum = 0;
-  for (int r = 0; r < kRounds; r++) {
-    const uint32_t e = base + r * kThreads + threadIdx.x;
-    if (e < a.held) sum += (uint32_t)stash_item(a, arr, e, t);
-  }
-  uint32_t tot;
-  block_excl_scan<kThreads>(sum, wsum, tot);
-  if (threadIdx.x == 0) a.tile_len[arr * a.tiles + blockIdx.x] = tot;
+  count_tile<kRounds>(a.tile_len, arr * a.tiles + blockIdx.x, wsum, base, a.held,
+                      [&](uint32_t e) { return stash_item(a, arr, e, t); });
 }
 
-__global__ void __launch_bounds__(kThreads) ds_write_kernel(StashArgs a) {
+__global__ void __launch_bounds__(kTextThreads) ds_write_kernel(StashArgs a) {
   __shared__ __align__(16) char stage[kTile * kStashItemMax + 16];
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const int arr = blockIdx.y;
   const uint32_t base = blockIdx.x * kTile;
-  write_tile<kStashItemMax>(a.tile_off[arr * a.tiles + blockIdx.x], a.body, stage, wsum, [&](int r, char *t) {
-    const uint32_t e = base + r * kThreads + threadIdx.x;
+  const uint32_t off = a.tile_off[arr * a.tiles + blockIdx.x];
+  write_tile<kStashItemMax, kRounds>(off, a.body, stage, wsum, [&](int r, char *t) {
+    const uint32_t e = base + r * kTextThreads + threadIdx.x;
     return e < a.held ? stash_item(a, arr, e, t) : 0;
   });
-}
-
-inline int nonfinite_fail(const char *msg) {
-  set_last_error(msg);
-  return B200DD_ERR_NONFINITE;
 }
 
 const char *const kDocHead[3] = {",\"delay\":[", "],\"doppler\":[", "],\"snr\":["};
@@ -460,11 +424,11 @@ int b200dd_detjson_render_device(b200dd_detjson *h, const double *d_delay, const
   a.ring = h->d_ring; a.ring_cap = h->ring_cap; a.rs = h->d_ring_state; a.info = h->d_info;
   a.tile_len = h->d_tile_len; a.tile_off = h->d_tile_off; a.body = h->d_body;
   B2_CUDA(cudaMemsetAsync(h->d_info, 0, sizeof(DjInfo), st));
-  dj_len_kernel<<<dim3(kDocTiles, 3), kThreads, 0, st>>>(a);
+  dj_len_kernel<<<dim3(kDocTiles, 3), kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)(3 * kDocTiles), &h->d_info->body);
   B2_LAUNCH_CHECK();
-  dj_write_kernel<<<dim3(kDocTiles, 3), kThreads, 0, st>>>(a);
+  dj_write_kernel<<<dim3(kDocTiles, 3), kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   h->pending = true;
   return B200DD_OK;
@@ -491,29 +455,10 @@ int b200dd_detjson_fetch(b200dd_detjson *h, uint64_t timestamp, char *out, size_
     h->pending = false;
     return nonfinite_fail("b200dd_detjson_fetch: a delay, Doppler or SNR has no JSON text: no document");
   }
-  const std::string hdr = "{\"timestamp\":" + std::to_string((unsigned long long)timestamp);
-  const uint32_t sec[3] = {ends[0], ends[1] - ends[0], ends[2] - ends[1]};
-  size_t total = hdr.size() + 2;
-  for (int i = 0; i < 3; i++) total += strlen(kDocHead[i]) + sec[i];
-  if (n_bytes) *n_bytes = total;
-  if (total > cap) {
-    set_last_error("b200dd_detjson_fetch: output capacity too small (see b200dd_detjson_max_bytes)");
-    return B200DD_ERR_CAPACITY;
-  }
-  char *p = out;
-  memcpy(p, hdr.data(), hdr.size());
-  p += hdr.size();
-  uint32_t from = 0;
-  for (int i = 0; i < 3; i++) {
-    memcpy(p, kDocHead[i], strlen(kDocHead[i]));
-    p += strlen(kDocHead[i]);
-    if (sec[i]) B2_CUDA(cudaMemcpyAsync(p, h->d_body + from, sec[i], cudaMemcpyDeviceToHost, st));
-    p += sec[i];
-    from += sec[i];
-  }
-  p[0] = ']';
-  p[1] = '}';
-  B2_CUDA(cudaStreamSynchronize(st));
+  const int rc = write_document("{\"timestamp\":" + std::to_string((unsigned long long)timestamp), 3, kDocHead, ends,
+                                h->d_body, out, cap, n_bytes,
+                                "b200dd_detjson_fetch: output capacity too small (see b200dd_detjson_max_bytes)", st);
+  if (rc != B200DD_OK) return rc;
   h->pending = false;
   if (info.range) {
     set_last_error("b200dd_detjson_fetch: a value's hundredths lie outside int32: the document was written, the "
@@ -531,13 +476,9 @@ int b200dd_detjson_fetch_stash(b200dd_detjson *h, char *out, size_t cap, size_t 
     set_last_error("b200dd_detjson_fetch_stash: the stash's ring overflowed (see max_held)");
     return B200DD_ERR_CAPACITY;
   }
-  if (h->records.empty()) {  // detection.js:10, output = []
-    if (n_bytes) *n_bytes = 2;
-    if (cap < 2) return B200DD_ERR_CAPACITY;
-    out[0] = '[';
-    out[1] = ']';
-    return B200DD_OK;
-  }
+  const char *cap_msg = "b200dd_detjson_fetch_stash: output capacity too small (see b200dd_detjson_stash_max_bytes)";
+  if (h->records.empty())  // detection.js:10, output = []
+    return write_document("[]", 0, nullptr, nullptr, nullptr, out, cap, n_bytes, cap_msg, nullptr);
   DeviceGuard guard(h->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
   const uint32_t held = (uint32_t)(h->tail - h->head);
@@ -563,40 +504,17 @@ int b200dd_detjson_fetch_stash(b200dd_detjson *h, char *out, size_t cap, size_t 
     a.ring = h->d_ring; a.ring_cap = h->ring_cap; a.head = (uint32_t)(h->head % h->ring_cap); a.held = held;
     a.doc_first = h->d_doc_first; a.doc_text = h->d_doc_text; a.texts = h->d_texts; a.n_docs = (uint32_t)first.size();
     a.tiles = tiles; a.tile_len = h->d_stile_len; a.tile_off = h->d_stile_off; a.body = h->d_stash;
-    ds_len_kernel<<<dim3(tiles, 4), kThreads, 0, st>>>(a);
+    ds_len_kernel<<<dim3(tiles, 4), kTextThreads, 0, st>>>(a);
     B2_LAUNCH_CHECK();
     scan_kernel<<<1, 1024, 0, st>>>(h->d_stile_len, h->d_stile_off, (int)(4 * tiles), h->d_stile_off + 4 * tiles);
     B2_LAUNCH_CHECK();
-    ds_write_kernel<<<dim3(tiles, 4), kThreads, 0, st>>>(a);
+    ds_write_kernel<<<dim3(tiles, 4), kTextThreads, 0, st>>>(a);
     B2_LAUNCH_CHECK();
     B2_CUDA(cudaMemcpy2DAsync(ends, sizeof(uint32_t), h->d_stile_off + tiles, sizeof(uint32_t) * tiles,
                               sizeof(uint32_t), 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA(cudaStreamSynchronize(st));
   }
-  size_t total = 2;
-  uint32_t sec[4];
-  for (int i = 0; i < 4; i++) {
-    sec[i] = ends[i] - (i ? ends[i - 1] : 0);
-    total += strlen(kStashHead[i]) + sec[i];
-  }
-  if (n_bytes) *n_bytes = total;
-  if (total > cap) {
-    set_last_error("b200dd_detjson_fetch_stash: output capacity too small (see b200dd_detjson_stash_max_bytes)");
-    return B200DD_ERR_CAPACITY;
-  }
-  char *p = out;
-  uint32_t from = 0;
-  for (int i = 0; i < 4; i++) {
-    memcpy(p, kStashHead[i], strlen(kStashHead[i]));
-    p += strlen(kStashHead[i]);
-    if (sec[i]) B2_CUDA(cudaMemcpyAsync(p, h->d_stash + from, sec[i], cudaMemcpyDeviceToHost, st));
-    p += sec[i];
-    from += sec[i];
-  }
-  p[0] = ']';
-  p[1] = '}';
-  B2_CUDA(cudaStreamSynchronize(st));
-  return B200DD_OK;
+  return write_document("", 4, kStashHead, ends, h->d_stash, out, cap, n_bytes, cap_msg, st);
 }
 
 int b200dd_detjson_render_host(const double *delay, const double *doppler, const double *snr, uint32_t n,

@@ -17,18 +17,16 @@
 //                    the bin's hundredths into the ring's uncommitted row and its text code (the hundredths, or a
 //                    mark for "-0.0") into a scratch row;
 //   scan_kernel      turns the tile counts into offsets;
-//   ij_write_kernel  rebuilds each text from its code with integer arithmetic, stages each tile at its 16-byte phase
-//                    and stores it aligned (mapjson.cu).
+//   ij_write_kernel  rebuilds each text from its code with integer arithmetic and stores each tile (text_tiles.cuh).
 // The ring has kDepth + 1 rows: the row a render writes is never a held one, so a render nobody fetches (or one the
 // fetch rejects) leaves the history intact.  The fetch composes the document around the body on the host and then
 // commits the row with its timestamp.  The stash fetch renders the held rows, oldest first, with the same
 // three-kernel pattern; the short head (timestamps, min / max / mean, the empty frequency arrays) is made on the host.
 #include "common.cuh"
 #include "json_fmt.cuh"
-#include "scan.cuh"
+#include "text_tiles.cuh"
 
 #include <math.h>
-#include <stdlib.h>
 
 #include <cstring>
 #include <deque>
@@ -43,10 +41,9 @@ namespace {
 constexpr uint32_t kMaxBins = 65536;     // the spectrum stage's bound
 constexpr uint32_t kDepth = 20;          // nCpi, api/stash/iqdata.js:3
 constexpr uint32_t kRows = kDepth + 1;   // + the row a render writes
-constexpr int kThreads = 256;
-constexpr int kRounds = 4;                 // stash items per thread
-constexpr int kTile = kThreads * kRounds;  // stash items per CTA
-constexpr int kDocTile = kThreads;         // document bins per CTA: one per thread, the render is latency-bound
+constexpr int kRounds = 4;                     // stash items per thread
+constexpr int kTile = kTextThreads * kRounds;  // stash items per CTA
+constexpr int kDocTile = kTextThreads;         // document bins per CTA: one per thread, the render is latency-bound
 constexpr int32_t kMinusZero = INT32_MIN;  // the text code of "-0.0"
 constexpr int kDocItemMax = jf::kMaxText + 1;                // "," before the value
 constexpr int kStashItemMax = jf::kMaxHundredthsText + 3;   // ",[" before the value, "]" after it
@@ -108,14 +105,12 @@ __device__ __forceinline__ int doc_item(const DocArgs &a, uint32_t j, char *t, i
   return *vlen < 0 ? n : n + *vlen;
 }
 
-__global__ void __launch_bounds__(kThreads) ij_len_kernel(DocArgs a) {
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
-  const uint32_t j = blockIdx.x * kDocTile + threadIdx.x;
-  uint32_t sum = 0;
-  if (j < a.n) {
-    char t[kDocItemMax];
+__global__ void __launch_bounds__(kTextThreads) ij_len_kernel(DocArgs a) {
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
+  char t[kDocItemMax];
+  count_tile<1>(a.tile_len, blockIdx.x, wsum, blockIdx.x * kDocTile, a.n, [&](uint32_t j) {
     int vlen;
-    sum = (uint32_t)doc_item(a, j, t, &vlen);
+    const int n = doc_item(a, j, t, &vlen);
     const char *vt = t + (j ? 1 : 0);
     int32_t k;
     // a finite bin lies within [-3233.1, 3082.6] dB: its text always has hundredths
@@ -125,40 +120,14 @@ __global__ void __launch_bounds__(kThreads) ij_len_kernel(DocArgs a) {
       a.ring[(size_t)(*a.row) * a.n + j] = k;
       a.code[j] = k == 0 && vt[0] == '-' ? kMinusZero : k;
     }
-  }
-  uint32_t tot;
-  block_excl_scan<kThreads>(sum, wsum, tot);
-  if (threadIdx.x == 0) a.tile_len[blockIdx.x] = tot;
-}
-
-// Stages a tile's texts at the 16-byte phase of its offset and stores them aligned (mapjson.cu: mj_write_kernel).
-template <int ITEM_MAX, int ROUNDS, class F>
-__device__ __forceinline__ void write_tile(uint32_t off, char *body, char *stage, uint32_t *wsum, F item) {
-  const uint32_t phase = off & 15u;  // stage[phase + i] <-> body[off + i]: same address mod 16
-  char t[ITEM_MAX];
-  uint32_t pos = phase;
-  for (int r = 0; r < ROUNDS; r++) {
-    const int n = item(r, t);
-    uint32_t tot;
-    const uint32_t ex = block_excl_scan<kThreads>((uint32_t)n, wsum, tot);
-    for (int i = 0; i < n; i++) stage[pos + ex + i] = t[i];
-    pos += tot;
-  }
-  __syncthreads();
-  const uint32_t g0 = off, g1 = off + (pos - phase);
-  uint32_t a0 = (g0 + 15u) & ~15u, a1 = g1 & ~15u;
-  if (a0 > g1) a0 = g1;
-  if (a1 < a0) a1 = a0;
-  for (uint32_t g = g0 + threadIdx.x; g < a0; g += kThreads) body[g] = stage[g - off + phase];
-  for (uint32_t g = a1 + threadIdx.x; g < g1; g += kThreads) body[g] = stage[g - off + phase];
-  for (uint32_t g = a0 + 16u * threadIdx.x; g < a1; g += 16u * kThreads)
-    *reinterpret_cast<uint4 *>(body + g) = *reinterpret_cast<const uint4 *>(stage + (g - off + phase));
+    return n;
+  });
 }
 
 // Writes the texts ij_len_kernel measured, from their codes (a rejected render's body is never read).
-__global__ void __launch_bounds__(kThreads) ij_write_kernel(DocArgs a) {
+__global__ void __launch_bounds__(kTextThreads) ij_write_kernel(DocArgs a) {
   __shared__ __align__(16) char stage[kDocTile * kDocItemMax + 16];
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   write_tile<kDocItemMax, 1>(a.tile_off[blockIdx.x], a.body, stage, wsum, [&](int, char *t) {
     const uint32_t j = blockIdx.x * kDocTile + threadIdx.x;
     if (j >= a.n) return 0;
@@ -183,57 +152,29 @@ struct StashArgs {
   char *body;
 };
 
-// item e = (held row e / n, bin e % n) of the /stash/iqdata spectrum arrays: "[" (",[" after the first row) before a
-// row's first value, "," before the others, "]" after a row's last
+// item e = (held row e / n, bin e % n) of the /stash/iqdata spectrum arrays
 __device__ __forceinline__ int stash_item(const StashArgs &a, uint32_t e, char *t) {
   const uint32_t r = e / a.n, j = e - r * a.n;
-  int n = 0;
-  if (j == 0) {
-    if (r) t[n++] = ',';
-    t[n++] = '[';
-  } else {
-    t[n++] = ',';
-  }
   const uint32_t slot = (a.head + r) % kRows;
-  n += jf::fmt_hundredths(a.ring[(size_t)slot * a.n + j], t + n);
-  if (j == a.n - 1) t[n++] = ']';
-  return n;
+  return row_item(r != 0, j, a.n, t, [&](char *v) { return jf::fmt_hundredths(a.ring[(size_t)slot * a.n + j], v); });
 }
 
-__global__ void __launch_bounds__(kThreads) is_len_kernel(StashArgs a) {
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+__global__ void __launch_bounds__(kTextThreads) is_len_kernel(StashArgs a) {
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const uint32_t base = blockIdx.x * kTile, items = a.held * a.n;
   char t[kStashItemMax];
-  uint32_t sum = 0;
-  for (int r = 0; r < kRounds; r++) {
-    const uint32_t e = base + r * kThreads + threadIdx.x;
-    if (e < items) sum += (uint32_t)stash_item(a, e, t);
-  }
-  uint32_t tot;
-  block_excl_scan<kThreads>(sum, wsum, tot);
-  if (threadIdx.x == 0) a.tile_len[blockIdx.x] = tot;
+  count_tile<kRounds>(a.tile_len, blockIdx.x, wsum, base, items, [&](uint32_t e) { return stash_item(a, e, t); });
 }
 
-__global__ void __launch_bounds__(kThreads) is_write_kernel(StashArgs a) {
+__global__ void __launch_bounds__(kTextThreads) is_write_kernel(StashArgs a) {
   __shared__ __align__(16) char stage[kTile * kStashItemMax + 16];
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const uint32_t base = blockIdx.x * kTile, items = a.held * a.n;
   write_tile<kStashItemMax, kRounds>(a.tile_off[blockIdx.x], a.body, stage, wsum, [&](int r, char *t) {
-    const uint32_t e = base + r * kThreads + threadIdx.x;
+    const uint32_t e = base + r * kTextThreads + threadIdx.x;
     return e < items ? stash_item(a, e, t) : 0;
   });
 }
-
-// the text Writer::Double gives a metric (written once); false when it has none
-bool metric_text(double v, std::string &out) {
-  char t[jf::kMaxText];
-  if (!jf::is_finite(v)) return false;
-  out.assign(t, (size_t)jf::fmt_double(v, t));
-  return true;
-}
-
-// JSON.stringify of what JSON.parse reads from that text
-std::string js_metric(const std::string &text) { return js_number_text(strtod(text.c_str(), nullptr)); }
 
 // everything of the document before the spectrum's values
 std::string doc_head(uint64_t ts, const std::string *metrics) {
@@ -244,16 +185,11 @@ std::string doc_head(uint64_t ts, const std::string *metrics) {
 int check_metrics(const char *who, double mn, double mx, double mean, std::string *texts) {
   const double v[3] = {mn, mx, mean};
   for (int i = 0; i < 3; i++)
-    if (!metric_text(v[i], texts[i])) {
+    if (!number_text(v[i], false, false, texts[i])) {
       set_last_error(std::string(who) + ": min, max and mean must be finite (rapidjson's Writer has no text otherwise)");
       return B200DD_ERR_ARG;
     }
   return B200DD_OK;
-}
-
-inline int nonfinite_fail(const char *msg) {
-  set_last_error(msg);
-  return B200DD_ERR_NONFINITE;
 }
 
 }  // namespace
@@ -344,9 +280,10 @@ int b200dd_iqjson_create(uint32_t n_spectrum, double min, double max, double mea
   h->n = n_spectrum;
   h->tiles = (n_spectrum + kDocTile - 1) / kDocTile;
   h->stash_tiles = (kDepth * n_spectrum + kTile - 1) / kTile;
+  const double v[3] = {min, max, mean};
   for (int i = 0; i < 3; i++) {
     h->metric[i] = metric[i];
-    h->js_metric[i] = js_metric(metric[i]);
+    number_text(v[i], false, true, h->js_metric[i]);  // check_metrics found a text for each
   }
   h->max_bytes = doc_head(~0ull, h->metric).size() + (size_t)n_spectrum * kDocItemMax + 2;
   // the head: 20 timestamps of at most 20 bytes ("18446744073709552000"), metrics, 20 "[]"
@@ -412,11 +349,11 @@ int b200dd_iqjson_render_device(b200dd_iqjson *h, const void *d_spectrum, void *
   a.spec = (const double2 *)d_spectrum; a.n = h->n; a.ring = h->d_ring; a.row = h->d_row; a.code = h->d_code; a.info = h->d_info;
   a.tile_len = h->d_tile_len; a.tile_off = h->d_tile_off; a.body = h->d_body;
   B2_CUDA(cudaMemsetAsync(h->d_info, 0, sizeof(IjInfo), st));
-  ij_len_kernel<<<h->tiles, kThreads, 0, st>>>(a);
+  ij_len_kernel<<<h->tiles, kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)h->tiles, &h->d_info->body);
   B2_LAUNCH_CHECK();
-  ij_write_kernel<<<h->tiles, kThreads, 0, st>>>(a);
+  ij_write_kernel<<<h->tiles, kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   h->pending = true;
   return B200DD_OK;
@@ -436,18 +373,9 @@ int b200dd_iqjson_fetch(b200dd_iqjson *h, uint64_t timestamp, char *out, size_t 
     return nonfinite_fail("b200dd_iqjson_fetch: a spectrum bin is zero, infinite or NaN (rapidjson's Writer has no "
                           "text for its value): no document");
   }
-  const std::string hdr = doc_head(timestamp, h->metric);
-  const size_t total = hdr.size() + info.body + 2;
-  if (n_bytes) *n_bytes = total;
-  if (total > cap) {
-    set_last_error("b200dd_iqjson_fetch: output capacity too small (see b200dd_iqjson_max_bytes)");
-    return B200DD_ERR_CAPACITY;
-  }
-  memcpy(out, hdr.data(), hdr.size());
-  B2_CUDA(cudaMemcpyAsync(out + hdr.size(), h->d_body, info.body, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  out[total - 2] = ']';
-  out[total - 1] = '}';
+  const int rc = write_document(doc_head(timestamp, h->metric), 1, nullptr, &info.body, h->d_body, out, cap, n_bytes,
+                                "b200dd_iqjson_fetch: output capacity too small (see b200dd_iqjson_max_bytes)", st);
+  if (rc != B200DD_OK) return rc;
   h->pending = false;
   return h->hist ? commit_shared(h, timestamp, st) : commit(h, timestamp, st);
 }
@@ -456,13 +384,9 @@ int b200dd_iqjson_fetch_stash(b200dd_iqjson *h, char *out, size_t cap, size_t *n
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_iqjson_fetch_stash: null argument");
   if (h->hist) h = h->hist;
-  if (h->ts_text.empty()) {  // iqdata.js:8, output = []
-    if (n_bytes) *n_bytes = 2;
-    if (cap < 2) return B200DD_ERR_CAPACITY;
-    out[0] = '[';
-    out[1] = ']';
-    return B200DD_OK;
-  }
+  const char *cap_msg = "b200dd_iqjson_fetch_stash: output capacity too small (see b200dd_iqjson_stash_max_bytes)";
+  if (h->ts_text.empty())  // iqdata.js:8, output = []
+    return write_document("[]", 0, nullptr, nullptr, nullptr, out, cap, n_bytes, cap_msg, nullptr);
   DeviceGuard guard(h->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
   const uint32_t held = (uint32_t)h->ts_text.size();
@@ -476,27 +400,16 @@ int b200dd_iqjson_fetch_stash(b200dd_iqjson *h, char *out, size_t cap, size_t *n
   a.ring = h->d_ring; a.n = h->n; a.head = h->head; a.held = held;
   a.tile_len = h->d_stile_len; a.tile_off = h->d_stile_off; a.body = h->d_stash;
   const uint32_t tiles = (held * h->n + kTile - 1) / kTile;
-  is_len_kernel<<<tiles, kThreads, 0, st>>>(a);
+  is_len_kernel<<<tiles, kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   scan_kernel<<<1, 1024, 0, st>>>(h->d_stile_len, h->d_stile_off, (int)tiles, h->d_stile_off + tiles);
   B2_LAUNCH_CHECK();
-  is_write_kernel<<<tiles, kThreads, 0, st>>>(a);
+  is_write_kernel<<<tiles, kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   uint32_t body = 0;
   B2_CUDA(cudaMemcpyAsync(&body, h->d_stile_off + tiles, sizeof(body), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
-  const size_t total = hdr.size() + body + 2;
-  if (n_bytes) *n_bytes = total;
-  if (total > cap) {
-    set_last_error("b200dd_iqjson_fetch_stash: output capacity too small (see b200dd_iqjson_stash_max_bytes)");
-    return B200DD_ERR_CAPACITY;
-  }
-  memcpy(out, hdr.data(), hdr.size());
-  B2_CUDA(cudaMemcpyAsync(out + hdr.size(), h->d_stash, body, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  out[total - 2] = ']';
-  out[total - 1] = '}';
-  return B200DD_OK;
+  return write_document(hdr, 1, nullptr, &body, h->d_stash, out, cap, n_bytes, cap_msg, st);
 }
 
 int b200dd_iqjson_render_host(const double *spectrum, uint32_t n, double min, double max, double mean,

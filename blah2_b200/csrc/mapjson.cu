@@ -7,21 +7,17 @@
 // with v = 10 log10|z| - noisePower per cell, row k <-> doppler[k].  json_fmt.cuh reproduces rapidjson's text for
 // one double; this file lays out the document.
 //
-// Only the data body scales with the map, so only the body is rendered on the device.  The map is cut into
-// tiles of kTile cells (one CTA each).  mj_len_kernel formats every cell once to count the tile's bytes,
-// scan_kernel turns the counts into tile offsets (fixed order), and mj_write_kernel formats the cells again,
-// places each cell's text with a block-wide prefix sum into a shared-memory copy of the tile whose start has the
-// same 16-byte phase as its global offset, and stores it with aligned 16-byte stores (bytewise only at the two
-// partial words at the tile's ends).  No per-cell state is kept between the kernels; nothing's order depends on
-// atomics.  The header (axes, metrics, timestamp) is composed on the host with the same formatter; the body is
-// copied from the device straight behind it.
+// Only the data body scales with the map, so only the body is rendered on the device, in tiles of kTile cells
+// (text_tiles.cuh): mj_len_kernel formats every cell once to count the tile's bytes, scan_kernel turns the counts
+// into tile offsets, and mj_write_kernel formats the cells again and stores each tile.  The header (axes, metrics,
+// timestamp) is composed on the host with the same formatter; the body is copied from the device straight behind
+// it.
 #include "common.cuh"
 #include "json_fmt.cuh"
-#include "scan.cuh"
+#include "text_tiles.cuh"
 
 #include <math.h>
 
-#include <cstring>
 #include <new>
 #include <string>
 #include <vector>
@@ -30,15 +26,9 @@ using namespace b2;
 
 namespace {
 
-constexpr int kThreads = 256;
 constexpr int kRounds = 4;
-constexpr int kTile = kThreads * kRounds;    // cells per CTA
-constexpr int kCellMax = jf::kMaxText + 3;  // ",[" before the value, "]" after it
-
-template <class TMAP> __device__ __forceinline__ double2 ld_cell(const TMAP *m, size_t i) {
-  const TMAP v = m[i];
-  return make_double2((double)v.x, (double)v.y);
-}
+constexpr int kTile = kTextThreads * kRounds;  // cells per CTA
+constexpr int kCellMax = jf::kMaxText + 3;     // ",[" before the value, "]" after it
 
 struct BodyArgs {
   const void *map;
@@ -52,70 +42,39 @@ struct BodyArgs {
   uint32_t *status;         // set to 1 when a cell has no JSON text (|z| = 0, inf or NaN)
 };
 
-// cell c's bytes: its separator (",", "[" or ",[" at a row start), its value, "]" at a row end
+// cell c's bytes in the data array; bad is set when its value has no text
 template <class TMAP>
 __device__ __forceinline__ int cell_text(const BodyArgs &a, double noise, size_t c, char *t, bool &bad) {
   const double2 z = ld_cell(reinterpret_cast<const TMAP *>(a.map), c);
-  const uint32_t j = (uint32_t)(c % a.nDel);
-  int n = 0;
-  if (j == 0) {
-    if (c) t[n++] = ',';
-    t[n++] = '[';
-  } else {
-    t[n++] = ',';
-  }
-  const int k = jf::fmt_double_twice(jf::cell_db(z.x, z.y, noise), t + n);
-  if (k < 0) bad = true;
-  else n += k;
-  if (j == a.nDel - 1) t[n++] = ']';
-  return n;
+  return row_item(c != 0, (uint32_t)(c % a.nDel), a.nDel, t, [&](char *v) {
+    const int k = jf::fmt_double_twice(jf::cell_db(z.x, z.y, noise), v);
+    if (k >= 0) return k;
+    bad = true;
+    return 0;
+  });
 }
 
-template <class TMAP> __global__ void __launch_bounds__(kThreads) mj_len_kernel(BodyArgs a) {
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+template <class TMAP> __global__ void __launch_bounds__(kTextThreads) mj_len_kernel(BodyArgs a) {
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const double noise = a.noise_dev ? *a.noise_dev : a.noise;
   const size_t base = (size_t)blockIdx.x * kTile;
   char t[kCellMax];
   bool bad = false;
-  uint32_t sum = 0;
-  for (int r = 0; r < kRounds; r++) {
-    const size_t c = base + (size_t)r * kThreads + threadIdx.x;
-    if (c < a.cells) sum += (uint32_t)cell_text<TMAP>(a, noise, c, t, bad);
-  }
+  count_tile<kRounds>(a.tile_len, blockIdx.x, wsum, base, a.cells,
+                      [&](size_t c) { return cell_text<TMAP>(a, noise, c, t, bad); });
   if (bad) *a.status = 1u;  // every writer stores the same value
-  uint32_t tot;
-  block_excl_scan<kThreads>(sum, wsum, tot);
-  if (threadIdx.x == 0) a.tile_len[blockIdx.x] = tot;
 }
 
-template <class TMAP> __global__ void __launch_bounds__(kThreads) mj_write_kernel(BodyArgs a) {
+template <class TMAP> __global__ void __launch_bounds__(kTextThreads) mj_write_kernel(BodyArgs a) {
   __shared__ __align__(16) char stage[kTile * kCellMax + 16];
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const double noise = a.noise_dev ? *a.noise_dev : a.noise;
   const size_t base = (size_t)blockIdx.x * kTile;
-  const uint32_t off = a.tile_off[blockIdx.x];
-  const uint32_t phase = off & 15u;  // stage[phase + i] <-> body[off + i]: same address mod 16
-  char t[kCellMax];
   bool bad = false;
-  uint32_t pos = phase;
-  for (int r = 0; r < kRounds; r++) {
-    const size_t c = base + (size_t)r * kThreads + threadIdx.x;
-    const int n = c < a.cells ? cell_text<TMAP>(a, noise, c, t, bad) : 0;
-    uint32_t tot;
-    const uint32_t ex = block_excl_scan<kThreads>((uint32_t)n, wsum, tot);
-    for (int i = 0; i < n; i++) stage[pos + ex + i] = t[i];
-    pos += tot;
-  }
-  __syncthreads();
-  const uint32_t g0 = off, g1 = off + (pos - phase);
-  uint32_t a0 = (g0 + 15u) & ~15u, a1 = g1 & ~15u;
-  if (a0 > g1) a0 = g1;
-  if (a1 < a0) a1 = a0;
-  char *body = a.body;
-  for (uint32_t g = g0 + threadIdx.x; g < a0; g += kThreads) body[g] = stage[g - off + phase];
-  for (uint32_t g = a1 + threadIdx.x; g < g1; g += kThreads) body[g] = stage[g - off + phase];
-  for (uint32_t g = a0 + 16u * threadIdx.x; g < a1; g += 16u * kThreads)
-    *reinterpret_cast<uint4 *>(body + g) = *reinterpret_cast<const uint4 *>(stage + (g - off + phase));
+  write_tile<kCellMax, kRounds>(a.tile_off[blockIdx.x], a.body, stage, wsum, [&](int r, char *t) {
+    const size_t c = base + (size_t)r * kTextThreads + threadIdx.x;
+    return c < a.cells ? cell_text<TMAP>(a, noise, c, t, bad) : 0;
+  });
 }
 
 template <class TMAP> __global__ void mj_cell_values_kernel(const TMAP *map, size_t cells, double noise, double *out) {
@@ -123,50 +82,6 @@ template <class TMAP> __global__ void mj_cell_values_kernel(const TMAP *map, siz
     const double2 z = ld_cell(map, i);
     out[i] = jf::cell_db(z.x, z.y, noise);
   }
-}
-
-__global__ void mj_format_kernel(const double *v, uint32_t n, char *text, int *len) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-    len[i] = jf::fmt_double_twice(v[i], text + (size_t)i * jf::kMaxText);
-}
-
-// "[a,b,..]" of the values' texts (once or twice formatted); false when one has no text
-bool array_text(const double *v, size_t n, bool twice, std::string &out) {
-  out = "[";
-  char t[jf::kMaxText];
-  for (size_t i = 0; i < n; i++) {
-    const int k = twice ? jf::fmt_double_twice(v[i], t) : (jf::is_finite(v[i]) ? jf::fmt_double(v[i], t) : -1);
-    if (k < 0) return false;
-    if (i) out += ',';
-    out.append(t, (size_t)k);
-  }
-  out += ']';
-  return true;
-}
-
-// n doubles' texts joined by commas (an empty field where a value has none), as the format_doubles entries return
-int join_texts(const char *text, const int *len, uint32_t n, char *out, size_t cap, size_t *n_bytes) {
-  size_t need = n ? n - 1 : 0;
-  for (uint32_t i = 0; i < n; i++) need += len[i] > 0 ? (size_t)len[i] : 0;
-  if (n_bytes) *n_bytes = need;
-  if (need > cap) {
-    set_last_error("b200dd_mapjson_format_doubles: output capacity too small");
-    return B200DD_ERR_CAPACITY;
-  }
-  char *p = out;
-  for (uint32_t i = 0; i < n; i++) {
-    if (i) *p++ = ',';
-    if (len[i] > 0) {
-      memcpy(p, text + (size_t)i * jf::kMaxText, (size_t)len[i]);
-      p += len[i];
-    }
-  }
-  return B200DD_OK;
-}
-
-inline int nonfinite_fail(const char *msg) {
-  set_last_error(msg);
-  return B200DD_ERR_NONFINITE;
 }
 
 }  // namespace
@@ -191,16 +106,12 @@ struct b200dd_mapjson {
 
 namespace {
 
-std::string compose_header(const b200dd_mapjson *h, const char *ts, const char *noise, const char *maxp) {
+std::string compose_header(const b200dd_mapjson *h, const std::string &ts, const std::string &noise,
+                           const std::string &maxp) {
   std::string s;
   s.reserve(160 + h->delay_txt.size() + h->doppler_txt.size());
-  s += "{\"timestamp\":";
-  s += ts;
-  s += ",\"nRows\":" + std::to_string(h->nDop) + ",\"nCols\":" + std::to_string(h->nDel);
-  s += ",\"noisePower\":";
-  s += noise;
-  s += ",\"maxPower\":";
-  s += maxp;
+  s += "{\"timestamp\":" + ts + ",\"nRows\":" + std::to_string(h->nDop) + ",\"nCols\":" + std::to_string(h->nDel);
+  s += ",\"noisePower\":" + noise + ",\"maxPower\":" + maxp;
   s += ",\"delay\":" + h->delay_txt + ",\"doppler\":" + h->doppler_txt + ",\"data\":[";
   return s;
 }
@@ -211,11 +122,11 @@ template <class TMAP> int enqueue_body(b200dd_mapjson *h, const void *d_map, dou
   a.map = d_map; a.cells = h->cells; a.nDel = h->nDel; a.noise = noise; a.noise_dev = noise_dev;
   a.tile_len = h->d_tile_len; a.tile_off = h->d_tile_off; a.body = h->d_body; a.status = h->d_info + 1;
   B2_CUDA(cudaMemsetAsync(h->d_info + 1, 0, sizeof(uint32_t), st));
-  mj_len_kernel<TMAP><<<h->nTiles, kThreads, 0, st>>>(a);
+  mj_len_kernel<TMAP><<<h->nTiles, kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)h->nTiles, h->d_info);
   B2_LAUNCH_CHECK();
-  mj_write_kernel<TMAP><<<h->nTiles, kThreads, 0, st>>>(a);
+  mj_write_kernel<TMAP><<<h->nTiles, kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   return B200DD_OK;
 }
@@ -246,13 +157,14 @@ int b200dd_mapjson_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, 
   // delay axis in km, written once (Map.cpp:176); the Doppler axis goes through to_json and delay_bin_to_km
   std::vector<double> km(n_del);
   for (uint32_t i = 0; i < n_del; i++) km[i] = jf::bin_to_km(delay[i], fs);
-  h->axes_ok = array_text(km.data(), n_del, false, h->delay_txt) && array_text(doppler, n_dop, true, h->doppler_txt);
+  h->axes_ok = numbers_text(km.data(), n_del, false, false, h->delay_txt) &&
+               numbers_text(doppler, n_dop, true, false, h->doppler_txt);
   // body: every cell's text is at most kMaxText bytes, plus n_del - 1 commas and two brackets per row, plus a
   // comma between rows
   h->body_max = h->cells * jf::kMaxText + (size_t)n_dop * (n_del + 1) + (n_dop - 1);
   if (h->body_max > 0xFFFFFFF0ull) return fail(geom_fail("b200dd_mapjson_create: map too large for 32-bit text offsets"));
   const std::string widest(jf::kMaxText, '0');
-  h->max_bytes = compose_header(h, "18446744073709551615", widest.c_str(), widest.c_str()).size() + h->body_max + 2;
+  h->max_bytes = compose_header(h, "18446744073709551615", widest, widest).size() + h->body_max + 2;
   int dev = device;
   if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
   h->device = dev;
@@ -316,24 +228,12 @@ int b200dd_mapjson_fetch(b200dd_mapjson *h, uint64_t timestamp, char *out, size_
   // rapidjson's Writer refuses NaN / inf (Writer::WriteDouble): blah2 would send a truncated document
   if (info[1]) return nonfinite_fail("b200dd_mapjson_fetch: a map cell is zero, infinite or NaN: no JSON text");
   if (!h->axes_ok) return nonfinite_fail("b200dd_mapjson_fetch: an axis value has no JSON text");
-  char tn[jf::kMaxText + 1], tm[jf::kMaxText + 1];
-  const int kn = jf::fmt_double_twice(m[0], tn), km = jf::fmt_double_twice(m[1], tm);
-  if (kn < 0 || km < 0) return nonfinite_fail("b200dd_mapjson_fetch: noisePower or maxPower has no JSON text");
-  tn[kn] = tm[km] = '\0';
-  const std::string hdr = compose_header(h, std::to_string((unsigned long long)timestamp).c_str(), tn, tm);
-  const size_t total = hdr.size() + info[0] + 2;
-  if (total > cap) {
-    if (n_bytes) *n_bytes = total;
-    set_last_error("b200dd_mapjson_fetch: output capacity too small (see b200dd_mapjson_max_bytes)");
-    return B200DD_ERR_CAPACITY;
-  }
-  memcpy(out, hdr.data(), hdr.size());
-  B2_CUDA(cudaMemcpyAsync(out + hdr.size(), h->d_body, info[0], cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  out[total - 2] = ']';
-  out[total - 1] = '}';
-  if (n_bytes) *n_bytes = total;
-  return B200DD_OK;
+  std::string tn, tm;
+  if (!number_text(m[0], true, false, tn) || !number_text(m[1], true, false, tm))
+    return nonfinite_fail("b200dd_mapjson_fetch: noisePower or maxPower has no JSON text");
+  const std::string hdr = compose_header(h, std::to_string((unsigned long long)timestamp), tn, tm);
+  return write_document(hdr, 1, nullptr, &info[0], h->d_body, out, cap, n_bytes,
+                        "b200dd_mapjson_fetch: output capacity too small (see b200dd_mapjson_max_bytes)", st);
 }
 
 int b200dd_mapjson_render_host(b200dd_mapjson *h, const double *map, double noise_power, double max_power,
@@ -346,49 +246,6 @@ int b200dd_mapjson_render_host(b200dd_mapjson *h, const double *map, double nois
   const int rc = b200dd_mapjson_render_device(h, h->d_maph, 1, noise_power, max_power, h->stream);
   if (rc != B200DD_OK) return rc;
   return b200dd_mapjson_fetch(h, timestamp, out, cap, n_bytes, h->stream);
-}
-
-int b200dd_mapjson_format_doubles_host(const double *v, uint32_t n, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if ((n && !v) || (cap && !out)) return arg_fail("b200dd_mapjson_format_doubles_host: null argument");
-  std::vector<char> text((size_t)n * jf::kMaxText);
-  std::vector<int> len(n);
-  for (uint32_t i = 0; i < n; i++) len[i] = jf::fmt_double_twice(v[i], text.data() + (size_t)i * jf::kMaxText);
-  return join_texts(text.data(), len.data(), n, out, cap, n_bytes);
-}
-
-int b200dd_mapjson_format_doubles_device(const double *v, uint32_t n, char *out, size_t cap, size_t *n_bytes,
-                                         int32_t device) {
-  if (n_bytes) *n_bytes = 0;
-  if ((n && !v) || (cap && !out)) return arg_fail("b200dd_mapjson_format_doubles_device: null argument");
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__);
-  DeviceGuard guard(dev);
-  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
-  if (n == 0) return join_texts(nullptr, nullptr, 0, out, cap, n_bytes);
-  std::vector<char> text((size_t)n * jf::kMaxText);
-  std::vector<int> len(n);
-  double *d_v = nullptr;
-  char *d_text = nullptr;
-  int *d_len = nullptr;
-  auto body = [&]() -> int {
-    B2_CUDA(cudaMalloc(&d_v, sizeof(double) * n));
-    B2_CUDA(cudaMalloc(&d_text, text.size()));
-    B2_CUDA(cudaMalloc(&d_len, sizeof(int) * n));
-    B2_CUDA(cudaMemcpy(d_v, v, sizeof(double) * n, cudaMemcpyHostToDevice));
-    const uint32_t blocks = (n + 255) / 256 < 132 * 16 ? (n + 255) / 256 : 132 * 16;
-    mj_format_kernel<<<blocks, 256>>>(d_v, n, d_text, d_len);
-    B2_LAUNCH_CHECK();
-    B2_CUDA(cudaMemcpy(text.data(), d_text, text.size(), cudaMemcpyDeviceToHost));
-    B2_CUDA(cudaMemcpy(len.data(), d_len, sizeof(int) * n, cudaMemcpyDeviceToHost));
-    return B200DD_OK;
-  };
-  const int rc = body();
-  free_dev(d_v);
-  free_dev(d_text);
-  free_dev(d_len);
-  if (rc != B200DD_OK) return rc;
-  return join_texts(text.data(), len.data(), n, out, cap, n_bytes);
 }
 
 int b200dd_mapjson_debug_cell_values(b200dd_mapjson *h, const void *d_map, int is_f64, double noise_power, void *d_out,

@@ -11,17 +11,14 @@
 // (one thread) accepts or rejects the CPI.  The ring has kDepth + 1 slots: the slot a push writes is never one of
 // the held ones, so a rejected CPI leaves the window intact without a copy.  head, count and the held header live
 // on the device, so a push works inside a recorded graph.  At fetch time mh_len_kernel takes the max over the held
-// slots and counts each tile's bytes, scan_kernel places the tiles, and mh_write_kernel writes the text with the
-// staged, aligned stores of mapjson.cu.  The header is composed on the host.
+// slots and counts each tile's bytes, scan_kernel places the tiles, and mh_write_kernel writes the text
+// (text_tiles.cuh).  The header is composed on the host.
 #include "common.cuh"
 #include "json_fmt.cuh"
-#include "scan.cuh"
+#include "text_tiles.cuh"
 
 #include <math.h>
-#include <stdio.h>
-#include <stdlib.h>
 
-#include <cstring>
 #include <new>
 #include <string>
 #include <vector>
@@ -32,9 +29,8 @@ namespace {
 
 constexpr uint32_t kDepth = 20;         // nCpi, api/stash/maxhold.js:3
 constexpr uint32_t kSlots = kDepth + 1;  // + the slot being written
-constexpr int kThreads = 256;
 constexpr int kRounds = 4;
-constexpr int kTile = kThreads * kRounds;
+constexpr int kTile = kTextThreads * kRounds;
 constexpr int kCellMax = jf::kMaxHundredthsText + 3;  // ",[" before the value, "]" after it
 constexpr double kNoiseBound = 1e7;  // |noisePower| <= 1e7 dB keeps every finite double cell inside int32 hundredths
 
@@ -46,11 +42,6 @@ struct MhState {
   int32_t status;  // the last push's verdict: B200DD_OK, B200DD_FILTER_FAILED or B200DD_ERR_NONFINITE
   double noise, maxp;  // header metrics of the latest accepted CPI
 };
-
-template <class TMAP> __device__ __forceinline__ double2 ld_cell(const TMAP *m, size_t i) {
-  const TMAP v = m[i];
-  return make_double2((double)v.x, (double)v.y);
-}
 
 template <class TMAP>
 __global__ void mh_push_kernel(const TMAP *__restrict__ map, size_t cells, double noise, const double *noise_dev,
@@ -99,30 +90,17 @@ struct RenderArgs {
   char *body;
 };
 
-// cell c's bytes: its separator (",", "[" or ",[" at a row start), its value, "]" at a row end
+// cell c's bytes in the data array, k being its held hundredths
 __device__ __forceinline__ int cell_text(const RenderArgs &a, size_t c, int32_t k, char *t) {
-  const uint32_t j = (uint32_t)(c % a.nDel);
-  int n = 0;
-  if (j == 0) {
-    if (c) t[n++] = ',';
-    t[n++] = '[';
-  } else {
-    t[n++] = ',';
-  }
-  n += jf::fmt_hundredths(k, t + n);
-  if (j == a.nDel - 1) t[n++] = ']';
-  return n;
+  return row_item(c != 0, (uint32_t)(c % a.nDel), a.nDel, t, [&](char *v) { return jf::fmt_hundredths(k, v); });
 }
 
-__global__ void __launch_bounds__(kThreads) mh_len_kernel(RenderArgs a) {
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+__global__ void __launch_bounds__(kTextThreads) mh_len_kernel(RenderArgs a) {
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const uint32_t head = a.s->head, count = a.s->count;
   const size_t base = (size_t)blockIdx.x * kTile;
   char t[kCellMax];
-  uint32_t sum = 0;
-  for (int r = 0; r < kRounds; r++) {
-    const size_t c = base + (size_t)r * kThreads + threadIdx.x;
-    if (c >= a.cells) continue;
+  count_tile<kRounds>(a.tile_len, blockIdx.x, wsum, base, a.cells, [&](size_t c) {
     uint32_t slot = head;
     int32_t m = INT32_MIN;
     for (uint32_t i = 0; i < count; i++) {  // the held slots, newest first
@@ -130,132 +108,21 @@ __global__ void __launch_bounds__(kThreads) mh_len_kernel(RenderArgs a) {
       m = max(m, a.ring[(size_t)slot * a.cells + c]);
     }
     a.held[c] = m;
-    sum += (uint32_t)cell_text(a, c, m, t);
-  }
-  uint32_t tot;
-  block_excl_scan<kThreads>(sum, wsum, tot);
-  if (threadIdx.x == 0) a.tile_len[blockIdx.x] = tot;
+    return cell_text(a, c, m, t);
+  });
 }
 
-__global__ void __launch_bounds__(kThreads) mh_write_kernel(RenderArgs a) {
+__global__ void __launch_bounds__(kTextThreads) mh_write_kernel(RenderArgs a) {
   __shared__ __align__(16) char stage[kTile * kCellMax + 16];
-  __shared__ uint32_t wsum[kThreads / 32 + 1];
+  __shared__ uint32_t wsum[kTextThreads / 32 + 1];
   const size_t base = (size_t)blockIdx.x * kTile;
-  const uint32_t off = a.tile_off[blockIdx.x];
-  const uint32_t phase = off & 15u;  // stage[phase + i] <-> body[off + i]: same address mod 16
-  char t[kCellMax];
-  uint32_t pos = phase;
-  for (int r = 0; r < kRounds; r++) {
-    const size_t c = base + (size_t)r * kThreads + threadIdx.x;
-    const int n = c < a.cells ? cell_text(a, c, a.held[c], t) : 0;
-    uint32_t tot;
-    const uint32_t ex = block_excl_scan<kThreads>((uint32_t)n, wsum, tot);
-    for (int i = 0; i < n; i++) stage[pos + ex + i] = t[i];
-    pos += tot;
-  }
-  __syncthreads();
-  const uint32_t g0 = off, g1 = off + (pos - phase);
-  uint32_t a0 = (g0 + 15u) & ~15u, a1 = g1 & ~15u;
-  if (a0 > g1) a0 = g1;
-  if (a1 < a0) a1 = a0;
-  char *body = a.body;
-  for (uint32_t g = g0 + threadIdx.x; g < a0; g += kThreads) body[g] = stage[g - off + phase];
-  for (uint32_t g = a1 + threadIdx.x; g < g1; g += kThreads) body[g] = stage[g - off + phase];
-  for (uint32_t g = a0 + 16u * threadIdx.x; g < a1; g += 16u * kThreads)
-    *reinterpret_cast<uint4 *>(body + g) = *reinterpret_cast<const uint4 *>(stage + (g - off + phase));
-}
-
-// the /stash/map text of a cell whose only held value is v[i] (len -1: none)
-__global__ void mh_format_kernel(const double *v, uint32_t n, char *text, int *len) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    int32_t k;
-    len[i] = jf::hundredths(v[i], &k) ? jf::fmt_hundredths(k, text + (size_t)i * jf::kMaxHundredthsText) : -1;
-  }
-}
-
-// JSON.stringify of the array JSON.parse reads from "[a,b,..]" of the values' texts (once or twice formatted, as
-// mapjson.cu writes the axes); false when a value has no text
-bool js_array_text(const double *v, size_t n, bool twice, std::string &out) {
-  out = "[";
-  char t[jf::kMaxText + 1];
-  for (size_t i = 0; i < n; i++) {
-    const int k = twice ? jf::fmt_double_twice(v[i], t) : (jf::is_finite(v[i]) ? jf::fmt_double(v[i], t) : -1);
-    if (k < 0) return false;
-    t[k] = '\0';
-    if (i) out += ',';
-    out += js_number_text(strtod(t, nullptr));  // JSON.parse: correctly rounded
-  }
-  out += ']';
-  return true;
-}
-
-// JSON.stringify of what JSON.parse reads from a text fmt_double_twice writes for v
-bool js_metric_text(double v, std::string &out) {
-  char t[jf::kMaxText + 1];
-  const int k = jf::fmt_double_twice(v, t);
-  if (k < 0) return false;
-  t[k] = '\0';
-  out = js_number_text(strtod(t, nullptr));
-  return true;
-}
-
-int join_texts(const char *text, const int *len, uint32_t n, char *out, size_t cap, size_t *n_bytes) {
-  size_t need = n ? n - 1 : 0;
-  for (uint32_t i = 0; i < n; i++) need += len[i] > 0 ? (size_t)len[i] : 0;
-  if (n_bytes) *n_bytes = need;
-  if (need > cap) {
-    set_last_error("b200dd_maxhold_format_doubles: output capacity too small");
-    return B200DD_ERR_CAPACITY;
-  }
-  char *p = out;
-  for (uint32_t i = 0; i < n; i++) {
-    if (i) *p++ = ',';
-    if (len[i] > 0) {
-      memcpy(p, text + (size_t)i * jf::kMaxHundredthsText, (size_t)len[i]);
-      p += len[i];
-    }
-  }
-  return B200DD_OK;
+  write_tile<kCellMax, kRounds>(a.tile_off[blockIdx.x], a.body, stage, wsum, [&](int r, char *t) {
+    const size_t c = base + (size_t)r * kTextThreads + threadIdx.x;
+    return c < a.cells ? cell_text(a, c, a.held[c], t) : 0;
+  });
 }
 
 }  // namespace
-
-// ECMAScript Number::toString (ECMA-262 6.1.6.1.20, radix 10) of a finite double: the fewest significant digits
-// that read back to d (the first precision whose correctly rounded %e text does), then the standard's layout.
-std::string b2::js_number_text(double d) {
-  if (d == 0.0) return "0";  // -0 too
-  std::string out;
-  if (d < 0) {
-    out = "-";
-    d = -d;
-  }
-  char buf[40];
-  for (int p = 1; p <= 17; p++) {
-    snprintf(buf, sizeof(buf), "%.*e", p - 1, d);
-    if (strtod(buf, nullptr) == d) break;
-  }
-  // buf = "D[.DDD]e[+-]XX": digits s (k of them), value = s * 10^(n - k)
-  std::string s;
-  const char *p = buf;
-  for (; *p != 'e'; p++)
-    if (*p != '.') s += *p;
-  const int n = atoi(p + 1) + 1;
-  while (s.size() > 1 && s.back() == '0') s.pop_back();
-  const int k = (int)s.size();
-  if (k <= n && n <= 21) {
-    out += s;
-    out.append((size_t)(n - k), '0');
-  } else if (0 < n && n <= 21) {
-    out += s.substr(0, (size_t)n) + "." + s.substr((size_t)n);
-  } else if (-6 < n && n <= 0) {
-    out += "0." + std::string((size_t)-n, '0') + s;
-  } else {
-    out += s.substr(0, 1);
-    if (k > 1) out += "." + s.substr(1);
-    out += (n - 1 < 0 ? "e-" : "e+") + std::to_string(n - 1 < 0 ? 1 - n : n - 1);
-  }
-  return out;
-}
 
 struct b200dd_maxhold {
   int device = 0;
@@ -325,8 +192,8 @@ int b200dd_maxhold_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, 
   // the axes as the map document carries them (mapjson.cu), then parsed and re-printed by the stash
   std::vector<double> km(n_del);
   for (uint32_t i = 0; i < n_del; i++) km[i] = jf::bin_to_km(delay[i], fs);
-  h->axes_ok = js_array_text(km.data(), n_del, false, h->delay_txt) &&
-               js_array_text(doppler, n_dop, true, h->doppler_txt);
+  h->axes_ok = numbers_text(km.data(), n_del, false, true, h->delay_txt) &&
+               numbers_text(doppler, n_dop, true, true, h->doppler_txt);
   h->body_max = h->cells * jf::kMaxHundredthsText + (size_t)n_dop * (n_del + 1) + (n_dop - 1);
   if (h->body_max > 0xFFFFFFF0ull) return fail(geom_fail("b200dd_maxhold_create: map too large for 32-bit text offsets"));
   // the longest texts: a timestamp, and a metric (Number::toString of a double is at most 25 bytes)
@@ -408,80 +275,23 @@ int b200dd_maxhold_fetch(b200dd_maxhold *h, uint64_t timestamp, char *out, size_
     return B200DD_ERR_NONFINITE;
   }
   std::string tn, tm;
-  js_metric_text(s.noise, tn);  // the commit accepted only metrics with a text
-  js_metric_text(s.maxp, tm);
+  number_text(s.noise, true, true, tn);  // the commit accepted only metrics with a text
+  number_text(s.maxp, true, true, tm);
   const std::string hdr = compose_header(h, js_number_text((double)timestamp), tn, tm);
   RenderArgs a;
   a.ring = h->d_ring; a.s = h->d_state; a.cells = h->cells; a.nDel = h->nDel; a.held = h->d_held;
   a.tile_len = h->d_tile_len; a.tile_off = h->d_tile_off; a.body = h->d_body;
-  mh_len_kernel<<<h->nTiles, kThreads, 0, st>>>(a);
+  mh_len_kernel<<<h->nTiles, kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)h->nTiles, h->d_total);
   B2_LAUNCH_CHECK();
-  mh_write_kernel<<<h->nTiles, kThreads, 0, st>>>(a);
+  mh_write_kernel<<<h->nTiles, kTextThreads, 0, st>>>(a);
   B2_LAUNCH_CHECK();
   uint32_t body = 0;
   B2_CUDA(cudaMemcpyAsync(&body, h->d_total, sizeof(body), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
-  const size_t total = hdr.size() + body + 2;
-  if (total > cap) {
-    if (n_bytes) *n_bytes = total;
-    set_last_error("b200dd_maxhold_fetch: output capacity too small (see b200dd_maxhold_max_bytes)");
-    return B200DD_ERR_CAPACITY;
-  }
-  memcpy(out, hdr.data(), hdr.size());
-  B2_CUDA(cudaMemcpyAsync(out + hdr.size(), h->d_body, body, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  out[total - 2] = ']';
-  out[total - 1] = '}';
-  if (n_bytes) *n_bytes = total;
-  return B200DD_OK;
-}
-
-int b200dd_maxhold_format_doubles_host(const double *v, uint32_t n, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if ((n && !v) || (cap && !out)) return arg_fail("b200dd_maxhold_format_doubles_host: null argument");
-  std::vector<char> text((size_t)n * jf::kMaxHundredthsText);
-  std::vector<int> len(n);
-  for (uint32_t i = 0; i < n; i++) {
-    int32_t k;
-    len[i] = jf::hundredths(v[i], &k) ? jf::fmt_hundredths(k, text.data() + (size_t)i * jf::kMaxHundredthsText) : -1;
-  }
-  return join_texts(text.data(), len.data(), n, out, cap, n_bytes);
-}
-
-int b200dd_maxhold_format_doubles_device(const double *v, uint32_t n, char *out, size_t cap, size_t *n_bytes,
-                                         int32_t device) {
-  if (n_bytes) *n_bytes = 0;
-  if ((n && !v) || (cap && !out)) return arg_fail("b200dd_maxhold_format_doubles_device: null argument");
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__);
-  DeviceGuard guard(dev);
-  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
-  if (n == 0) return join_texts(nullptr, nullptr, 0, out, cap, n_bytes);
-  std::vector<char> text((size_t)n * jf::kMaxHundredthsText);
-  std::vector<int> len(n);
-  double *d_v = nullptr;
-  char *d_text = nullptr;
-  int *d_len = nullptr;
-  auto body = [&]() -> int {
-    B2_CUDA(cudaMalloc(&d_v, sizeof(double) * n));
-    B2_CUDA(cudaMalloc(&d_text, text.size()));
-    B2_CUDA(cudaMalloc(&d_len, sizeof(int) * n));
-    B2_CUDA(cudaMemcpy(d_v, v, sizeof(double) * n, cudaMemcpyHostToDevice));
-    const uint32_t blocks = (n + 255) / 256 < 132 * 16 ? (n + 255) / 256 : 132 * 16;
-    mh_format_kernel<<<blocks, 256>>>(d_v, n, d_text, d_len);
-    B2_LAUNCH_CHECK();
-    B2_CUDA(cudaMemcpy(text.data(), d_text, text.size(), cudaMemcpyDeviceToHost));
-    B2_CUDA(cudaMemcpy(len.data(), d_len, sizeof(int) * n, cudaMemcpyDeviceToHost));
-    return B200DD_OK;
-  };
-  const int rc = body();
-  free_dev(d_v);
-  free_dev(d_text);
-  free_dev(d_len);
-  if (rc != B200DD_OK) return rc;
-  return join_texts(text.data(), len.data(), n, out, cap, n_bytes);
+  return write_document(hdr, 1, nullptr, &body, h->d_body, out, cap, n_bytes,
+                        "b200dd_maxhold_fetch: output capacity too small (see b200dd_maxhold_max_bytes)", st);
 }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
 // scan.cuh -- block-wide and single-CTA exclusive prefix sums (fixed order, no atomics), shared by the ordered
-// compactions of det.cu and the text layout of mapjson.cu.
+// compactions of det.cu, the tiled JSON bodies (text_tiles.cuh) and the track document of tracker.cu.
 #pragma once
 
 #include <stdint.h>
