@@ -61,6 +61,18 @@ enum TmSlot {
 };
 enum TmPath { kTmNone, kTmHost, kTmRspduo, kTmDevice };
 
+// The stages whose fetches read the last CPI: one bit each in LastCpi::stages.
+enum StageBit : unsigned {
+  kIqBit = 1u,
+  kMapBit = 2u,
+  kMaxholdBit = 4u,
+  kDetBit = 8u,
+  kTrackBit = 16u,
+  kTimingBit = 32u,
+  kAllBits = 63u,
+  kShareBits = kIqBit | kMaxholdBit | kDetBit | kTrackBit | kTimingBit,  // the stages a share set takes over
+};
+
 }  // namespace
 
 // The stateful stages of a share set (b200dd_pipeline_share_history): one max-hold window, one detection history,
@@ -82,6 +94,26 @@ struct ShareSet {
   bool ev_recorded = false;
 };
 
+// The last CPI submitted to a pipeline, written once per submit by pipeline_submitted: what its fetches read, and
+// how far they have got with it.
+struct LastCpi {
+  void *stream = nullptr;  // the stream it was submitted on: its products are there, its fetches run there
+  // StageBit: set by every submit, cleared when the stage is enabled or the pipeline joins a share set.  A stage
+  // whose bit is clear has no CPI submitted since then to fetch.
+  unsigned stages = 0;
+  int path = kTmNone;      // how it came in
+  bool filter = false;     // the clutter filter ran on it
+  bool spectrum = false;   // the spectrum stage ran on it
+  int64_t cpi = -1;        // a share-set member: the set's number of it ...
+  bool unfetched = false;  // ... and b200dd_pipeline_fetch has not taken it yet
+  const void *map = nullptr;  // its float2 map, pushed into the set's max-hold window at fetch
+  bool tr_pending = false;    // its detections have not been given to the tracker yet
+  bool tm_fetched = false;    // b200dd_pipeline_fetch took it ...
+  int tm_fs = 0;              // ... and read this clutter-filter status
+  int tm_track = 0;           // a track fetch ran the tracker on it (1, stamped) or skipped it (2, CFAR overflow)
+  bool tm_done = false;       // its timing document was committed
+};
+
 struct b200dd_pipeline {
   b200dd_pipeline_params p;
   int device = 0;
@@ -91,29 +123,16 @@ struct b200dd_pipeline {
   b200dd_det *det = nullptr;
   b200dd_spectrum *spec = nullptr;  // optional first stage (blah2.cpp:263-265)
   b200dd_iqjson *ij = nullptr;      // optional, after the spectrum: the IQ-data document (blah2.cpp:299-300) and its stash
-  void *ij_stream = nullptr;        // stream of the last submit, where its document was rendered
   b200dd_mapjson *mj = nullptr;     // optional last stage: the map document (blah2.cpp:303-304)
-  void *mj_stream = nullptr;        // stream of the last submit, where its document was rendered
   b200dd_maxhold *mh = nullptr;     // optional: the API's max-hold window (api/stash/maxhold.js)
-  void *mh_stream = nullptr;        // stream of the last submit, where its push was enqueued
   b200dd_detjson *dj = nullptr;     // optional: the detection document (blah2.cpp:312-317) and its stash
-  void *dj_stream = nullptr;        // stream of the last submit, where its document was rendered
   b200dd_tracker *tr = nullptr;     // optional: the tracker (blah2.cpp:291-296), run at fetch time
-  void *tr_stream = nullptr;        // stream of the last submit
-  bool tr_pending = false;          // the last submit's detections have not been given to the tracker yet
   // optional: the timing document (blah2.cpp:331-345) from device stamps at the chain's stage boundaries, and its
   // /stash/timing history (null for a share-set member: the set's)
   bool tm_on = false;               // the submits enqueue stamps
   TimingHistory *tm = nullptr;
   uint64_t tm_t_start = 0;
   uint64_t *d_tm = nullptr;         // the last submit's stamps, TmSlot
-  void *tm_stream = nullptr;        // ... enqueued on this stream
-  int tm_path = kTmNone;            // how the last submit came in
-  bool tm_spec = false;             // it ran the spectrum stage
-  bool tm_fetched = false;          // b200dd_pipeline_fetch took it ...
-  int tm_fs = 0;                    // ... and read this clutter-filter status
-  int tm_track = 0;                 // a track fetch ran the tracker on it (1, stamped) or skipped it (2, CFAR overflow)
-  bool tm_done = false;             // its document was committed
   std::vector<const char *> tm_names;  // behind the last document written
   std::vector<double> tm_values;
   uint32_t spec_bins = 0, spec_nfft = 0;
@@ -126,7 +145,7 @@ struct b200dd_pipeline {
   double2 *d_mapd = nullptr;
   float2 *d_map = nullptr;
   short4 *d_iq16 = nullptr;  // int16 ingest staging
-  bool last_had_filter = false;
+  LastCpi last;
   // CUDA-graph replay of the device chain (b200dd_pipeline_submit_device): one instantiated graph per
   // (d_x, d_y, d_map) triple given to b200dd_pipeline_prepare_device
   struct GraphEntry {
@@ -143,17 +162,52 @@ struct b200dd_pipeline {
   uint32_t dj_max_held = 0;
   b200dd_tracker_params tr_params{};
   uint32_t tr_max_tracks = 0, tr_max_history = 0;
-  // share-set membership: the stateful stages above are null and the set's are used
-  ShareSet *set = nullptr;
-  int64_t cpi = -1;             // the set's number of the last CPI submitted here
-  bool unfetched = false;       // ... and b200dd_pipeline_fetch has not taken it yet
-  void *cpi_stream = nullptr;   // the stream it was submitted on
-  const void *cpi_map = nullptr;  // its float2 map, pushed into the set's max-hold window at fetch
+  ShareSet *set = nullptr;  // share-set membership: the stateful stages above are null and the set's are used
 };
 
-extern "C" {
+static void pipeline_drop_graphs(b200dd_pipeline *h) {
+  for (auto &e : h->graphs)
+    if (e.exec) cudaGraphExecDestroy(e.exec);
+  h->graphs.clear();
+}
 
-static void pipeline_drop_graphs(b200dd_pipeline *h);
+// the set's operations run after the previous one (see ShareSet)
+static int set_wait(ShareSet *s, void *st) {
+  if (s->ev_recorded) B2_CUDA(cudaStreamWaitEvent((cudaStream_t)st, s->ev, 0));
+  return B200DD_OK;
+}
+
+static int set_record(ShareSet *s, void *st) {
+  B2_CUDA(cudaEventRecord(s->ev, (cudaStream_t)st));
+  s->ev_recorded = true;
+  return B200DD_OK;
+}
+
+// op(), which enqueues on `st`, as one of the set's operations: after the previous one, and before the next one
+// whatever op() returns.  Outside a share set, op() alone.
+template <class Op> static int set_ordered(ShareSet *s, void *st, Op op) {
+  if (!s) return op();
+  int rc = set_wait(s, st);
+  if (rc != B200DD_OK) return rc;
+  rc = op();
+  const int rr = set_record(s, st);
+  return rc != B200DD_OK ? rc : rr;
+}
+
+// Before a stage's handle is created again: nothing in flight on the pipeline's stream, no graph that recorded the
+// old stage (when the stage is in the chain), the old handle destroyed, and no CPI for the stage's fetches until the
+// next submit.
+template <class T>
+static int stage_reset(b200dd_pipeline *h, T *&stage, void (*destroy)(T *), unsigned bit, bool in_chain = true) {
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  if (in_chain) pipeline_drop_graphs(h);
+  destroy(stage);
+  stage = nullptr;
+  h->last.stages &= ~bit;
+  return B200DD_OK;
+}
+
+extern "C" {
 
 int b200dd_pipeline_create(const b200dd_pipeline_params *params, b200dd_pipeline **out) {
   if (!params || !out) return arg_fail("b200dd_pipeline_create: null argument");
@@ -241,23 +295,23 @@ int b200dd_pipeline_get_axes(const b200dd_pipeline *h, int32_t *delay, double *d
 
 void *b200dd_pipeline_stream(b200dd_pipeline *h) { return h ? (void *)h->stream : nullptr; }
 
+// the max-hold window `mh` takes the CPI's map `map` with the metrics and clutter-filter status its chain left, on `st`
+static int maxhold_push(const b200dd_pipeline *h, b200dd_maxhold *mh, const void *map, void *st) {
+  return maxhold_enqueue_with_metrics(mh, map, det_device_metrics(h->det), h->wh ? b200dd_wh_device_status(h->wh) : nullptr,
+                                      (cudaStream_t)st);
+}
+
 // the optional stages after set_metrics, on the map `map` of the CPI just enqueued on `st`
 static int pipeline_enqueue_products(b200dd_pipeline *h, float2 *map, void *st) {
-  h->tr_stream = st;
-  h->tr_pending = true;
   if (h->mj) {
-    h->mj_stream = st;
     const int rc = mapjson_enqueue_with_metrics(h->mj, map, det_device_metrics(h->det), (cudaStream_t)st);
     if (rc != B200DD_OK) return rc;
   }
   if (h->mh) {
-    h->mh_stream = st;
-    const int rc = maxhold_enqueue_with_metrics(h->mh, map, det_device_metrics(h->det),
-                                                h->wh ? b200dd_wh_device_status(h->wh) : nullptr, (cudaStream_t)st);
+    const int rc = maxhold_push(h, h->mh, map, st);
     if (rc != B200DD_OK) return rc;
   }
   if (h->dj) {
-    h->dj_stream = st;
     DetDeviceList l;
     const int rc = det_device_list(h->det, &l);
     if (rc != B200DD_OK) return rc;
@@ -266,32 +320,30 @@ static int pipeline_enqueue_products(b200dd_pipeline *h, float2 *map, void *st) 
   return B200DD_OK;
 }
 
-// the IQ-data document of the spectrum the spectrum stage just enqueued on `st`, from its own buffer
-static int pipeline_enqueue_iqdata(b200dd_pipeline *h, void *st) {
-  if (!h->ij) return B200DD_OK;
-  h->ij_stream = st;
-  return b200dd_iqjson_render_device(h->ij, spectrum_device_output(h->spec), st);
-}
-
 // the timing stage's stamp closing the stage that ends at `slot`, on `st` (nothing when the stage is off)
 static int tm_stamp(b200dd_pipeline *h, int slot, void *st) {
   return h->tm_on ? timing_stamp(h->d_tm + slot, (cudaStream_t)st) : B200DD_OK;
 }
 
-// after a submit: its stamps are the ones the next timing document reads
-static void tm_submitted(b200dd_pipeline *h, int path, void *st) {
-  if (!h->tm_on) return;
-  h->tm_path = path;
-  h->tm_stream = st;
-  h->tm_spec = h->spec != nullptr;
-  h->tm_fetched = h->tm_done = false;
-  h->tm_fs = 0;
-  h->tm_track = 0;
+// after the spectrum kernels on `st`: the IQ-data document of their output, from the spectrum's own buffer, and the
+// spectrum's closing stamp
+static int pipeline_enqueue_after_spectrum(b200dd_pipeline *h, void *st) {
+  if (h->ij) {
+    const int rc = b200dd_iqjson_render_device(h->ij, spectrum_device_output(h->spec), st);
+    if (rc != B200DD_OK) return rc;
+  }
+  return tm_stamp(h, kTmSpectrum, st);
 }
 
-// the detection stage's closing stamp and the products after it, closed by the output stamp
-static int pipeline_enqueue_outputs(b200dd_pipeline *h, float2 *map, void *st) {
-  int rc = h->p.detection_enable ? tm_stamp(h, kTmDetector, st) : B200DD_OK;
+// the CAF of x and y into `map`, set_metrics and the detection stages, then the products after them, on `st`
+static int pipeline_enqueue_tail(b200dd_pipeline *h, const void *x, const void *y, uint32_t n, float2 *map, void *st) {
+  int rc = b200dd_caf_process_device(h->caf, x, y, n, map, st);
+  if (rc != B200DD_OK) return rc;
+  // Map::set_metrics runs after every Ambiguity::process, detection or not (blah2.cpp:278-279): stage 0 = metrics only
+  const int last = h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0;
+  rc = b200dd_det_chain_device_async(h->det, last, map, h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(),
+                                     h->doppler.data(), st);
+  if (rc == B200DD_OK && h->p.detection_enable) rc = tm_stamp(h, kTmDetector, st);
   if (rc == B200DD_OK) rc = pipeline_enqueue_products(h, map, st);
   if (rc == B200DD_OK) rc = tm_stamp(h, kTmOutput, st);
   return rc;
@@ -305,36 +357,39 @@ static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const vo
   if (h->spec) {  // spectrumAnalyser->process(x), blah2.cpp:264, before the filter touches anything
     if (n < h->spec_nfft) return arg_fail("b200dd_pipeline_submit_device: the spectrum stage needs nfft samples");
     rc = b200dd_spectrum_process_device(h->spec, d_x, n, nullptr, st);
-    if (rc != B200DD_OK) return rc;
-    rc = pipeline_enqueue_iqdata(h, st);
-    if (rc != B200DD_OK) return rc;
-    rc = tm_stamp(h, kTmSpectrum, st);
+    if (rc == B200DD_OK) rc = pipeline_enqueue_after_spectrum(h, st);
     if (rc != B200DD_OK) return rc;
   }
   if (h->wh) {
     rc = b200dd_wh_process_device(h->wh, d_x, d_y, h->d_yf, st);  // failed solve -> y passes through
+    if (rc == B200DD_OK) rc = tm_stamp(h, kTmClutter, st);
     if (rc != B200DD_OK) return rc;
     y = h->d_yf;
-    rc = tm_stamp(h, kTmClutter, st);
-    if (rc != B200DD_OK) return rc;
   }
-  h->last_had_filter = h->wh != nullptr;
-  float2 *map = d_map ? (float2 *)d_map : h->d_map;
-  rc = b200dd_caf_process_device(h->caf, d_x, y, n, map, st);
-  if (rc != B200DD_OK) return rc;
-  // Map::set_metrics runs after every Ambiguity::process, detection or not (blah2.cpp:278-279): stage 0 = metrics only
-  const int last = h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0;
-  rc = b200dd_det_chain_device_async(h->det, last, map, h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(),
-                                     h->doppler.data(), st);
-  if (rc != B200DD_OK) return rc;
-  return pipeline_enqueue_outputs(h, map, st);
+  return pipeline_enqueue_tail(h, d_x, y, n, d_map ? (float2 *)d_map : h->d_map, st);
 }
 
-
-static void pipeline_drop_graphs(b200dd_pipeline *h) {
-  for (auto &e : h->graphs)
-    if (e.exec) cudaGraphExecDestroy(e.exec);
-  h->graphs.clear();
+// After a submit enqueued its CPI on `st`, eagerly or as a graph replay, with map `map` (null: the pipeline's own):
+// the record its fetches read.  Every entry point calls this once, on success, and nothing else that a submit runs
+// changes that record: stream capture records the enqueue functions, and a replay runs none of their host code.
+static void pipeline_submitted(b200dd_pipeline *h, int path, void *st, const void *map) {
+  LastCpi &c = h->last;
+  c.stream = st;
+  c.stages = kAllBits;
+  c.path = path;
+  c.filter = h->wh != nullptr;
+  c.spectrum = h->spec != nullptr;
+  if (ShareSet *s = h->set) {
+    c.cpi = s->next_cpi++;
+    c.unfetched = true;
+  }
+  c.map = map ? map : h->d_map;
+  c.tr_pending = true;
+  c.tm_fetched = c.tm_done = false;
+  c.tm_fs = c.tm_track = 0;
+  // an eager render marks its document itself; a replayed one cannot
+  if (h->dj) detjson_mark_rendered(h->dj, true);
+  if (h->ij) iqjson_mark_rendered(h->ij, true);
 }
 
 static const b200dd_pipeline::GraphEntry *pipeline_find_graph(const b200dd_pipeline *h, const void *d_x, const void *d_y,
@@ -346,16 +401,7 @@ static const b200dd_pipeline::GraphEntry *pipeline_find_graph(const b200dd_pipel
 
 // A share-set member takes one CPI at a time: B200DD_ERR_ARG while its last one is not fetched.
 static int member_may_submit(const b200dd_pipeline *h, const char *msg) {
-  return h->set && h->unfetched ? arg_fail(msg) : B200DD_OK;
-}
-
-// a share-set member numbers the CPI just enqueued on `st` with map `map`
-static void member_submitted(b200dd_pipeline *h, void *st, const void *map) {
-  if (!h->set) return;
-  h->cpi = h->set->next_cpi++;
-  h->unfetched = true;
-  h->cpi_stream = st;
-  h->cpi_map = map ? map : h->d_map;
+  return h->set && h->last.unfetched ? arg_fail(msg) : B200DD_OK;
 }
 
 // A CPI is 12+ kernel launches on the single submitting thread.  The chain's arguments only depend on the caller's
@@ -364,24 +410,10 @@ static void member_submitted(b200dd_pipeline *h, void *st, const void *map) {
 // Replay pays off in a submit -> fetch -> submit loop; in a deep queue of CPIs enqueued ahead eager launches can be
 // faster, so replay is opt-in per triple (b200dd_pipeline_prepare_device).
 static int pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
-                                  void *stream) {
+                                  void *st) {
   DeviceGuard guard(h->device);
-  void *st = stream ? stream : (void *)h->stream;
   const b200dd_pipeline::GraphEntry *g = pipeline_find_graph(h, d_x, d_y, n, d_map);
   if (!g) return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
-  h->last_had_filter = h->wh != nullptr;
-  h->mj_stream = st;
-  h->mh_stream = st;
-  h->tr_stream = st;
-  h->tr_pending = true;
-  if (h->dj) {
-    h->dj_stream = st;
-    detjson_mark_rendered(h->dj, true);
-  }
-  if (h->ij) {
-    h->ij_stream = st;
-    iqjson_mark_rendered(h->ij, true);
-  }
   B2_CUDA(cudaGraphLaunch(g->exec, (cudaStream_t)st));
   return B200DD_OK;
 }
@@ -392,11 +424,9 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   if (h->wh && n != h->p.caf.n_samples) return arg_fail("b200dd_pipeline_submit_device: the clutter filter needs exactly n_samples");
   int rc = member_may_submit(h, "b200dd_pipeline_submit_device: the share-set member's last CPI is not fetched yet");
   if (rc != B200DD_OK) return rc;
-  rc = pipeline_submit_device(h, d_x, d_y, n, d_map, stream);
-  if (rc == B200DD_OK) {
-    member_submitted(h, stream ? stream : (void *)h->stream, d_map);
-    tm_submitted(h, kTmDevice, stream ? stream : (void *)h->stream);
-  }
+  void *st = stream ? stream : (void *)h->stream;
+  rc = pipeline_submit_device(h, d_x, d_y, n, d_map, st);
+  if (rc == B200DD_OK) pipeline_submitted(h, kTmDevice, st, d_map);
   return rc;
 }
 
@@ -413,8 +443,7 @@ int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const vo
     if (rc != B200DD_OK) return rc;
     rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
     if (rc != B200DD_OK) return rc;
-    member_submitted(h, st, d_map);
-    tm_submitted(h, kTmDevice, st);
+    pipeline_submitted(h, kTmDevice, st, d_map);
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     if (cudaStreamBeginCapture((cudaStream_t)st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -436,37 +465,40 @@ int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const vo
   return B200DD_OK;
 }
 
-// the set's operations run after the previous one (see ShareSet)
-static int set_wait(ShareSet *s, void *st) {
-  if (s->ev_recorded) B2_CUDA(cudaStreamWaitEvent((cudaStream_t)st, s->ev, 0));
+// Enqueues on `st` the read of the last CPI's clutter-filter status into *fs (0 when the filter did not run on it)
+// and, given its detection list `l`, of CFAR's count into *cfar.  With `sync` the host waits for what was enqueued;
+// without, the caller's next synchronisation of `st` does.
+static int read_status(const b200dd_pipeline *h, cudaStream_t st, bool sync, int *fs, const DetDeviceList *l = nullptr,
+                       uint32_t *cfar = nullptr) {
+  *fs = 0;
+  if (h->last.filter) B2_CUDA(cudaMemcpyAsync(fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (l) B2_CUDA(cudaMemcpyAsync(cfar, l->cfar_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  if (sync && (h->last.filter || l)) B2_CUDA(cudaStreamSynchronize(st));
   return B200DD_OK;
 }
 
-static int set_record(ShareSet *s, void *st) {
-  B2_CUDA(cudaEventRecord(s->ev, (cudaStream_t)st));
-  s->ev_recorded = true;
-  return B200DD_OK;
+// A CPI whose clutter-filter solve failed publishes nothing after the filter: the reference skips the rest of it,
+// `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273).
+static int filter_failed(const char *msg) {
+  set_last_error(msg);
+  return B200DD_FILTER_FAILED;
 }
 
 // b200dd_pipeline_fetch of a share-set member: its CPI must be the set's oldest unfetched one; it enters the
 // max-hold window now, on the stream it was submitted on
 static int member_fetch(b200dd_pipeline *h) {
   ShareSet *s = h->set;
-  if (!h->unfetched) return arg_fail("b200dd_pipeline_fetch: the share-set member has no unfetched CPI");
+  LastCpi &c = h->last;
+  if (!c.unfetched) return arg_fail("b200dd_pipeline_fetch: the share-set member has no unfetched CPI");
   for (const b200dd_pipeline *m : s->members)
-    if (m != h && m->unfetched && m->cpi < h->cpi)
+    if (m != h && m->last.unfetched && m->last.cpi < c.cpi)
       return arg_fail("b200dd_pipeline_fetch: an older CPI of the share set is not fetched yet (fetch in submit order)");
   if (s->mh) {
-    int rc = set_wait(s, h->cpi_stream);
+    const int rc = set_ordered(s, c.stream, [&] { return maxhold_push(h, s->mh, c.map, c.stream); });
     if (rc != B200DD_OK) return rc;
-    rc = maxhold_enqueue_with_metrics(s->mh, h->cpi_map, det_device_metrics(h->det),
-                                      h->wh ? b200dd_wh_device_status(h->wh) : nullptr, (cudaStream_t)h->cpi_stream);
-    if (rc != B200DD_OK) return rc;
-    rc = set_record(s, h->cpi_stream);
-    if (rc != B200DD_OK) return rc;
-    s->mh_last = h->cpi;
+    s->mh_last = c.cpi;
   }
-  h->unfetched = false;
+  c.unfetched = false;
   return B200DD_OK;
 }
 
@@ -483,14 +515,15 @@ int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double 
   result->n_detections = 0;
   result->noise_power = 0.0;
   result->max_power = 0.0;
-  int fs = 0;
-  if (h->last_had_filter) B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, (cudaStream_t)st));
+  int fs;
+  int rc = read_status(h, (cudaStream_t)st, false, &fs);
+  if (rc != B200DD_OK) return rc;
   double metrics[2] = {0.0, 0.0};
   uint32_t n = 0;
-  const int rc = b200dd_det_chain_fetch(h->det, metrics, o_delay, o_doppler, o_snr, cap, &n, st);  // synchronises st
-  if (h->tm_path != kTmNone && (rc == B200DD_OK || rc == B200DD_ERR_CAPACITY)) {
-    h->tm_fetched = true;
-    h->tm_fs = fs;
+  rc = b200dd_det_chain_fetch(h->det, metrics, o_delay, o_doppler, o_snr, cap, &n, st);  // synchronises st
+  if (rc == B200DD_OK || rc == B200DD_ERR_CAPACITY) {
+    h->last.tm_fetched = true;
+    h->last.tm_fs = fs;
   }
   if (fs != 0) {
     // The reference skips the whole CPI when the Cholesky solve fails: `if (!filter->process(x, y)) continue;`
@@ -505,30 +538,58 @@ int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double 
   return rc;
 }
 
+// A host submit's sample counts, checked in this order: the clutter filter and the CAF read *need samples of x and
+// y, and the spectrum reads nfft <= n_samples samples of x (SpectrumAnalyser.cpp:36-39), so *need_x of x are copied.
+static int host_counts(const b200dd_pipeline *h, uint32_t n, uint32_t *need, uint32_t *need_x, const char *count_msg,
+                       const char *member_msg, const char *nfft_msg) {
+  const uint32_t N = h->p.caf.n_samples;
+  *need = *need_x = h->wh ? N : h->g.n_used;
+  if (h->wh ? (n != N) : (n < *need)) return arg_fail(count_msg);
+  const int rc = member_may_submit(h, member_msg);
+  if (rc != B200DD_OK) return rc;
+  if (h->spec && h->spec_nfft > *need) {
+    if (n < h->spec_nfft) return arg_fail(nfft_msg);
+    *need_x = h->spec_nfft;
+  }
+  return B200DD_OK;
+}
+
+// the host submits' device staging, allocated at first use: complex64 x and y, the complex128 map map_out is copied
+// from, and the submit's input: complex128 x and y (`f64`) or the int16 ingest buffer
+static int host_staging(b200dd_pipeline *h, bool f64, bool map_out) {
+  const size_t N = h->p.caf.n_samples;
+  if (!h->d_xf) B2_CUDA(cudaMalloc(&h->d_xf, sizeof(float2) * N));
+  if (!h->d_yf2) B2_CUDA(cudaMalloc(&h->d_yf2, sizeof(float2) * N));
+  if (map_out && !h->d_mapd) B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * (size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
+  if (f64 && !h->d_xd) B2_CUDA(cudaMalloc(&h->d_xd, sizeof(double2) * N));
+  if (f64 && !h->d_yd) B2_CUDA(cudaMalloc(&h->d_yd, sizeof(double2) * N));
+  if (!f64 && !h->d_iq16) B2_CUDA(cudaMalloc(&h->d_iq16, sizeof(short4) * N));
+  return B200DD_OK;
+}
+
+// the end of a host submit's enqueue: the map widened to complex128 into map_out (nullable), then the CPI's record
+static int host_submitted(b200dd_pipeline *h, int path, double *map_out) {
+  if (map_out) {
+    const uint32_t cells = h->g.n_doppler_bins * h->g.n_delay_bins;
+    pl_widen_kernel<<<grid_for(cells), 256, 0, h->stream>>>(h->d_map, h->d_mapd, cells);
+    B2_LAUNCH_CHECK();
+    B2_CUDA(cudaMemcpyAsync(map_out, h->d_mapd, sizeof(double2) * cells, cudaMemcpyDeviceToHost, h->stream));
+  }
+  pipeline_submitted(h, path, h->stream, h->d_map);
+  return B200DD_OK;
+}
+
 int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out) {
   if (!h || !x || !y) return arg_fail("b200dd_pipeline_submit_host: null argument");
-  const uint32_t N = h->p.caf.n_samples;
-  const uint32_t need = h->wh ? N : h->g.n_used;
-  if (h->wh ? (n != N) : (n < need)) return arg_fail("b200dd_pipeline_submit_host: wrong number of samples");
-  int rc = member_may_submit(h, "b200dd_pipeline_submit_host: the share-set member's last CPI is not fetched yet");
+  uint32_t need, need_x;
+  int rc = host_counts(h, n, &need, &need_x, "b200dd_pipeline_submit_host: wrong number of samples",
+                       "b200dd_pipeline_submit_host: the share-set member's last CPI is not fetched yet",
+                       "b200dd_pipeline_submit_host: the spectrum stage needs nfft samples");
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
-  if (!h->d_xd) {
-    B2_CUDA(cudaMalloc(&h->d_xd, sizeof(double2) * N));
-    B2_CUDA(cudaMalloc(&h->d_yd, sizeof(double2) * N));
-    if (!h->d_xf) {
-      B2_CUDA(cudaMalloc(&h->d_xf, sizeof(float2) * N));
-      B2_CUDA(cudaMalloc(&h->d_yf2, sizeof(float2) * N));
-    }
-    if (!h->d_mapd) B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * (size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
-  }
-  uint32_t need_x = need;
-  if (h->spec && h->spec_nfft > need_x) {  // the spectrum reads nfft <= n_samples samples of x (SpectrumAnalyser.cpp:36-39)
-    if (n < h->spec_nfft) return arg_fail("b200dd_pipeline_submit_host: the spectrum stage needs nfft samples");
-    need_x = h->spec_nfft;
-  }
-  rc = tm_stamp(h, kTmExtract0, st);
+  rc = host_staging(h, true, map_out != nullptr);
+  if (rc == B200DD_OK) rc = tm_stamp(h, kTmExtract0, st);
   if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaMemcpyAsync(h->d_xd, x, sizeof(double2) * need_x, cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemcpyAsync(h->d_yd, y, sizeof(double2) * need, cudaMemcpyHostToDevice, st));
@@ -536,83 +597,64 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   if (rc != B200DD_OK) return rc;
   if (h->spec) {  // on the caller's doubles, unrounded
     rc = b200dd_spectrum_process_device_f64(h->spec, h->d_xd, need_x, nullptr, st);
-    if (rc != B200DD_OK) return rc;
-    rc = pipeline_enqueue_iqdata(h, st);
-    if (rc != B200DD_OK) return rc;
-    rc = tm_stamp(h, kTmSpectrum, st);
+    if (rc == B200DD_OK) rc = pipeline_enqueue_after_spectrum(h, st);
     if (rc != B200DD_OK) return rc;
   }
   if (h->wh) {
     // the filter sees the caller's complex128 samples unrounded (FP64 kernels, in place)
     rc = b200dd_wh_process_device_f64(h->wh, h->d_xd, h->d_yd, h->d_yd, st);
-    if (rc != B200DD_OK) return rc;
-    rc = tm_stamp(h, kTmClutter, st);
+    if (rc == B200DD_OK) rc = tm_stamp(h, kTmClutter, st);
     if (rc != B200DD_OK) return rc;
   }
-  h->last_had_filter = h->wh != nullptr;
   pl_narrow_kernel<<<grid_for(need), 256, 0, st>>>(h->d_xd, h->d_xf, need);
   B2_LAUNCH_CHECK();
   pl_narrow_kernel<<<grid_for(need), 256, 0, st>>>(h->d_yd, h->d_yf2, need);
   B2_LAUNCH_CHECK();
   rc = tm_stamp(h, kTmNarrow, st);
-  if (rc != B200DD_OK) return rc;
-  rc = b200dd_caf_process_device(h->caf, h->d_xf, h->d_yf2, need, h->d_map, st);
-  if (rc != B200DD_OK) return rc;
-  rc = b200dd_det_chain_device_async(h->det, h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0, h->d_map,
-                                     h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(), st);
-  if (rc != B200DD_OK) return rc;
-  rc = pipeline_enqueue_outputs(h, h->d_map, st);
-  if (rc != B200DD_OK) return rc;
-  if (map_out) {
-    const uint32_t cells = h->g.n_doppler_bins * h->g.n_delay_bins;
-    pl_widen_kernel<<<grid_for(cells), 256, 0, st>>>(h->d_map, h->d_mapd, cells);
-    B2_LAUNCH_CHECK();
-    B2_CUDA(cudaMemcpyAsync(map_out, h->d_mapd, sizeof(double2) * cells, cudaMemcpyDeviceToHost, st));
-  }
-  member_submitted(h, st, h->d_map);
-  tm_submitted(h, kTmHost, st);
-  return B200DD_OK;
+  if (rc == B200DD_OK) rc = pipeline_enqueue_tail(h, h->d_xf, h->d_yf2, need, h->d_map, st);
+  if (rc == B200DD_OK) rc = host_submitted(h, kTmHost, map_out);
+  return rc;
 }
 
 int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, uint32_t n, double *map_out) {
   if (!h || !iq) return arg_fail("b200dd_pipeline_submit_host_rspduo: null argument");
-  const uint32_t N = h->p.caf.n_samples;
-  uint32_t need = h->wh ? N : h->g.n_used;
-  if (h->wh ? (n != N) : (n < need)) return arg_fail("b200dd_pipeline_submit_host_rspduo: wrong number of samples");
-  int rc = member_may_submit(h, "b200dd_pipeline_submit_host_rspduo: the share-set member's last CPI is not fetched yet");
+  uint32_t need, need_x;  // the CAF consumes n_used of the need_x instants
+  int rc = host_counts(h, n, &need, &need_x, "b200dd_pipeline_submit_host_rspduo: wrong number of samples",
+                       "b200dd_pipeline_submit_host_rspduo: the share-set member's last CPI is not fetched yet",
+                       "b200dd_pipeline_submit_host_rspduo: the spectrum stage needs nfft samples");
   if (rc != B200DD_OK) return rc;
-  if (h->spec && h->spec_nfft > need) {
-    if (n < h->spec_nfft) return arg_fail("b200dd_pipeline_submit_host_rspduo: the spectrum stage needs nfft samples");
-    need = h->spec_nfft;  // <= n_samples; the CAF still consumes n_used of them
-  }
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
-  if (!h->d_iq16) {
-    B2_CUDA(cudaMalloc(&h->d_iq16, sizeof(short4) * N));
-    if (!h->d_xf) {
-      B2_CUDA(cudaMalloc(&h->d_xf, sizeof(float2) * N));
-      B2_CUDA(cudaMalloc(&h->d_yf2, sizeof(float2) * N));
-    }
-  }
-  if (map_out && !h->d_mapd) B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * (size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
-  rc = tm_stamp(h, kTmExtract0, st);  // the device chain's first stamp closes extract_buffer
+  rc = host_staging(h, false, map_out != nullptr);
+  if (rc == B200DD_OK) rc = tm_stamp(h, kTmExtract0, st);  // the device chain's first stamp closes extract_buffer
   if (rc != B200DD_OK) return rc;
-  B2_CUDA(cudaMemcpyAsync(h->d_iq16, iq, sizeof(short4) * need, cudaMemcpyHostToDevice, st));
-  pl_ingest_rspduo_kernel<<<grid_for(need), 256, 0, st>>>(h->d_iq16, h->d_xf, h->d_yf2, need);
+  B2_CUDA(cudaMemcpyAsync(h->d_iq16, iq, sizeof(short4) * need_x, cudaMemcpyHostToDevice, st));
+  pl_ingest_rspduo_kernel<<<grid_for(need_x), 256, 0, st>>>(h->d_iq16, h->d_xf, h->d_yf2, need_x);
   B2_LAUNCH_CHECK();
   // int16 samples are exact in float32, so the float2 device path gives the same result as the
   // complex128 host path
-  rc = pipeline_submit_device(h, h->d_xf, h->d_yf2, need, h->d_map, st);
-  if (rc != B200DD_OK) return rc;
-  if (map_out) {
-    const uint32_t cells = h->g.n_doppler_bins * h->g.n_delay_bins;
-    pl_widen_kernel<<<grid_for(cells), 256, 0, st>>>(h->d_map, h->d_mapd, cells);
-    B2_LAUNCH_CHECK();
-    B2_CUDA(cudaMemcpyAsync(map_out, h->d_mapd, sizeof(double2) * cells, cudaMemcpyDeviceToHost, st));
-  }
-  member_submitted(h, st, h->d_map);
-  tm_submitted(h, kTmRspduo, st);
-  return B200DD_OK;
+  rc = pipeline_submit_device(h, h->d_xf, h->d_yf2, need_x, h->d_map, st);
+  if (rc == B200DD_OK) rc = host_submitted(h, kTmRspduo, map_out);
+  return rc;
+}
+
+// The stateful stages' handles from the parameters their enable calls stored in `h`: a pipeline's own, and a share
+// set's from its first member.
+static int maxhold_create(const b200dd_pipeline *h, b200dd_maxhold **out) {
+  return b200dd_maxhold_create(h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(), h->p.caf.fs,
+                               h->device, out);
+}
+
+static int detjson_create(const b200dd_pipeline *h, b200dd_detjson **out) {
+  return b200dd_detjson_create(h->p.caf.fs, h->dj_max_held, h->device, out);
+}
+
+static int iqjson_create(const b200dd_pipeline *h, b200dd_iqjson **out) {
+  return b200dd_iqjson_create(h->spec_bins, h->ij_metrics[0], h->ij_metrics[1], h->ij_metrics[2], h->device, out);
+}
+
+static int tracker_create(const b200dd_pipeline *h, b200dd_tracker **out) {
+  return b200dd_tracker_create(&h->tr_params, h->tr_max_tracks, h->tr_max_history, h->device, out);
 }
 
 int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32_t *n_spectrum) {
@@ -620,15 +662,13 @@ int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32
   if (h->set && h->set->ij)
     return arg_fail("b200dd_pipeline_enable_spectrum: the member's share set keeps an IQ-data history of its spectra");
   DeviceGuard guard(h->device);
-  B2_CUDA(cudaStreamSynchronize(h->stream));
-  pipeline_drop_graphs(h);  // the chain changes
-  b200dd_iqjson_destroy(h->ij);  // its bin count may change: the IQ-data stage is enabled again after this
-  h->ij = nullptr;
-  h->ij_stream = nullptr;
+  // the IQ-data stage goes too: its bin count may change, it is enabled again after this
+  int rc = stage_reset(h, h->ij, b200dd_iqjson_destroy, kIqBit);
+  if (rc != B200DD_OK) return rc;
   b200dd_spectrum_destroy(h->spec);
   h->spec = nullptr;
   h->spec_bins = h->spec_nfft = 0;
-  const int rc = b200dd_spectrum_create(h->p.caf.n_samples, bandwidth, h->device, &h->spec);
+  rc = b200dd_spectrum_create(h->p.caf.n_samples, bandwidth, h->device, &h->spec);
   if (rc != B200DD_OK) return rc;
   b200dd_spectrum_geometry sg;
   b200dd_spectrum_get_geometry(h->spec, &sg);
@@ -649,13 +689,10 @@ int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectrum_out, uin
 int b200dd_pipeline_enable_map_json(b200dd_pipeline *h, size_t *max_bytes) {
   if (!h) return arg_fail("b200dd_pipeline_enable_map_json: null handle");
   DeviceGuard guard(h->device);
-  B2_CUDA(cudaStreamSynchronize(h->stream));
-  pipeline_drop_graphs(h);  // the chain changes
-  b200dd_mapjson_destroy(h->mj);
-  h->mj = nullptr;
-  h->mj_stream = nullptr;
-  const int rc = b200dd_mapjson_create(h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(),
-                                       h->p.caf.fs, h->device, &h->mj);
+  int rc = stage_reset(h, h->mj, b200dd_mapjson_destroy, kMapBit);
+  if (rc == B200DD_OK)
+    rc = b200dd_mapjson_create(h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(), h->p.caf.fs,
+                               h->device, &h->mj);
   if (rc != B200DD_OK) return rc;
   if (max_bytes) *max_bytes = b200dd_mapjson_max_bytes(h->mj);
   return B200DD_OK;
@@ -665,18 +702,13 @@ int b200dd_pipeline_fetch_map_json(b200dd_pipeline *h, uint64_t timestamp, char 
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_map_json: null argument");
   if (!h->mj) return arg_fail("b200dd_pipeline_fetch_map_json: the map JSON stage is not enabled");
-  if (!h->mj_stream) return arg_fail("b200dd_pipeline_fetch_map_json: no CPI submitted since the stage was enabled");
+  if (!(h->last.stages & kMapBit)) return arg_fail("b200dd_pipeline_fetch_map_json: no CPI submitted since the stage was enabled");
   DeviceGuard guard(h->device);
-  cudaStream_t st = (cudaStream_t)h->mj_stream;
-  if (h->last_had_filter) {
-    int fs = 0;
-    B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaStreamSynchronize(st));
-    if (fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273): no map is sent
-      set_last_error("b200dd_pipeline_fetch_map_json: the CPI's clutter-filter solve failed; it has no map");
-      return B200DD_FILTER_FAILED;
-    }
-  }
+  cudaStream_t st = (cudaStream_t)h->last.stream;
+  int fs;
+  const int rc = read_status(h, st, true, &fs);
+  if (rc != B200DD_OK) return rc;
+  if (fs != 0) return filter_failed("b200dd_pipeline_fetch_map_json: the CPI's clutter-filter solve failed; it has no map");
   return b200dd_mapjson_fetch(h->mj, timestamp, out, cap, n_bytes, st);
 }
 
@@ -684,13 +716,8 @@ int b200dd_pipeline_enable_maxhold(b200dd_pipeline *h, size_t *max_bytes) {
   if (!h) return arg_fail("b200dd_pipeline_enable_maxhold: null handle");
   if (h->set) return arg_fail("b200dd_pipeline_enable_maxhold: a share-set member's stateful stages are the set's");
   DeviceGuard guard(h->device);
-  B2_CUDA(cudaStreamSynchronize(h->stream));
-  pipeline_drop_graphs(h);  // the chain changes
-  b200dd_maxhold_destroy(h->mh);
-  h->mh = nullptr;
-  h->mh_stream = nullptr;
-  const int rc = b200dd_maxhold_create(h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(),
-                                       h->p.caf.fs, h->device, &h->mh);
+  int rc = stage_reset(h, h->mh, b200dd_maxhold_destroy, kMaxholdBit);
+  if (rc == B200DD_OK) rc = maxhold_create(h, &h->mh);
   if (rc != B200DD_OK) return rc;
   if (max_bytes) *max_bytes = b200dd_maxhold_max_bytes(h->mh);
   return B200DD_OK;
@@ -699,20 +726,21 @@ int b200dd_pipeline_enable_maxhold(b200dd_pipeline *h, size_t *max_bytes) {
 int b200dd_pipeline_fetch_maxhold(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_maxhold: null argument");
-  if (ShareSet *s = h->set) {
-    if (!s->mh) return arg_fail("b200dd_pipeline_fetch_maxhold: the max-hold stage is not enabled");
-    if (h->cpi < 0 || h->unfetched || h->cpi != s->mh_last)
-      return arg_fail("b200dd_pipeline_fetch_maxhold: the share-set member's CPI is not the last one the window took "
-                      "(call after b200dd_pipeline_fetch, before the next CPI of the set is fetched)");
-    DeviceGuard guard(h->device);
-    const int rc = set_wait(s, h->cpi_stream);
-    if (rc != B200DD_OK) return rc;
-    return b200dd_maxhold_fetch(s->mh, timestamp, out, cap, n_bytes, h->cpi_stream);
-  }
-  if (!h->mh) return arg_fail("b200dd_pipeline_fetch_maxhold: the max-hold stage is not enabled");
-  if (!h->mh_stream) return arg_fail("b200dd_pipeline_fetch_maxhold: no CPI submitted since the stage was enabled");
+  const LastCpi &c = h->last;
+  ShareSet *s = h->set;
+  b200dd_maxhold *mh = s ? s->mh : h->mh;
+  if (!mh) return arg_fail("b200dd_pipeline_fetch_maxhold: the max-hold stage is not enabled");
+  if (s && (c.cpi < 0 || c.unfetched || c.cpi != s->mh_last))
+    return arg_fail("b200dd_pipeline_fetch_maxhold: the share-set member's CPI is not the last one the window took "
+                    "(call after b200dd_pipeline_fetch, before the next CPI of the set is fetched)");
+  if (!s && !(c.stages & kMaxholdBit))
+    return arg_fail("b200dd_pipeline_fetch_maxhold: no CPI submitted since the stage was enabled");
   DeviceGuard guard(h->device);
-  return b200dd_maxhold_fetch(h->mh, timestamp, out, cap, n_bytes, h->mh_stream);
+  if (s) {
+    const int rc = set_wait(s, c.stream);
+    if (rc != B200DD_OK) return rc;
+  }
+  return b200dd_maxhold_fetch(mh, timestamp, out, cap, n_bytes, c.stream);
 }
 
 int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held, size_t *doc_bytes,
@@ -723,14 +751,11 @@ int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held,
   int rc = detjson_check_axes(h->delay.data(), h->g.n_delay_bins, h->doppler.data(), h->g.n_doppler_bins, h->p.caf.fs);
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  B2_CUDA(cudaStreamSynchronize(h->stream));
-  pipeline_drop_graphs(h);  // the chain changes
-  b200dd_detjson_destroy(h->dj);
-  h->dj = nullptr;
-  h->dj_stream = nullptr;
-  rc = b200dd_detjson_create(h->p.caf.fs, max_held, h->device, &h->dj);
+  rc = stage_reset(h, h->dj, b200dd_detjson_destroy, kDetBit);
   if (rc != B200DD_OK) return rc;
   h->dj_max_held = max_held;
+  rc = detjson_create(h, &h->dj);
+  if (rc != B200DD_OK) return rc;
   if (doc_bytes) *doc_bytes = b200dd_detjson_max_bytes(h->dj);
   if (stash_bytes) *stash_bytes = b200dd_detjson_stash_max_bytes(h->dj);
   return B200DD_OK;
@@ -741,40 +766,33 @@ int b200dd_pipeline_fetch_detection_json(b200dd_pipeline *h, uint64_t timestamp,
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_detection_json: null argument");
   if (!h->dj) return arg_fail("b200dd_pipeline_fetch_detection_json: the detection JSON stage is not enabled");
-  if (!h->dj_stream) return arg_fail("b200dd_pipeline_fetch_detection_json: no CPI submitted since the stage was enabled");
+  if (!(h->last.stages & kDetBit))
+    return arg_fail("b200dd_pipeline_fetch_detection_json: no CPI submitted since the stage was enabled");
   DeviceGuard guard(h->device);
-  cudaStream_t st = (cudaStream_t)h->dj_stream;
+  cudaStream_t st = (cudaStream_t)h->last.stream;
   ShareSet *s = h->set;
-  if (s && h->cpi < s->dj_last)
+  if (s && h->last.cpi < s->dj_last)
     return arg_fail("b200dd_pipeline_fetch_detection_json: the share set's history has taken a later CPI");
   DetDeviceList l;
   int rc = det_device_list(h->det, &l);
   if (rc != B200DD_OK) return rc;
-  if (s) {
-    rc = set_wait(s, st);
-    if (rc != B200DD_OK) return rc;
-  }
-  int fs = 0;
-  uint32_t cfar = 0;
-  if (h->last_had_filter) B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaMemcpyAsync(&cfar, l.cfar_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  if (fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273): no detections are sent
-    detjson_mark_rendered(h->dj, false);
-    set_last_error("b200dd_pipeline_fetch_detection_json: the CPI's clutter-filter solve failed; it has no detections");
-    return B200DD_FILTER_FAILED;
-  }
-  if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
-    detjson_mark_rendered(h->dj, false);
-    set_last_error("b200dd_pipeline_fetch_detection_json: more CFAR detections than the list capacity (2^18)");
-    return B200DD_ERR_CAPACITY;
-  }
-  rc = b200dd_detjson_fetch(h->dj, timestamp, out, cap, n_bytes, st);
-  if (s) {
-    const int rr = set_record(s, st);
-    if (rr != B200DD_OK) return rr;
-    if (rc == B200DD_OK) s->dj_last = h->cpi;
-  }
+  rc = set_ordered(s, st, [&]() -> int {
+    int fs;
+    uint32_t cfar;
+    const int rs = read_status(h, st, true, &fs, &l, &cfar);
+    if (rs != B200DD_OK) return rs;
+    if (fs != 0) {
+      detjson_mark_rendered(h->dj, false);
+      return filter_failed("b200dd_pipeline_fetch_detection_json: the CPI's clutter-filter solve failed; it has no detections");
+    }
+    if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
+      detjson_mark_rendered(h->dj, false);
+      set_last_error("b200dd_pipeline_fetch_detection_json: more CFAR detections than the list capacity (2^18)");
+      return B200DD_ERR_CAPACITY;
+    }
+    return b200dd_detjson_fetch(h->dj, timestamp, out, cap, n_bytes, st);
+  });
+  if (rc == B200DD_OK && s) s->dj_last = h->last.cpi;
   return rc;
 }
 
@@ -783,7 +801,7 @@ int b200dd_pipeline_fetch_detection_stash(b200dd_pipeline *h, char *out, size_t 
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_detection_stash: null argument");
   if (!h->dj) return arg_fail("b200dd_pipeline_fetch_detection_stash: the detection JSON stage is not enabled");
   DeviceGuard guard(h->device);
-  void *st = h->dj_stream ? h->dj_stream : (void *)h->stream;
+  void *st = h->last.stages & kDetBit ? h->last.stream : (void *)h->stream;
   if (h->set) {
     const int rc = set_wait(h->set, st);
     if (rc != B200DD_OK) return rc;
@@ -796,26 +814,48 @@ int b200dd_pipeline_enable_tracker(b200dd_pipeline *h, const b200dd_tracker_para
   if (!h || !params) return arg_fail("b200dd_pipeline_enable_tracker: null argument");
   if (h->set) return arg_fail("b200dd_pipeline_enable_tracker: a share-set member's stateful stages are the set's");
   if (!h->p.detection_enable) return arg_fail("b200dd_pipeline_enable_tracker: detection is not enabled");
-  b200dd_tracker_params tp = *params;
-  tp.cpi = h->g.cpi;  // ambiguity->get_cpi(), blah2.cpp:195
-  tp.fs = h->p.caf.fs;
   DeviceGuard guard(h->device);
-  B2_CUDA(cudaStreamSynchronize(h->stream));
-  b200dd_tracker_destroy(h->tr);
-  h->tr = nullptr;
-  h->tr_stream = nullptr;
-  h->tr_pending = false;
-  const int rc = b200dd_tracker_create(&tp, max_tracks, max_history, h->device, &h->tr);
+  int rc = stage_reset(h, h->tr, b200dd_tracker_destroy, kTrackBit, false);  // it runs at fetch time, not in the chain
   if (rc != B200DD_OK) return rc;
-  h->tr_params = tp;
+  h->tr_params = *params;
+  h->tr_params.cpi = h->g.cpi;  // ambiguity->get_cpi(), blah2.cpp:195
+  h->tr_params.fs = h->p.caf.fs;
   h->tr_max_tracks = max_tracks;
   h->tr_max_history = max_history;
+  rc = tracker_create(h, &h->tr);
+  if (rc != B200DD_OK) return rc;
   if (max_bytes) *max_bytes = b200dd_tracker_max_bytes(h->tr);
   return B200DD_OK;
 }
 
+// the tracker update of the last CPI, once, then the document
 static int track_json(b200dd_pipeline *h, b200dd_tracker *tr, uint64_t timestamp, char *out, size_t cap,
-                      size_t *n_bytes, cudaStream_t st);
+                      size_t *n_bytes, cudaStream_t st) {
+  LastCpi &c = h->last;
+  if (c.tr_pending) {
+    DetDeviceList l;
+    int rc = det_device_list(h->det, &l);
+    if (rc != B200DD_OK) return rc;
+    int fs;
+    uint32_t cfar;
+    rc = read_status(h, st, true, &fs, &l, &cfar);
+    if (rc != B200DD_OK) return rc;
+    if (fs != 0) return filter_failed("b200dd_pipeline_fetch_track_json: the CPI's clutter-filter solve failed; the tracker skips it");
+    if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
+      c.tm_track = 2;  // the tracker did not run: its time is 0
+      set_last_error("b200dd_pipeline_fetch_track_json: more CFAR detections than the list capacity (2^18)");
+      return B200DD_ERR_CAPACITY;
+    }
+    rc = tm_stamp(h, kTmTracker0, st);
+    if (rc == B200DD_OK) rc = b200dd_tracker_process_device(tr, l.delay, l.doppler, l.snr, l.count, timestamp, st);
+    if (rc == B200DD_OK) rc = tm_stamp(h, kTmTracker1, st);
+    if (rc != B200DD_OK) return rc;
+    c.tm_track = 1;
+    c.tr_pending = false;
+    if (h->set) h->set->tr_last = c.cpi;
+  }
+  return b200dd_tracker_fetch(tr, timestamp, out, cap, n_bytes, st);
+}
 
 int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
   if (n_bytes) *n_bytes = 0;
@@ -823,52 +863,13 @@ int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, cha
   ShareSet *s = h->set;
   b200dd_tracker *tr = s ? s->tr : h->tr;
   if (!tr) return arg_fail("b200dd_pipeline_fetch_track_json: the tracker stage is not enabled");
-  if (!h->tr_stream) return arg_fail("b200dd_pipeline_fetch_track_json: no CPI submitted since the stage was enabled");
-  if (s && h->unfetched) return arg_fail("b200dd_pipeline_fetch_track_json: the share-set member's CPI is not fetched yet");
-  if (s && h->cpi < s->tr_last) return arg_fail("b200dd_pipeline_fetch_track_json: the share set's tracker has taken a later CPI");
+  if (!(h->last.stages & kTrackBit))
+    return arg_fail("b200dd_pipeline_fetch_track_json: no CPI submitted since the stage was enabled");
+  if (s && h->last.unfetched) return arg_fail("b200dd_pipeline_fetch_track_json: the share-set member's CPI is not fetched yet");
+  if (s && h->last.cpi < s->tr_last) return arg_fail("b200dd_pipeline_fetch_track_json: the share set's tracker has taken a later CPI");
   DeviceGuard guard(h->device);
-  cudaStream_t st = (cudaStream_t)h->tr_stream;
-  if (s) {
-    int rc = set_wait(s, st);
-    if (rc == B200DD_OK) rc = track_json(h, tr, timestamp, out, cap, n_bytes, st);
-    const int rr = set_record(s, st);
-    return rc != B200DD_OK ? rc : rr;
-  }
-  return track_json(h, tr, timestamp, out, cap, n_bytes, st);
-}
-
-// the tracker update of the last CPI, once, then the document
-static int track_json(b200dd_pipeline *h, b200dd_tracker *tr, uint64_t timestamp, char *out, size_t cap,
-                      size_t *n_bytes, cudaStream_t st) {
-  if (h->tr_pending) {
-    DetDeviceList l;
-    int rc = det_device_list(h->det, &l);
-    if (rc != B200DD_OK) return rc;
-    int fs = 0;
-    uint32_t cfar = 0;
-    if (h->last_had_filter) B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaMemcpyAsync(&cfar, l.cfar_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaStreamSynchronize(st));
-    if (fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273): the tracker does not run
-      set_last_error("b200dd_pipeline_fetch_track_json: the CPI's clutter-filter solve failed; the tracker skips it");
-      return B200DD_FILTER_FAILED;
-    }
-    if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
-      if (h->tm_on) h->tm_track = 2;  // the tracker did not run: its time is 0
-      set_last_error("b200dd_pipeline_fetch_track_json: more CFAR detections than the list capacity (2^18)");
-      return B200DD_ERR_CAPACITY;
-    }
-    rc = tm_stamp(h, kTmTracker0, st);
-    if (rc != B200DD_OK) return rc;
-    rc = b200dd_tracker_process_device(tr, l.delay, l.doppler, l.snr, l.count, timestamp, st);
-    if (rc != B200DD_OK) return rc;
-    rc = tm_stamp(h, kTmTracker1, st);
-    if (rc != B200DD_OK) return rc;
-    if (h->tm_on) h->tm_track = 1;
-    h->tr_pending = false;
-    if (h->set) h->set->tr_last = h->cpi;
-  }
-  return b200dd_tracker_fetch(tr, timestamp, out, cap, n_bytes, st);
+  cudaStream_t st = (cudaStream_t)h->last.stream;
+  return set_ordered(s, st, [&] { return track_json(h, tr, timestamp, out, cap, n_bytes, st); });
 }
 
 int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double max, double mean, size_t *doc_bytes,
@@ -877,58 +878,42 @@ int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double ma
   if (h->set) return arg_fail("b200dd_pipeline_enable_iqdata_json: a share-set member's stateful stages are the set's");
   if (!h->spec) return arg_fail("b200dd_pipeline_enable_iqdata_json: the spectrum stage is not enabled");
   DeviceGuard guard(h->device);
-  B2_CUDA(cudaStreamSynchronize(h->stream));
-  pipeline_drop_graphs(h);  // the chain changes
-  b200dd_iqjson_destroy(h->ij);
-  h->ij = nullptr;
-  h->ij_stream = nullptr;
-  const int rc = b200dd_iqjson_create(h->spec_bins, min, max, mean, h->device, &h->ij);
+  int rc = stage_reset(h, h->ij, b200dd_iqjson_destroy, kIqBit);
   if (rc != B200DD_OK) return rc;
   h->ij_metrics[0] = min;
   h->ij_metrics[1] = max;
   h->ij_metrics[2] = mean;
+  rc = iqjson_create(h, &h->ij);
+  if (rc != B200DD_OK) return rc;
   if (doc_bytes) *doc_bytes = b200dd_iqjson_max_bytes(h->ij);
   if (stash_bytes) *stash_bytes = b200dd_iqjson_stash_max_bytes(h->ij);
   return B200DD_OK;
 }
 
 // the last CPI's IQ-data document, committed to the history
-static int iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
-                       cudaStream_t st);
-
 int b200dd_pipeline_fetch_iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_iqdata_json: null argument");
   if (!h->ij) return arg_fail("b200dd_pipeline_fetch_iqdata_json: the IQ-data JSON stage is not enabled");
-  if (!h->ij_stream) return arg_fail("b200dd_pipeline_fetch_iqdata_json: no CPI submitted since the stage was enabled");
+  if (!(h->last.stages & kIqBit))
+    return arg_fail("b200dd_pipeline_fetch_iqdata_json: no CPI submitted since the stage was enabled");
   ShareSet *s = h->set;
-  if (s && h->cpi < s->ij_last)
+  if (s && h->last.cpi < s->ij_last)
     return arg_fail("b200dd_pipeline_fetch_iqdata_json: the share set's history has taken a later CPI");
   DeviceGuard guard(h->device);
-  cudaStream_t st = (cudaStream_t)h->ij_stream;
-  if (s) {
-    int rc = set_wait(s, st);
-    if (rc == B200DD_OK) rc = iqdata_json(h, timestamp, out, cap, n_bytes, st);
-    const int rr = set_record(s, st);
-    if (rc == B200DD_OK) s->ij_last = h->cpi;
-    return rc != B200DD_OK ? rc : rr;
-  }
-  return iqdata_json(h, timestamp, out, cap, n_bytes, st);
-}
-
-static int iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes,
-                       cudaStream_t st) {
-  if (h->last_had_filter) {
-    int fs = 0;
-    B2_CUDA(cudaMemcpyAsync(&fs, b200dd_wh_device_status(h->wh), sizeof(int), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaStreamSynchronize(st));
-    if (fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273): no IQ-data document is sent
+  cudaStream_t st = (cudaStream_t)h->last.stream;
+  const int rc = set_ordered(s, st, [&]() -> int {
+    int fs;
+    const int rs = read_status(h, st, true, &fs);
+    if (rs != B200DD_OK) return rs;
+    if (fs != 0) {
       iqjson_mark_rendered(h->ij, false);
-      set_last_error("b200dd_pipeline_fetch_iqdata_json: the CPI's clutter-filter solve failed; it has no document");
-      return B200DD_FILTER_FAILED;
+      return filter_failed("b200dd_pipeline_fetch_iqdata_json: the CPI's clutter-filter solve failed; it has no document");
     }
-  }
-  return b200dd_iqjson_fetch(h->ij, timestamp, out, cap, n_bytes, st);
+    return b200dd_iqjson_fetch(h->ij, timestamp, out, cap, n_bytes, st);
+  });
+  if (rc == B200DD_OK && s) s->ij_last = h->last.cpi;
+  return rc;
 }
 
 int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes) {
@@ -936,7 +921,7 @@ int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_iqdata_stash: null argument");
   if (!h->ij) return arg_fail("b200dd_pipeline_fetch_iqdata_stash: the IQ-data JSON stage is not enabled");
   DeviceGuard guard(h->device);
-  void *st = h->ij_stream ? h->ij_stream : (void *)h->stream;
+  void *st = h->last.stages & kIqBit ? h->last.stream : (void *)h->stream;
   if (h->set) {
     const int rc = set_wait(h->set, st);
     if (rc != B200DD_OK) return rc;
@@ -948,19 +933,16 @@ int b200dd_pipeline_enable_timing_json(b200dd_pipeline *h, uint64_t t_start, siz
   if (!h) return arg_fail("b200dd_pipeline_enable_timing_json: null handle");
   if (h->set) return arg_fail("b200dd_pipeline_enable_timing_json: a share-set member's stateful stages are the set's");
   DeviceGuard guard(h->device);
-  B2_CUDA(cudaStreamSynchronize(h->stream));
-  pipeline_drop_graphs(h);  // the chain changes
+  int rc = stage_reset(h, h->tm, timing_history_destroy, kTimingBit);
+  if (rc != B200DD_OK) return rc;
   if (!h->d_tm) {
     B2_CUDA(cudaMalloc(&h->d_tm, sizeof(uint64_t) * kTmSlots));
     B2_CUDA(cudaMemset(h->d_tm, 0, sizeof(uint64_t) * kTmSlots));
   }
-  TimingHistory *t = timing_history_create(t_start);
-  if (!t) return arg_fail("b200dd_pipeline_enable_timing_json: out of host memory");
-  timing_history_destroy(h->tm);
-  h->tm = t;
   h->tm_t_start = t_start;
+  h->tm = timing_history_create(t_start);
+  if (!h->tm) return arg_fail("b200dd_pipeline_enable_timing_json: out of host memory");
   h->tm_on = true;
-  h->tm_path = kTmNone;
   h->tm_names.clear();
   h->tm_values.clear();
   det_set_metrics_stamp(h->det, h->d_tm + kTmAmbiguity);
@@ -978,12 +960,13 @@ static void timing_values(b200dd_pipeline *h, const uint64_t *t, bool tracker) {
     h->tm_names.push_back(name);
     h->tm_values.push_back(v);
   };
-  const bool host = h->tm_path == kTmHost;
-  const uint64_t first = h->tm_path == kTmDevice ? t[kTmChain] : t[kTmExtract0];
+  const LastCpi &c = h->last;
+  const bool host = c.path == kTmHost;
+  const uint64_t first = c.path == kTmDevice ? t[kTmChain] : t[kTmExtract0];
   uint64_t prev = t[kTmChain];
-  double extract = h->tm_path == kTmDevice ? 0.0 : ms(t[kTmChain], t[kTmExtract0]);
+  double extract = c.path == kTmDevice ? 0.0 : ms(t[kTmChain], t[kTmExtract0]);
   double spectrum = 0.0, clutter = 0.0;
-  if (h->tm_spec) {
+  if (c.spectrum) {
     spectrum = ms(t[kTmSpectrum], prev);
     prev = t[kTmSpectrum];
   }
@@ -996,7 +979,7 @@ static void timing_values(b200dd_pipeline *h, const uint64_t *t, bool tracker) {
     prev = t[kTmNarrow];
   }
   put("extract_buffer", extract);
-  if (h->tm_spec) put("spectrum", spectrum);
+  if (c.spectrum) put("spectrum", spectrum);
   if (h->wh) put("clutter_filter", clutter);
   put("ambiguity_processing", ms(t[kTmAmbiguity], prev));
   prev = t[kTmAmbiguity];
@@ -1004,7 +987,7 @@ static void timing_values(b200dd_pipeline *h, const uint64_t *t, bool tracker) {
     put("detector", ms(t[kTmDetector], prev));
     prev = t[kTmDetector];
   }
-  const double track = h->tm_track == 1 ? ms(t[kTmTracker1], t[kTmTracker0]) : 0.0;
+  const double track = c.tm_track == 1 ? ms(t[kTmTracker1], t[kTmTracker0]) : 0.0;
   if (tracker) put("tracker", track);
   put("output_radar_data", ms(t[kTmOutput], prev));
   put("cpi", ms(t[kTmOutput], first) + track);
@@ -1015,29 +998,27 @@ int b200dd_pipeline_fetch_timing_json(b200dd_pipeline *h, uint64_t timestamp, ch
   if (!h || !out) return arg_fail("b200dd_pipeline_fetch_timing_json: null argument");
   ShareSet *s = h->set;
   TimingHistory *tm = s ? s->tm : h->tm;
+  LastCpi &c = h->last;
   if (!h->tm_on || !tm) return arg_fail("b200dd_pipeline_fetch_timing_json: the timing JSON stage is not enabled");
-  if (h->tm_path == kTmNone) return arg_fail("b200dd_pipeline_fetch_timing_json: no CPI submitted since the stage was enabled");
-  if (!h->tm_fetched) return arg_fail("b200dd_pipeline_fetch_timing_json: call after the CPI's b200dd_pipeline_fetch");
-  if (h->tm_done) return arg_fail("b200dd_pipeline_fetch_timing_json: the CPI's document was fetched already");
-  if (h->tm_fs != 0) {  // `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273) skips Timing::update
-    set_last_error("b200dd_pipeline_fetch_timing_json: the CPI's clutter-filter solve failed; it has no document");
-    return B200DD_FILTER_FAILED;
-  }
+  if (!(c.stages & kTimingBit)) return arg_fail("b200dd_pipeline_fetch_timing_json: no CPI submitted since the stage was enabled");
+  if (!c.tm_fetched) return arg_fail("b200dd_pipeline_fetch_timing_json: call after the CPI's b200dd_pipeline_fetch");
+  if (c.tm_done) return arg_fail("b200dd_pipeline_fetch_timing_json: the CPI's document was fetched already");
+  if (c.tm_fs != 0) return filter_failed("b200dd_pipeline_fetch_timing_json: the CPI's clutter-filter solve failed; it has no document");
   const bool tracker = (s ? s->tr : h->tr) != nullptr;
-  if (tracker && h->tm_track == 0)
+  if (tracker && c.tm_track == 0)
     return arg_fail("b200dd_pipeline_fetch_timing_json: with the tracker enabled, call after the CPI's track fetch");
-  if (s && h->cpi < s->tm_last)
+  if (s && c.cpi < s->tm_last)
     return arg_fail("b200dd_pipeline_fetch_timing_json: the share set's history has taken a later CPI");
   DeviceGuard guard(h->device);
   uint64_t t[kTmSlots];
-  B2_CUDA(cudaMemcpyAsync(t, h->d_tm, sizeof(t), cudaMemcpyDeviceToHost, (cudaStream_t)h->tm_stream));
-  B2_CUDA(cudaStreamSynchronize((cudaStream_t)h->tm_stream));
+  B2_CUDA(cudaMemcpyAsync(t, h->d_tm, sizeof(t), cudaMemcpyDeviceToHost, (cudaStream_t)c.stream));
+  B2_CUDA(cudaStreamSynchronize((cudaStream_t)c.stream));
   timing_values(h, t, tracker);
   const int rc = timing_history_fetch(tm, timestamp, h->tm_names.data(), h->tm_values.data(),
                                       (uint32_t)h->tm_names.size(), out, cap, n_bytes);
   if (rc == B200DD_OK) {
-    h->tm_done = true;
-    if (s) s->tm_last = h->cpi;
+    c.tm_done = true;
+    if (s) s->tm_last = c.cpi;
   }
   return rc;
 }
@@ -1150,16 +1131,10 @@ int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
   auto body = [&]() -> int {
     for (uint32_t i = 0; i < n; i++) B2_CUDA(cudaStreamSynchronize(members[i]->stream));
     B2_CUDA(cudaEventCreateWithFlags(&s->ev, cudaEventDisableTiming));
-    int rc = B200DD_OK;
-    if (h0->mh)
-      rc = b200dd_maxhold_create(h0->g.n_doppler_bins, h0->g.n_delay_bins, h0->delay.data(), h0->doppler.data(),
-                                 h0->p.caf.fs, h0->device, &s->mh);
-    if (rc == B200DD_OK && h0->dj) rc = b200dd_detjson_create(h0->p.caf.fs, h0->dj_max_held, h0->device, &s->dj);
-    if (rc == B200DD_OK && h0->ij)
-      rc = b200dd_iqjson_create(h0->spec_bins, h0->ij_metrics[0], h0->ij_metrics[1], h0->ij_metrics[2], h0->device,
-                                &s->ij);
-    if (rc == B200DD_OK && h0->tr)
-      rc = b200dd_tracker_create(&h0->tr_params, h0->tr_max_tracks, h0->tr_max_history, h0->device, &s->tr);
+    int rc = h0->mh ? maxhold_create(h0, &s->mh) : B200DD_OK;
+    if (rc == B200DD_OK && h0->dj) rc = detjson_create(h0, &s->dj);
+    if (rc == B200DD_OK && h0->ij) rc = iqjson_create(h0, &s->ij);
+    if (rc == B200DD_OK && h0->tr) rc = tracker_create(h0, &s->tr);
     if (rc == B200DD_OK && h0->tm_on && !(s->tm = timing_history_create(h0->tm_t_start)))
       rc = arg_fail("b200dd_pipeline_share_history: out of host memory");
     return rc;
@@ -1179,17 +1154,13 @@ int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
     pipeline_drop_graphs(m);  // they record the window's push
     b200dd_maxhold_destroy(m->mh);
     m->mh = nullptr;
-    m->mh_stream = nullptr;
     b200dd_tracker_destroy(m->tr);
     m->tr = nullptr;
-    m->tr_stream = nullptr;
-    m->tr_pending = false;
     timing_history_destroy(m->tm);
     m->tm = nullptr;
-    m->tm_path = kTmNone;
-    m->dj_stream = m->ij_stream = nullptr;
-    m->cpi = -1;
-    m->unfetched = false;
+    m->last.stages &= ~kShareBits;
+    m->last.cpi = -1;
+    m->last.unfetched = false;
     m->set = s;
     s->members.push_back(m);
   }

@@ -874,6 +874,12 @@ class Pipeline:
         self.iqdata_json_max_bytes = self.iqdata_stash_max_bytes = 0  # see enable_iqdata_json
         self._iqjson = self._iqstash = np.empty(1, dtype=np.uint8)
 
+    def _fetch_into(self, fn, buf, *args):
+        """fn(handle, *args, buf, its size, &n), then the n bytes it wrote into buf."""
+        n = C.c_size_t()
+        capi.check(fn(self._h, *args, capi.ptr(buf), buf.size, C.byref(n)))
+        return buf[:n.value].tobytes()
+
     def fetch_track_json(self, timestamp) -> bytes:
         """The track document after the last fetched CPI (call after fetch()): the first call per CPI runs the tracker
         on that CPI's detections with `timestamp`.  Raises B200ddError with code FILTER_FAILED when that CPI's
@@ -891,34 +897,22 @@ class Pipeline:
         """The detection document of the last fetched CPI (call after fetch()), committed to the /stash/detection
         history.  Raises B200ddError with code FILTER_FAILED when that CPI's clutter-filter solve failed (nothing is
         sent, the history is unchanged), ERR_CAPACITY when CFAR overflowed the list."""
-        n = C.c_size_t()
-        capi.check(self._lib.b200dd_pipeline_fetch_detection_json(self._h, int(timestamp), capi.ptr(self._detjson),
-                                                                  self._detjson.size, C.byref(n)))
-        return self._detjson[:n.value].tobytes()
+        return self._fetch_into(self._lib.b200dd_pipeline_fetch_detection_json, self._detjson, int(timestamp))
 
     def fetch_detection_stash(self) -> bytes:
         """The /stash/detection document of the documents fetched so far."""
-        n = C.c_size_t()
-        capi.check(self._lib.b200dd_pipeline_fetch_detection_stash(self._h, capi.ptr(self._detstash),
-                                                                   self._detstash.size, C.byref(n)))
-        return self._detstash[:n.value].tobytes()
+        return self._fetch_into(self._lib.b200dd_pipeline_fetch_detection_stash, self._detstash)
 
     def fetch_maxhold(self, timestamp) -> bytes:
         """The /stash/map document after the last fetched CPI (call after fetch()).  Raises B200ddError with code
         FILTER_FAILED when that CPI's clutter-filter solve failed (the window is unchanged), ERR_ARG when the stage
         is not enabled or nothing has been submitted."""
-        n = C.c_size_t()
-        capi.check(self._lib.b200dd_pipeline_fetch_maxhold(self._h, int(timestamp), capi.ptr(self._maxhold),
-                                                           self._maxhold.size, C.byref(n)))
-        return self._maxhold[:n.value].tobytes()
+        return self._fetch_into(self._lib.b200dd_pipeline_fetch_maxhold, self._maxhold, int(timestamp))
 
     def fetch_map_json(self, timestamp) -> bytes:
         """The map document of the last fetched CPI (call after fetch()).  Raises B200ddError with code
         FILTER_FAILED when that CPI's clutter-filter solve failed: the reference sends no map then."""
-        n = C.c_size_t()
-        capi.check(self._lib.b200dd_pipeline_fetch_map_json(self._h, int(timestamp), capi.ptr(self._json),
-                                                            self._json.size, C.byref(n)))
-        return self._json[:n.value].tobytes()
+        return self._fetch_into(self._lib.b200dd_pipeline_fetch_map_json, self._json, int(timestamp))
 
     def enable_iqdata_json(self, min, max, mean):
         """Renders the IQ-data document of every CPI submitted from now on (blah2.cpp:299-300), right after the spectrum
@@ -936,17 +930,11 @@ class Pipeline:
         """The IQ-data document of the last fetched CPI (call after fetch()), committed to the /stash/iqdata history.
         Raises B200ddError with code FILTER_FAILED when that CPI's clutter-filter solve failed (nothing is sent, the
         history is unchanged), ERR_NONFINITE when a spectrum bin has no text."""
-        n = C.c_size_t()
-        capi.check(self._lib.b200dd_pipeline_fetch_iqdata_json(self._h, int(timestamp), capi.ptr(self._iqjson),
-                                                               self._iqjson.size, C.byref(n)))
-        return self._iqjson[:n.value].tobytes()
+        return self._fetch_into(self._lib.b200dd_pipeline_fetch_iqdata_json, self._iqjson, int(timestamp))
 
     def fetch_iqdata_stash(self) -> bytes:
         """The /stash/iqdata document of the documents fetched so far."""
-        n = C.c_size_t()
-        capi.check(self._lib.b200dd_pipeline_fetch_iqdata_stash(self._h, capi.ptr(self._iqstash), self._iqstash.size,
-                                                                C.byref(n)))
-        return self._iqstash[:n.value].tobytes()
+        return self._fetch_into(self._lib.b200dd_pipeline_fetch_iqdata_stash, self._iqstash)
 
     def enable_timing_json(self, t_start):
         """Stamps every CPI submitted from now on at its stage boundaries on the device and builds blah2's timing
@@ -973,10 +961,7 @@ class Pipeline:
 
     def fetch_timing_stash(self) -> bytes:
         """The /stash/timing document of the documents committed so far."""
-        n = C.c_size_t()
-        capi.check(self._lib.b200dd_pipeline_fetch_timing_stash(self._h, capi.ptr(self._tmstash), self._tmstash.size,
-                                                                C.byref(n)))
-        return self._tmstash[:n.value].tobytes()
+        return self._fetch_into(self._lib.b200dd_pipeline_fetch_timing_stash, self._tmstash)
 
     def timing_values(self):
         """The stage names and times (ms) behind the last timing document written (a test aid)."""
