@@ -7,11 +7,13 @@
 // factorisation of the matrix the reference builds (WienerHopf.cpp:85-97) -- weights AND the "not positive definite"
 // verdict.  No GPU needed (compiled by nvcc as host code).
 #include "../../blah2_b200/csrc/solve_steps.cuh"
+#include "solve_file.h"
 
 #include <cmath>
 #include <complex>
 #include <cstdio>
 #include <cstdlib>
+#include <string>
 #include <vector>
 
 using namespace b2::solve;
@@ -116,6 +118,7 @@ static void make_system(int n, int seed, std::vector<cld> &a, std::vector<cld> &
 }
 
 int main(int argc, char **argv) {
+  if (argc == 4 && std::string(argv[1]) == "--system") return solve_file("SOLVE_LONG_SIM", sim_solve, argv[2], argv[3]);
   int bad = 0;
   // the kernel's tap range: its first size, a thread with one live row (2049 = 4 * 512 + 1), the old kernel's
   // footprint boundary, the plan boundary, the limit

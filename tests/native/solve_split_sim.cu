@@ -7,11 +7,13 @@
 // verdict.  What is NOT simulated is the synchronisation (named barriers, the queue counter, the sleeping warps): the
 // GPU tests cover that.  No GPU needed (compiled by nvcc as host code).
 #include "../../blah2_b200/csrc/solve_steps.cuh"
+#include "solve_file.h"
 
 #include <cmath>
 #include <complex>
 #include <cstdio>
 #include <cstdlib>
+#include <string>
 #include <vector>
 
 using namespace b2::solve;
@@ -169,7 +171,8 @@ static void make_system(int n, int seed, std::vector<cld> &a, std::vector<cld> &
   for (int k = 0; k < n; k++) b[k] = cld(u() - 0.5L, u() - 0.5L);
 }
 
-int main() {
+int main(int argc, char **argv) {
+  if (argc == 4 && std::string(argv[1]) == "--system") return solve_file("SOLVE_SPLIT_SIM", sim_solve, argv[2], argv[3]);
   int bad = 0;
   const int sizes[] = {1, 2, 3, 31, 32, 33, 64, 65, 100, 257, 410, 448};
   for (int n : sizes) {
