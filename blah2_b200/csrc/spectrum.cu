@@ -175,6 +175,7 @@ __global__ void __launch_bounds__(32 * RED_WARPS) spec_reduce_kernel(const doubl
 // (nSpec <= 12288; reads are warp-broadcasts), else read through L1.
 constexpr int DFT_RESEED = 64;  // in terms per chain (no re-seed at all below 8192 bins)
 constexpr int DFT_ILP = 4;
+constexpr uint32_t DFT_SMEM_BINS = 12288;  // g staged in shared memory up to here (196608 B)
 
 template <bool SMEM>
 __global__ void __launch_bounds__(DFT_THREADS) spec_dft_kernel(const double2 *__restrict__ g, const double2 *__restrict__ wtab,
@@ -276,7 +277,7 @@ template <class TIN> int run_spectrum(b200dd_spectrum *h, const TIN *d_x, double
   spec_reduce_kernel<<<(h->nSpectrum + 31) / 32, 32 * RED_WARPS, 0, st>>>(h->d_part, h->d_t2, h->d_g, h->nSpectrum, nChunks);
   B2_LAUNCH_CHECK();
   const int gridD = (int)((h->nSpectrum + DFT_OUT - 1) / DFT_OUT);
-  if (h->nSpectrum <= 12288) {
+  if (h->nSpectrum <= DFT_SMEM_BINS) {
     const size_t smem = sizeof(double2) * (size_t)h->nSpectrum;
     spec_dft_kernel<true><<<gridD, DFT_THREADS, smem, st>>>(h->d_g, h->d_w, d_out, h->nSpectrum);
   } else {
@@ -395,9 +396,10 @@ int b200dd_spectrum_create(uint32_t n, double bandwidth, int32_t device, b200dd_
     B2_CUDA(cudaMemcpy(h->d_t1, t1.data(), sizeof(double2) * decimation, cudaMemcpyHostToDevice));
     B2_CUDA(cudaMemcpy(h->d_t2, t2.data(), sizeof(double2) * nSpectrum, cudaMemcpyHostToDevice));
     B2_CUDA(cudaMemcpy(h->d_w, w.data(), sizeof(double2) * nSpectrum, cudaMemcpyHostToDevice));
-    if (nSpectrum <= 12288)
-      B2_CUDA(cudaFuncSetAttribute(spec_dft_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)(sizeof(double2) * (size_t)nSpectrum)));
+    // per function, not per handle: always the largest g any handle stages (12288 bins, 196608 B + 4 KB static),
+    // so that creating a smaller handle never lowers the limit a live larger one launches with
+    B2_CUDA(cudaFuncSetAttribute(spec_dft_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)(sizeof(double2) * (size_t)DFT_SMEM_BINS)));
     return B200DD_OK;
   };
   const int rc = body();

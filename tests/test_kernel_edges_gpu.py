@@ -19,39 +19,12 @@ import edge_cases as E
 from blah2_b200 import capi
 from blah2_b200.process import Ambiguity, Pipeline, WienerHopf, WienerHopfChunk, _DetHandle
 from blah2_b200.scene import make_scene, random_iq, Target
+from guarded import Guarded
 from oracle import blah2_oracle as O
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-5
-GUARD = 64   # complex64 elements on each side
-
-
-class Guarded:
-    """n complex64 values at element G + off of a buffer of n + 2G whose guards hold NaN: off = 0 starts the view
-    on a 16-byte boundary, off = 1 on an 8-byte one, and the view ends where its guard begins."""
-
-    def __init__(self, n, off, fill=None):
-        import torch
-        self.buf = torch.full((n + 2 * GUARD,), complex(float("nan"), float("nan")), dtype=torch.complex64, device="cuda")
-        self.lo, self.hi = GUARD + off, GUARD + off + n
-        self.view = self.buf[self.lo:self.hi]
-        assert (self.view.data_ptr() % 16 == 0) == (off == 0)
-        if fill is not None:
-            self.view.copy_(torch.as_tensor(fill, dtype=torch.complex64))
-        self._guards = self._guard_bits().clone()
-
-    def _guard_bits(self):
-        import torch
-        b = torch.view_as_real(self.buf).view(torch.int32)
-        return torch.cat([b[:self.lo], b[self.hi:]])
-
-    def intact(self):
-        import torch
-        return torch.equal(self._guard_bits(), self._guards)
-
-    def numpy(self):
-        return self.view.cpu().numpy()
 
 
 def _c64(a):
