@@ -11,10 +11,13 @@
 // detection list is carried between stages as device arrays.  The reference emits detections in
 // row-major order (Doppler row, then delay bin) and later stages preserve order, so every stage
 // ends with an ORDERED compaction (bit masks + prefix sums; no atomics decide the output order).
-// Arithmetic that decides a detection (|z z|, window mean, threshold) uses explicitly rounded
-// FP64 operations in the reference's order (no FMA contraction) and alpha = n (pfa^(-1/n) - 1) is
-// tabulated on the HOST with the same libm call as the reference, so decisions only differ from a
-// CPU run on the same map at a last-ulp tie of hypot().
+// Arithmetic that decides a detection (|z z|, window mean, threshold) or produces a value (every dB value
+// 10 log10|z| - noisePower, the parabola of Interpolate) uses explicitly rounded FP64 operations in the
+// reference's order (no FMA contraction: a contracted fma(log10|z|, 10, -noisePower) is off by an ulp in most
+// cells and turns an Interpolate plateau s1 == s0 into s1 < s0), and alpha = n (pfa^(-1/n) - 1) is tabulated on
+// the HOST with the same libm call as the reference.  A cell's dB value is jf::cell_db, the value the map
+// document prints, so decisions and values only differ from a CPU run on the same map where CUDA's log10() or
+// hypot() differs from the CPU's libm.
 //
 // Reference quirks reproduced: left training window excludes index 0 (CfarDetector1D.cpp:61, k > 0);
 // nGuard / nTrain / minDelay are int8_t; Centroid's window edges are uint16_t (Centroid.cpp:28) and
@@ -22,6 +25,7 @@
 // stays at the CFAR snr.  Fenced (undefined behaviour in the reference): a detection whose
 // neighbour cells fall outside the map is dropped instead of read out of bounds.
 #include "common.cuh"
+#include "json_fmt.cuh"
 #include "scan.cuh"
 
 #include <cmath>
@@ -36,8 +40,10 @@ namespace {
 constexpr int kBlock = 256;
 constexpr uint32_t kMaxDetections = 1u << 18;
 
-// 10 log10 |z|  (Map.cpp:198, CfarDetector1D.cpp:48, Interpolate.cpp:50)
-__device__ __forceinline__ double db_abs(double2 z) { return 10.0 * log10(hypot(z.x, z.y)); }
+// 10 log10 |z|, the product rounded on its own  (Map.cpp:198)
+__device__ __forceinline__ double db_abs(double2 z) { return __dmul_rn(10.0, log10(hypot(z.x, z.y))); }
+// 10 log10 |z| - noisePower, each operation rounded on its own  (CfarDetector1D.cpp:48, Interpolate.cpp:50-52,71-73)
+__device__ __forceinline__ double cell_snr(double2 z, double noisePower) { return jf::cell_db(z.x, z.y, noisePower); }
 
 // ------------------------------------------------------------------ set_metrics
 template <class TMAP>
@@ -47,7 +53,7 @@ __global__ void __launch_bounds__(kBlock) metrics_partial_kernel(const TMAP *map
   double sum = 0.0, mx = 0.0;  // running max starts at 0 (Map.cpp:193)
   for (size_t i = (size_t)blockIdx.x * kBlock + threadIdx.x; i < cells; i += (size_t)gridDim.x * kBlock) {
     const double v = db_abs(ld_cell(map, i));
-    sum += v;
+    sum = __dadd_rn(sum, v);
     mx = (mx < v) ? v : mx;
   }
   for (int o = 16; o > 0; o >>= 1) {
@@ -185,7 +191,7 @@ template <class TMAP> __global__ void __launch_bounds__(kBlock) cfar_emit_kernel
       if (o < a.cap) {
         a.out.delay[o] = (double)(j + a.delay[0]);              // CfarDetector1D.cpp:88
         a.out.doppler[o] = a.doppler[i];                        // :89
-        a.out.snr[o] = db_abs(ld_cell(row, j)) - noisePower;  // :48,90
+        a.out.snr[o] = cell_snr(ld_cell(row, j), noisePower);  // :48,90
       }
     }
     running += tot;
@@ -261,7 +267,7 @@ template <class TMAP> __device__ __forceinline__ void interp_one(const InterpArg
   bool keep = true;
   const int row = hz_to_bin(a.doppler, a.nDop, f);
   const double d0 = (double)a.delay[0];
-  auto db = [&](int r, int c) { return db_abs(ld_cell(map, (size_t)r * a.nDel + c)) - noisePower; };
+  auto db = [&](int r, int c) { return cell_snr(ld_cell(map, (size_t)r * a.nDel + c), noisePower); };
   if (a.doDelay) {
     if (d == d0 || d == (double)a.delay[a.nDel - 1]) keep = false;  // :46-49
     if (keep) {
