@@ -154,6 +154,8 @@ SIGNATURES = [
                                                C.c_uint32]),
     ("b200dd_pipeline_submit_host", C.c_int, [_VP, _VP, _VP, C.c_uint32, _VP]),
     ("b200dd_pipeline_submit_host_rspduo", C.c_int, [_VP, _VP, C.c_uint32, _VP]),
+    ("b200dd_pipeline_submit_host_ci8", C.c_int, [_VP, _VP, _VP, C.c_uint32, _VP]),
+    ("b200dd_pipeline_submit_host_cf32", C.c_int, [_VP, _VP, _VP, C.c_uint32, _VP]),
     ("b200dd_pipeline_submit_device", C.c_int, [_VP, _VP, _VP, C.c_uint32, _VP, _VP]),
     ("b200dd_pipeline_prepare_device", C.c_int, [_VP, _VP, _VP, C.c_uint32, _VP, _VP]),
     ("b200dd_pipeline_fetch", C.c_int, [_VP, C.POINTER(CpiResult), _VP, _VP, _VP, C.c_uint32, _VP]),

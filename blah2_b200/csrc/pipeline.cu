@@ -2,11 +2,12 @@
 // intermediates resident in HBM (the body of the reference's process thread, src/blah2.cpp:268-287).
 // Composes the per-class handles of caf.cu / wh.cu / det.cu / spectrum.cu / iqjson.cu / mapjson.cu / maxhold.cu / detjson.cu /
 // tracker.cu through their C ABI, and timing.cu's stamps and history; the only kernels
-// defined here are the complex128 <-> complex64 conversions of the host entry point.
+// defined here are the host entry points' conversions: complex128 <-> complex64 and the int16 / int8 ingest.
 #include "common.cuh"
 
 #include <algorithm>
 #include <new>
+#include <string>
 #include <vector>
 
 using namespace b2;
@@ -39,6 +40,35 @@ __global__ void pl_ingest_rspduo_kernel(const short4 *__restrict__ in, float2 *_
   }
 }
 
+// int8 I/Q, one buffer per channel: HackRF's transfer buffer (reference src/capture/hackrf/HackRf.cpp:116-128) and
+// rtl-sdr's bytes read as int8_t, as Kraken does (src/capture/kraken/Kraken.cpp:97-112).  Byte k of the 32-bit word w
+// as a signed value.
+__device__ __forceinline__ float ci8_byte(int w, int k) { return (float)((w << (24 - 8 * k)) >> 24); }
+
+// One 8-byte load per channel covers four instants; the n % 4 trailing instants take one 2-byte load each.  The
+// staging buffers and x, y come from cudaMalloc, so every vector access is aligned.
+__global__ void pl_ingest_ci8_kernel(const int8_t *__restrict__ x8, const int8_t *__restrict__ y8,
+                                     float2 *__restrict__ x, float2 *__restrict__ y, uint32_t n) {
+  const uint32_t quads = n / 4u, items = quads + n % 4u;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < items; i += gridDim.x * blockDim.x) {
+    if (i < quads) {
+      const int2 a = reinterpret_cast<const int2 *>(x8)[i];
+      const int2 b = reinterpret_cast<const int2 *>(y8)[i];
+      float4 *xo = reinterpret_cast<float4 *>(x) + 2 * i, *yo = reinterpret_cast<float4 *>(y) + 2 * i;
+      xo[0] = make_float4(ci8_byte(a.x, 0), ci8_byte(a.x, 1), ci8_byte(a.x, 2), ci8_byte(a.x, 3));
+      xo[1] = make_float4(ci8_byte(a.y, 0), ci8_byte(a.y, 1), ci8_byte(a.y, 2), ci8_byte(a.y, 3));
+      yo[0] = make_float4(ci8_byte(b.x, 0), ci8_byte(b.x, 1), ci8_byte(b.x, 2), ci8_byte(b.x, 3));
+      yo[1] = make_float4(ci8_byte(b.y, 0), ci8_byte(b.y, 1), ci8_byte(b.y, 2), ci8_byte(b.y, 3));
+    } else {
+      const uint32_t j = 4 * quads + (i - quads);
+      const char2 a = reinterpret_cast<const char2 *>(x8)[j];
+      const char2 b = reinterpret_cast<const char2 *>(y8)[j];
+      x[j] = make_float2((float)a.x, (float)a.y);
+      y[j] = make_float2((float)b.x, (float)b.y);
+    }
+  }
+}
+
 inline int grid_for(uint32_t n) {
   int b = (int)((n + 255u) / 256u);
   return b > 132 * 8 ? 132 * 8 : (b < 1 ? 1 : b);
@@ -59,7 +89,12 @@ enum TmSlot {
   kTmTracker1,
   kTmSlots
 };
-enum TmPath { kTmNone, kTmHost, kTmRspduo, kTmDevice };
+// kTmIngest: the host submits of capture-driver samples (int16, int8, complex64), whose extract_buffer is the H2D copy
+// and any de-interleave before the device chain
+enum TmPath { kTmNone, kTmHost, kTmIngest, kTmDevice };
+
+// the sample format a host submit takes
+enum HostFormat { kC128, kInt16, kCi8, kCf32 };
 
 // The stages whose fetches read the last CPI: one bit each in LastCpi::stages.
 enum StageBit : unsigned {
@@ -145,6 +180,7 @@ struct b200dd_pipeline {
   double2 *d_mapd = nullptr;
   float2 *d_map = nullptr;
   short4 *d_iq16 = nullptr;  // int16 ingest staging
+  int8_t *d_x8 = nullptr, *d_y8 = nullptr;  // int8 ingest staging, 2 N bytes per channel
   LastCpi last;
   // CUDA-graph replay of the device chain (b200dd_pipeline_submit_device): one instantiated graph per
   // (d_x, d_y, d_map) triple given to b200dd_pipeline_prepare_device
@@ -277,6 +313,8 @@ void b200dd_pipeline_destroy(b200dd_pipeline *h) {
     free_dev(h->d_mapd);
     free_dev(h->d_map);
     free_dev(h->d_iq16);
+    free_dev(h->d_x8);
+    free_dev(h->d_y8);
     if (h->stream) cudaStreamDestroy(h->stream);
   }
   delete h;
@@ -555,15 +593,18 @@ static int host_counts(const b200dd_pipeline *h, uint32_t n, uint32_t *need, uin
 }
 
 // the host submits' device staging, allocated at first use: complex64 x and y, the complex128 map map_out is copied
-// from, and the submit's input: complex128 x and y (`f64`) or the int16 ingest buffer
-static int host_staging(b200dd_pipeline *h, bool f64, bool map_out) {
+// from, and the submit's input in format `fmt`: complex128 x and y, the int16 ingest buffer or the two int8 ones
+// (complex64 samples are copied straight into x and y)
+static int host_staging(b200dd_pipeline *h, HostFormat fmt, bool map_out) {
   const size_t N = h->p.caf.n_samples;
   if (!h->d_xf) B2_CUDA(cudaMalloc(&h->d_xf, sizeof(float2) * N));
   if (!h->d_yf2) B2_CUDA(cudaMalloc(&h->d_yf2, sizeof(float2) * N));
   if (map_out && !h->d_mapd) B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * (size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
-  if (f64 && !h->d_xd) B2_CUDA(cudaMalloc(&h->d_xd, sizeof(double2) * N));
-  if (f64 && !h->d_yd) B2_CUDA(cudaMalloc(&h->d_yd, sizeof(double2) * N));
-  if (!f64 && !h->d_iq16) B2_CUDA(cudaMalloc(&h->d_iq16, sizeof(short4) * N));
+  if (fmt == kC128 && !h->d_xd) B2_CUDA(cudaMalloc(&h->d_xd, sizeof(double2) * N));
+  if (fmt == kC128 && !h->d_yd) B2_CUDA(cudaMalloc(&h->d_yd, sizeof(double2) * N));
+  if (fmt == kInt16 && !h->d_iq16) B2_CUDA(cudaMalloc(&h->d_iq16, sizeof(short4) * N));
+  if (fmt == kCi8 && !h->d_x8) B2_CUDA(cudaMalloc(&h->d_x8, 2 * N));
+  if (fmt == kCi8 && !h->d_y8) B2_CUDA(cudaMalloc(&h->d_y8, 2 * N));
   return B200DD_OK;
 }
 
@@ -588,7 +629,7 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
-  rc = host_staging(h, true, map_out != nullptr);
+  rc = host_staging(h, kC128, map_out != nullptr);
   if (rc == B200DD_OK) rc = tm_stamp(h, kTmExtract0, st);
   if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaMemcpyAsync(h->d_xd, x, sizeof(double2) * need_x, cudaMemcpyHostToDevice, st));
@@ -616,26 +657,63 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   return rc;
 }
 
-int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, uint32_t n, double *map_out) {
-  if (!h || !iq) return arg_fail("b200dd_pipeline_submit_host_rspduo: null argument");
-  uint32_t need, need_x;  // the CAF consumes n_used of the need_x instants
-  int rc = host_counts(h, n, &need, &need_x, "b200dd_pipeline_submit_host_rspduo: wrong number of samples",
-                       "b200dd_pipeline_submit_host_rspduo: the share-set member's last CPI is not fetched yet",
-                       "b200dd_pipeline_submit_host_rspduo: the spectrum stage needs nfft samples");
+}  // extern "C"
+
+// A host submit of capture-driver samples (int16, int8 or complex64, all exact in float32): the counts, the staging
+// and the stamp that opens extract_buffer, then ingest(need_x) -- the H2D copy of need_x instants of x and y and any
+// conversion into the complex64 d_xf, d_yf2 -- and the device chain on those, whose first stamp closes extract_buffer.
+// The CAF consumes n_used of the need_x instants.
+template <class Ingest>
+static int host_ingest(b200dd_pipeline *h, const char *entry, HostFormat fmt, uint32_t n, double *map_out,
+                       Ingest ingest) {
+  const std::string e = entry;
+  uint32_t need, need_x;
+  int rc = host_counts(h, n, &need, &need_x, (e + ": wrong number of samples").c_str(),
+                       (e + ": the share-set member's last CPI is not fetched yet").c_str(),
+                       (e + ": the spectrum stage needs nfft samples").c_str());
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  cudaStream_t st = h->stream;
-  rc = host_staging(h, false, map_out != nullptr);
-  if (rc == B200DD_OK) rc = tm_stamp(h, kTmExtract0, st);  // the device chain's first stamp closes extract_buffer
-  if (rc != B200DD_OK) return rc;
-  B2_CUDA(cudaMemcpyAsync(h->d_iq16, iq, sizeof(short4) * need_x, cudaMemcpyHostToDevice, st));
-  pl_ingest_rspduo_kernel<<<grid_for(need_x), 256, 0, st>>>(h->d_iq16, h->d_xf, h->d_yf2, need_x);
-  B2_LAUNCH_CHECK();
-  // int16 samples are exact in float32, so the float2 device path gives the same result as the
-  // complex128 host path
-  rc = pipeline_submit_device(h, h->d_xf, h->d_yf2, need_x, h->d_map, st);
-  if (rc == B200DD_OK) rc = host_submitted(h, kTmRspduo, map_out);
+  rc = host_staging(h, fmt, map_out != nullptr);
+  if (rc == B200DD_OK) rc = tm_stamp(h, kTmExtract0, h->stream);
+  if (rc == B200DD_OK) rc = ingest(need_x);
+  if (rc == B200DD_OK) rc = pipeline_submit_device(h, h->d_xf, h->d_yf2, need_x, h->d_map, h->stream);
+  if (rc == B200DD_OK) rc = host_submitted(h, kTmIngest, map_out);
   return rc;
+}
+
+extern "C" {
+
+int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, uint32_t n, double *map_out) {
+  if (!h || !iq) return arg_fail("b200dd_pipeline_submit_host_rspduo: null argument");
+  return host_ingest(h, "b200dd_pipeline_submit_host_rspduo", kInt16, n, map_out, [&](uint32_t m) -> int {
+    B2_CUDA(cudaMemcpyAsync(h->d_iq16, iq, sizeof(short4) * m, cudaMemcpyHostToDevice, h->stream));
+    pl_ingest_rspduo_kernel<<<grid_for(m), 256, 0, h->stream>>>(h->d_iq16, h->d_xf, h->d_yf2, m);
+    B2_LAUNCH_CHECK();
+    return B200DD_OK;
+  });
+}
+
+int b200dd_pipeline_submit_host_ci8(b200dd_pipeline *h, const int8_t *x_iq, const int8_t *y_iq, uint32_t n,
+                                    double *map_out) {
+  if (!h || !x_iq || !y_iq) return arg_fail("b200dd_pipeline_submit_host_ci8: null argument");
+  return host_ingest(h, "b200dd_pipeline_submit_host_ci8", kCi8, n, map_out, [&](uint32_t m) -> int {
+    B2_CUDA(cudaMemcpyAsync(h->d_x8, x_iq, 2 * (size_t)m, cudaMemcpyHostToDevice, h->stream));
+    B2_CUDA(cudaMemcpyAsync(h->d_y8, y_iq, 2 * (size_t)m, cudaMemcpyHostToDevice, h->stream));
+    pl_ingest_ci8_kernel<<<grid_for(m / 4 + m % 4), 256, 0, h->stream>>>(h->d_x8, h->d_y8, h->d_xf, h->d_yf2, m);
+    B2_LAUNCH_CHECK();
+    return B200DD_OK;
+  });
+}
+
+int b200dd_pipeline_submit_host_cf32(b200dd_pipeline *h, const float *x_iq, const float *y_iq, uint32_t n,
+                                     double *map_out) {
+  if (!h || !x_iq || !y_iq) return arg_fail("b200dd_pipeline_submit_host_cf32: null argument");
+  // complex64 is the device chain's own format: the samples go straight into its buffers
+  return host_ingest(h, "b200dd_pipeline_submit_host_cf32", kCf32, n, map_out, [&](uint32_t m) -> int {
+    B2_CUDA(cudaMemcpyAsync(h->d_xf, x_iq, sizeof(float2) * m, cudaMemcpyHostToDevice, h->stream));
+    B2_CUDA(cudaMemcpyAsync(h->d_yf2, y_iq, sizeof(float2) * m, cudaMemcpyHostToDevice, h->stream));
+    return B200DD_OK;
+  });
 }
 
 // The stateful stages' handles from the parameters their enable calls stored in `h`: a pipeline's own, and a share

@@ -59,6 +59,24 @@ def _c128(a):
     return np.ascontiguousarray(np.asarray(a, dtype=np.complex128))
 
 
+def _channel_count(name, x, y, dtypes, per_instant):
+    """The instant count n of two contiguous channel buffers (numpy arrays or torch tensors) of a dtype in `dtypes`
+    holding `per_instant` values per instant each; ValueError when they do not qualify or their counts differ."""
+    counts = []
+    for a in (x, y):
+        torch_like = hasattr(a, "numel")
+        dtype = str(a.dtype).replace("torch.", "")
+        if dtype not in dtypes or not (a.is_contiguous() if torch_like else a.flags.c_contiguous):
+            raise ValueError(f"{name}: channel buffers must be contiguous {' or '.join(dtypes)}, got {dtype}")
+        size = a.numel() if torch_like else a.size
+        if size % per_instant:
+            raise ValueError(f"{name}: {size} values are not whole instants of {per_instant}")
+        counts.append(size // per_instant)
+    if counts[0] != counts[1]:
+        raise ValueError(f"{name}: the channels hold {counts[0]} and {counts[1]} instants")
+    return counts[0]
+
+
 class Ambiguity:
     """Ambiguity(delayMin, delayMax, dopplerMin, dopplerMax, fs, n, roundHamming=False)
     -- src/process/ambiguity/Ambiguity.h:34."""
@@ -1023,6 +1041,24 @@ class Pipeline:
         self._pending_map = map_out
         capi.check(self._lib.b200dd_pipeline_submit_host_rspduo(self._h, capi.ptr(iq), int(n),
                                                                 capi.ptr(map_out) if map_out is not None else None))
+
+    def submit_host_ci8(self, x_iq, y_iq, map_out=None):
+        """Asynchronous host path fed with HackRF's / Kraken's format: reference and surveillance channel as two int8
+        arrays or tensors of 2n values (or shape (n, 2)), interleaved I, Q.  A uint8 buffer (rtl-sdr's bytes) is read
+        as int8, as blah2's Kraken source does: no offset is removed.  Pair with fetch(); the buffers must stay alive
+        (pinned for real overlap) until fetch() returns."""
+        n = _channel_count("submit_host_ci8", x_iq, y_iq, ("int8", "uint8"), 2)
+        self._pending_map = map_out
+        capi.check(self._lib.b200dd_pipeline_submit_host_ci8(self._h, capi.ptr(x_iq), capi.ptr(y_iq), int(n),
+                                                             capi.ptr(map_out) if map_out is not None else None))
+
+    def submit_host_cf32(self, x, y, map_out=None):
+        """Asynchronous host path fed with USRP's format: reference and surveillance channel as two complex64 arrays
+        or tensors of n samples.  Pair with fetch(), lifetimes as submit_host_ci8."""
+        n = _channel_count("submit_host_cf32", x, y, ("complex64",), 1)
+        self._pending_map = map_out
+        capi.check(self._lib.b200dd_pipeline_submit_host_cf32(self._h, capi.ptr(x), capi.ptr(y), int(n),
+                                                              capi.ptr(map_out) if map_out is not None else None))
 
     def submit_device(self, d_x, d_y, d_map=None, stream=None):
         n = d_x.numel() if hasattr(d_x, "numel") else self.n_samples

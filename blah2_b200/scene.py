@@ -8,7 +8,8 @@ values are exactly representable in float32, which is the device IQ format.
 
 ``write_rspduo`` / ``read_rspduo`` implement the reference's replay layout: little-endian
 int16 ``I1 Q1 I2 Q2`` per time instant (reader at
-test/unit/process/ambiguity/TestAmbiguity.cpp:39-69).
+test/unit/process/ambiguity/TestAmbiguity.cpp:39-69).  ``iq_from_ci8`` / ``iq_from_cf32`` state the samples blah2
+takes from its HackRF / Kraken (int8) and USRP (complex float32) sources.
 """
 from __future__ import annotations
 
@@ -79,6 +80,27 @@ def write_rspduo(path: str, x: np.ndarray, y: np.ndarray) -> None:
     buf[:, 2] = np.clip(np.round(y.real), -32768, 32767)
     buf[:, 3] = np.clip(np.round(y.imag), -32768, 32767)
     buf.tofile(path)
+
+
+def _complex(re: np.ndarray, im: np.ndarray) -> np.ndarray:
+    out = np.empty(re.shape[0], dtype=np.complex128)
+    out.real, out.imag = re, im  # not re + 1j * im, which loses the sign of a -0.0 imaginary part
+    return out
+
+
+def iq_from_ci8(buf) -> np.ndarray:
+    """The complex128 samples blah2 pushes into IqData from one channel's int8 I/Q buffer: every byte read as int8_t
+    and widened to double.  HackRF hands over int8 (src/capture/hackrf/HackRf.cpp:116-128); Kraken reads rtl-sdr's
+    offset-binary bytes through an int8_t pointer (src/capture/kraken/Kraken.cpp:97-112), so 0x80 becomes -128."""
+    b = np.ascontiguousarray(buf).view(np.int8).reshape(-1, 2).astype(np.float64)
+    return _complex(b[:, 0], b[:, 1])
+
+
+def iq_from_cf32(buf) -> np.ndarray:
+    """The complex128 samples blah2 pushes into IqData from one channel's UHD fc32 buffer
+    (src/capture/usrp/Usrp.cpp:54-91): each float widened to double."""
+    f = np.ascontiguousarray(buf).view(np.float32).reshape(-1, 2).astype(np.float64)
+    return _complex(f[:, 0], f[:, 1])
 
 
 def read_rspduo(path: str, n: int | None = None):

@@ -693,6 +693,24 @@ B200DD_API int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, 
  * in float32, so results equal the complex128 entry point's. */
 B200DD_API int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, uint32_t n, double *map_out);
 
+/* Same as b200dd_pipeline_submit_host_rspduo, fed with HackRF's and Kraken's sample format: x_iq (reference) and
+ * y_iq (surveillance) are two buffers of n time instants each, every instant an int8 pair I, Q.  HackRF delivers one
+ * such buffer per device (src/capture/hackrf/HackRf.cpp:116-128).  Kraken's rtl-sdr bytes are offset binary centred
+ * on 127.5, but blah2 reads them as int8_t (src/capture/kraken/Kraken.cpp:97-112), so a byte >= 0x80 is negative
+ * here too and no offset is removed.  4 bytes per instant cross PCIe; the conversion to complex64 runs on the
+ * device.  int8 is exact in float32, so results equal the int16 entry point's on the same values.  Asynchronous on
+ * the pipeline's stream; pair with b200dd_pipeline_fetch.  x_iq, y_iq and map_out (nullable) must stay valid until
+ * the fetch returns (pinned memory for overlap).  Errors as b200dd_pipeline_submit_host_rspduo's. */
+B200DD_API int b200dd_pipeline_submit_host_ci8(b200dd_pipeline *h, const int8_t *x_iq, const int8_t *y_iq, uint32_t n,
+                                               double *map_out);
+
+/* Same, fed with USRP's sample format: x_iq and y_iq are two buffers of n complex float32 samples (I, Q) each, the
+ * UHD fc32 host format blah2 receives (src/capture/usrp/Usrp.cpp:54-91).  16 bytes per instant cross PCIe, copied
+ * straight into the device chain's complex64 buffers; results equal b200dd_pipeline_submit_device's on the same
+ * samples.  Asynchronous, lifetimes and errors as b200dd_pipeline_submit_host_ci8's. */
+B200DD_API int b200dd_pipeline_submit_host_cf32(b200dd_pipeline *h, const float *x_iq, const float *y_iq, uint32_t n,
+                                                double *map_out);
+
 /* DEVICE buffers (float2), asynchronous on `stream` (NULL = the pipeline's stream).  d_map
  * (nullable) receives the float2 map.  Results stay on the device until b200dd_pipeline_fetch. */
 B200DD_API int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n,
