@@ -712,7 +712,7 @@ struct b200dd_caf {
   b200dd_caf_params params;
   HostGeom g;
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   // range stage plan
   int log2m = 12, nSeg = 1, L = 0, nParts = 1, segPerPart = 1;
   int num_sms = 132;
@@ -720,12 +720,12 @@ struct b200dd_caf {
   int log2m2 = 10;
   RangeKernel range;  // the kernels of (log2m, log2m2)
   DopplerKernels dop;
-  float2 *d_tw1 = nullptr, *d_tw2 = nullptr, *d_chirp = nullptr, *d_bhat = nullptr;
-  float2 *d_R = nullptr, *d_map = nullptr;
-  float2 *d_xrot = nullptr;                      // device path, dopplerMiddle != 0
-  double2 *d_xd = nullptr, *d_yd = nullptr;      // host path staging
-  float2 *d_xf = nullptr, *d_yf = nullptr;
-  double2 *d_mapd = nullptr;
+  DevBuf<float2> d_tw1, d_tw2, d_chirp, d_bhat;
+  DevBuf<float2> d_R, d_map;
+  DevBuf<float2> d_xrot;        // device path, dopplerMiddle != 0
+  DevBuf<double2> d_xd, d_yd;   // host path staging
+  DevBuf<float2> d_xf, d_yf;
+  DevBuf<double2> d_mapd;
   uint32_t n_stage = 0;
 };
 
@@ -786,11 +786,11 @@ int caf_setup_device(b200dd_caf *h) {
   if (rc == B200DD_OK) rc = h->dop.doppler.set_smem_limit();
   if (rc == B200DD_OK) rc = h->dop.fft_forward.set_smem_limit();
   if (rc != B200DD_OK) return rc;
-  B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  B2_CUDA(h->stream.create());
   const int M1 = 1 << h->log2m, M2 = 1 << h->log2m2;
   auto tw1 = twiddle_table_f32(M1), tw2 = twiddle_table_f32(M2);
-  B2_CUDA(cudaMalloc(&h->d_tw1, sizeof(float2) * M1));
-  B2_CUDA(cudaMalloc(&h->d_tw2, sizeof(float2) * M2));
+  B2_CUDA(h->d_tw1.alloc(M1));
+  B2_CUDA(h->d_tw2.alloc(M2));
   B2_CUDA(cudaMemcpy(h->d_tw1, tw1.data(), sizeof(float2) * M1, cudaMemcpyHostToDevice));
   B2_CUDA(cudaMemcpy(h->d_tw2, tw2.data(), sizeof(float2) * M2, cudaMemcpyHostToDevice));
   // Bluestein chirp c[k] = exp(-i pi k^2 / n), k^2 reduced mod 2n exactly
@@ -805,23 +805,23 @@ int caf_setup_device(b200dd_caf *h) {
     bw[k] = make_float2(c, s);  // conj(chirp)
     if (k) bw[M2 - k] = make_float2(c, s);
   }
-  B2_CUDA(cudaMalloc(&h->d_chirp, sizeof(float2) * n));
+  B2_CUDA(h->d_chirp.alloc(n));
   B2_CUDA(cudaMemcpy(h->d_chirp, chirp.data(), sizeof(float2) * n, cudaMemcpyHostToDevice));
-  float2 *d_bw = nullptr;
-  B2_CUDA(cudaMalloc(&d_bw, sizeof(float2) * M2));
-  B2_CUDA(cudaMalloc(&h->d_bhat, sizeof(float2) * M2));
+  DevBuf<float2> d_bw;
+  B2_CUDA(d_bw.alloc(M2));
+  B2_CUDA(h->d_bhat.alloc(M2));
   B2_CUDA(cudaMemcpy(d_bw, bw.data(), sizeof(float2) * M2, cudaMemcpyHostToDevice));
   rc = h->dop.fft_forward.launch(1, h->stream, d_bw, h->d_bhat, h->d_tw2);
-  if (rc != B200DD_OK) { cudaFree(d_bw); return rc; }
+  if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaStreamSynchronize(h->stream));
-  cudaFree(d_bw);
-  B2_CUDA(cudaMalloc(&h->d_R, sizeof(float2) * (size_t)h->nParts * g.nDop * g.nDel));
-  B2_CUDA(cudaMalloc(&h->d_map, sizeof(float2) * (size_t)g.nDop * g.nDel));
+  d_bw.reset();
+  B2_CUDA(h->d_R.alloc((size_t)h->nParts * g.nDop * g.nDel));
+  B2_CUDA(h->d_map.alloc((size_t)g.nDop * g.nDel));
   return B200DD_OK;
 }
 
 int caf_run_device(b200dd_caf *h, const float2 *d_x, const float2 *d_y, float2 *d_map, cudaStream_t st,
-                   cudaEvent_t *ev = nullptr) {
+                   const Event *ev = nullptr) {
   const HostGeom &g = h->g;
   RangeArgs ra;
   ra.x = d_x;
@@ -919,43 +919,21 @@ int b200dd_caf_plan(const b200dd_caf_params *params, b200dd_caf_geometry *out, i
 int b200dd_caf_create(const b200dd_caf_params *params, b200dd_caf **out) {
   if (!params || !out) return arg_fail("b200dd_caf_create: null argument");
   *out = nullptr;
-  b200dd_caf *h = new (std::nothrow) b200dd_caf();
+  Owned<b200dd_caf> h(new (std::nothrow) b200dd_caf(), b200dd_caf_destroy);
   if (!h) return arg_fail("b200dd_caf_create: out of host memory");
-  auto fail = [&](int rc) { b200dd_caf_destroy(h); return rc; };
-  int rc = caf_host_plan(params, h);
-  if (rc != B200DD_OK) return fail(rc);
-  int dev = params->device;
-  if (dev < 0) {
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  }
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
-  rc = caf_setup_device(h);
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  if (int rc = caf_host_plan(params, h.get())) return rc;
+  if (int rc = resolve_device(params->device, &h->device)) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+  if (int rc = caf_setup_device(h.get())) return rc;
+  *out = h.release();
   return B200DD_OK;
 }
 
 void b200dd_caf_destroy(b200dd_caf *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_dev(h->d_tw1);
-    free_dev(h->d_tw2);
-    free_dev(h->d_chirp);
-    free_dev(h->d_bhat);
-    free_dev(h->d_R);
-    free_dev(h->d_map);
-    free_dev(h->d_xrot);
-    free_dev(h->d_xd);
-    free_dev(h->d_yd);
-    free_dev(h->d_xf);
-    free_dev(h->d_yf);
-    free_dev(h->d_mapd);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
@@ -990,10 +968,10 @@ int b200dd_caf_process_device(b200dd_caf *h, const void *d_x, const void *d_y, u
   const uint32_t n_used = h->g.nDop * h->g.nCorr;
   if (n < n_used) return arg_fail("b200dd_caf_process_device: fewer samples than nDopplerBins * nCorr");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   const float2 *x = (const float2 *)d_x;
   if (h->g.dopplerMiddle != 0.0) {
-    if (!h->d_xrot) B2_CUDA(cudaMalloc(&h->d_xrot, sizeof(float2) * n_used));
+    if (!h->d_xrot) B2_CUDA(h->d_xrot.alloc(n_used));
     caf_prerotate_kernel<<<grid_for(n_used), 256, 0, st>>>(x, h->d_xrot, n_used, h->g.dopplerMiddle, (double)h->g.fs);
     B2_LAUNCH_CHECK();
     x = h->d_xrot;
@@ -1009,15 +987,14 @@ int b200dd_caf_process_host(b200dd_caf *h, const double *x, const double *y, uin
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
   if (h->n_stage < n_used) {
-    free_dev(h->d_xd); free_dev(h->d_yd); free_dev(h->d_xf); free_dev(h->d_yf);
-    B2_CUDA(cudaMalloc(&h->d_xd, sizeof(double2) * n_used));
-    B2_CUDA(cudaMalloc(&h->d_yd, sizeof(double2) * n_used));
-    B2_CUDA(cudaMalloc(&h->d_xf, sizeof(float2) * n_used));
-    B2_CUDA(cudaMalloc(&h->d_yf, sizeof(float2) * n_used));
+    B2_CUDA(h->d_xd.alloc(n_used));
+    B2_CUDA(h->d_yd.alloc(n_used));
+    B2_CUDA(h->d_xf.alloc(n_used));
+    B2_CUDA(h->d_yf.alloc(n_used));
     h->n_stage = n_used;
   }
   const size_t cells = (size_t)g.nDop * g.nDel;
-  if (!h->d_mapd) B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * cells));
+  if (!h->d_mapd) B2_CUDA(h->d_mapd.alloc(cells));
   B2_CUDA(cudaMemcpyAsync(h->d_xd, x, sizeof(double2) * n_used, cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemcpyAsync(h->d_yd, y, sizeof(double2) * n_used, cudaMemcpyHostToDevice, st));
   caf_convert_kernel<<<grid_for(n_used), 256, 0, st>>>(h->d_xd, h->d_xf, n_used, g.dopplerMiddle, (double)g.fs);
@@ -1039,17 +1016,15 @@ int b200dd_caf_profile_device(b200dd_caf *h, const void *d_x, const void *d_y, u
   if (n < h->g.nDop * h->g.nCorr) return arg_fail("b200dd_caf_profile_device: too few samples");
   if (h->g.dopplerMiddle != 0.0) return arg_fail("b200dd_caf_profile_device: symmetric Doppler windows only");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  cudaEvent_t ev[3];
-  for (int i = 0; i < 3; i++) B2_CUDA(cudaEventCreate(&ev[i]));
-  int rc = caf_run_device(h, (const float2 *)d_x, (const float2 *)d_y, d_map ? (float2 *)d_map : h->d_map, st, ev);
-  if (rc == B200DD_OK) {
-    B2_CUDA(cudaEventSynchronize(ev[2]));
-    B2_CUDA(cudaEventElapsedTime(ms_range, ev[0], ev[1]));
-    B2_CUDA(cudaEventElapsedTime(ms_doppler, ev[1], ev[2]));
-  }
-  for (int i = 0; i < 3; i++) cudaEventDestroy(ev[i]);
-  return rc;
+  cudaStream_t st = stream_or(stream, h->stream);
+  Event ev[3];
+  for (auto &e : ev) B2_CUDA(e.create());
+  if (int rc = caf_run_device(h, (const float2 *)d_x, (const float2 *)d_y, d_map ? (float2 *)d_map : h->d_map, st, ev))
+    return rc;
+  B2_CUDA(cudaEventSynchronize(ev[2]));
+  B2_CUDA(cudaEventElapsedTime(ms_range, ev[0], ev[1]));
+  B2_CUDA(cudaEventElapsedTime(ms_doppler, ev[1], ev[2]));
+  return B200DD_OK;
 }
 
 int b200dd_caf_range_device(b200dd_caf *h, const void *d_x, const void *d_y, uint32_t batch0, uint32_t n_batches,
@@ -1059,7 +1034,7 @@ int b200dd_caf_range_device(b200dd_caf *h, const void *d_x, const void *d_y, uin
   if (n_batches == 0 || (uint64_t)batch0 + n_batches > g.nDop) return arg_fail("b200dd_caf_range_device: batch range outside the CPI");
   if (g.dopplerMiddle != 0.0) return geom_fail("b200dd_caf_range_device: symmetric Doppler windows only");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   RangeArgs ra;
   // the kernel indexes batches absolutely; the caller hands over the slice that STARTS at batch0
   ra.x = (const float2 *)d_x - (size_t)batch0 * g.nCorr;
@@ -1084,7 +1059,7 @@ int b200dd_caf_doppler_device(b200dd_caf *h, const void *d_R, uint32_t col0, uin
   const HostGeom &g = h->g;
   if (n_cols == 0 || (uint64_t)col0 + n_cols > g.nDel) return arg_fail("b200dd_caf_doppler_device: column range outside the map");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   DopplerArgs da;
   da.R = (const float2 *)d_R; da.nParts = 1; da.out = (float2 *)d_map_tile; da.chirp = h->d_chirp; da.bhat = h->d_bhat;
   da.tw = h->d_tw2; da.nDop = (int)g.nDop; da.nDel = (int)g.nDel; da.col0 = (int)col0; da.nCols = (int)n_cols;
@@ -1097,7 +1072,7 @@ int b200dd_caf_place_tile_device(b200dd_caf *h, const void *d_tile, uint32_t col
   const HostGeom &g = h->g;
   if (n_cols == 0 || (uint64_t)col0 + n_cols > g.nDel) return arg_fail("b200dd_caf_place_tile_device: column range outside the map");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   B2_CUDA(cudaMemcpy2DAsync((float2 *)d_map + col0, sizeof(float2) * g.nDel, d_tile, sizeof(float2) * n_cols, sizeof(float2) * n_cols,
                             g.nDop, cudaMemcpyDeviceToDevice, st));
   return B200DD_OK;
@@ -1108,7 +1083,7 @@ int b200dd_caf_place_tiles_device(b200dd_caf *h, const void *d_tiles, uint32_t n
   const HostGeom &g = h->g;
   if (n_tiles == 0 || n_tiles > g.nDel) return arg_fail("b200dd_caf_place_tiles_device: bad tile count");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   caf_place_tiles_kernel<<<grid_for(g.nDop * g.nDel), 256, 0, st>>>((const float2 *)d_tiles, (int)n_tiles, (int)g.nDop, (int)g.nDel,
                                                                      (float2 *)d_map);
   B2_LAUNCH_CHECK();

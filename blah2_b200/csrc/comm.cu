@@ -98,9 +98,9 @@ int nccl_fail(ncclResult_t r, const char *what) {
 
 struct b200dd_comm {
   int rank = 0, world = 1, device = 0;
+  Stream stream;
+  Event ev_in, ev_out;
   ncclComm_t comm = nullptr;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
 };
 
 namespace {
@@ -134,46 +134,33 @@ int b200dd_comm_create(int32_t rank, int32_t world, const uint8_t *id128, int32_
   if (world < 1 || rank < 0 || rank >= world) return arg_fail("b200dd_comm_create: bad rank / world");
   NcclApi &a = nccl_api();
   if (!a.error.empty()) { set_last_error(a.error); return B200DD_ERR_CUDA; }
-  b200dd_comm *c = new (std::nothrow) b200dd_comm();
+  Owned<b200dd_comm> c(new (std::nothrow) b200dd_comm(), b200dd_comm_destroy);
   if (!c) return arg_fail("b200dd_comm_create: out of host memory");
   c->rank = rank;
   c->world = world;
-  int dev = device;
-  auto fail = [&](int rc) { b200dd_comm_destroy(c); return rc; };
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  c->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    B2_CUDA(cudaEventCreateWithFlags(&c->ev_in, cudaEventDisableTiming));
-    B2_CUDA(cudaEventCreateWithFlags(&c->ev_out, cudaEventDisableTiming));
-    ncclUniqueId id;
-    memcpy(id.internal, id128, 128);
-    // The exchanges of this path are small (a map, a range matrix, a halo) and run BESIDE kernels that need whole SMs
-    // (255 registers x 256 threads): every channel is a resident CTA that spins while it waits for its peer.  Two
-    // point-to-point channels carry the ~1 MB messages at NVLink speed; the caller's own NCCL_* settings win.
-    setenv("NCCL_MAX_P2P_NCHANNELS", "2", 0);
-    setenv("NCCL_MIN_P2P_NCHANNELS", "1", 0);
-    B2_NCCL(a.CommInitRank(&c->comm, world, id, rank));
-    return B200DD_OK;
-  };
-  const int rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = c;
+  if (int rc = resolve_device(device, &c->device)) return rc;
+  DeviceGuard guard(c->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+  B2_CUDA(c->stream.create());
+  B2_CUDA(c->ev_in.create(cudaEventDisableTiming));
+  B2_CUDA(c->ev_out.create(cudaEventDisableTiming));
+  ncclUniqueId id;
+  memcpy(id.internal, id128, 128);
+  // The exchanges of this path are small (a map, a range matrix, a halo) and run BESIDE kernels that need whole SMs
+  // (255 registers x 256 threads): every channel is a resident CTA that spins while it waits for its peer.  Two
+  // point-to-point channels carry the ~1 MB messages at NVLink speed; the caller's own NCCL_* settings win.
+  setenv("NCCL_MAX_P2P_NCHANNELS", "2", 0);
+  setenv("NCCL_MIN_P2P_NCHANNELS", "1", 0);
+  B2_NCCL(a.CommInitRank(&c->comm, world, id, rank));
+  *out = c.release();
   return B200DD_OK;
 }
 
 void b200dd_comm_destroy(b200dd_comm *c) {
   if (!c) return;
-  {
-    DeviceGuard guard(c->device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    if (c->comm) nccl_api().CommDestroy(c->comm);
-    if (c->ev_in) cudaEventDestroy(c->ev_in);
-    if (c->ev_out) cudaEventDestroy(c->ev_out);
-    if (c->stream) cudaStreamDestroy(c->stream);
-  }
+  DeviceGuard guard(c->device);  // held while the members go
+  if (c->stream) cudaStreamSynchronize(c->stream);
+  if (c->comm) nccl_api().CommDestroy(c->comm);
   delete c;
 }
 

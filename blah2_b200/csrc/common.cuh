@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 #include <cstdio>
+#include <memory>
 #include <string>
 
 #include "../../include/b200dd.h"
@@ -65,10 +66,84 @@ struct DeviceGuard {
   }
 };
 
-template <class T> inline void free_dev(T *&p) {
-  if (p) cudaFree(p);
-  p = nullptr;
+// Owning device array of T: alloc(n) frees what it held and allocates n elements (check it with B2_CUDA); reset()
+// frees; the destructor frees.  Converts to T*, so kernels and copies take it as they would the raw pointer.  The
+// handles' destroy functions keep their DeviceGuard alive while the members free.
+template <class T> class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+  DevBuf &operator=(DevBuf &&o) noexcept {
+    if (this != &o) {
+      reset();
+      p_ = o.p_;
+      o.p_ = nullptr;
+    }
+    return *this;
+  }
+  ~DevBuf() { reset(); }
+  cudaError_t alloc(size_t n) {
+    reset();
+    return cudaMalloc(&p_, sizeof(T) * n);
+  }
+  void reset() {
+    if (p_) cudaFree(p_);
+    p_ = nullptr;
+  }
+  T *get() const { return p_; }
+  operator T *() const { return p_; }
+  T *operator->() const { return p_; }  // device addresses of members: &buf->field
+
+ private:
+  T *p_ = nullptr;
+};
+
+// Owning CUDA stream (non-blocking) and event; create() is checked with B2_CUDA, the destructor destroys.
+class Stream {
+ public:
+  Stream() = default;
+  Stream(const Stream &) = delete;
+  Stream &operator=(const Stream &) = delete;
+  ~Stream() {
+    if (s_) cudaStreamDestroy(s_);
+  }
+  cudaError_t create() { return cudaStreamCreateWithFlags(&s_, cudaStreamNonBlocking); }
+  operator cudaStream_t() const { return s_; }
+
+ private:
+  cudaStream_t s_ = nullptr;
+};
+
+class Event {
+ public:
+  Event() = default;
+  Event(const Event &) = delete;
+  Event &operator=(const Event &) = delete;
+  ~Event() {
+    if (e_) cudaEventDestroy(e_);
+  }
+  cudaError_t create(unsigned flags = cudaEventDefault) { return cudaEventCreateWithFlags(&e_, flags); }
+  operator cudaEvent_t() const { return e_; }
+
+ private:
+  cudaEvent_t e_ = nullptr;
+};
+
+// *dev = requested, or the current device when requested < 0.
+inline int resolve_device(int requested, int *dev) {
+  *dev = requested;
+  if (requested < 0 && cudaGetDevice(dev) != cudaSuccess)
+    return cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__);
+  return B200DD_OK;
 }
+
+// the caller's stream, else the handle's own
+inline cudaStream_t stream_or(void *stream, cudaStream_t own) { return stream ? (cudaStream_t)stream : own; }
+
+// A handle under construction, released into *out on success; a failed create frees it with the handle's destroy.
+template <class H> using Owned = std::unique_ptr<H, void (*)(H *)>;
 
 // Hooks between translation units that the C ABI does not expose.
 // det.cu: device address of {noisePower, maxPower} as the async chain's set_metrics leaves them.

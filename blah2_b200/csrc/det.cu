@@ -397,18 +397,18 @@ template <class TMAP> __global__ void __launch_bounds__(1024) det_tail_kernel(Ta
 struct b200dd_det {
   b200dd_det_params p;
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   uint32_t maxDop = 0, maxDel = 0, cap = 0;
   int nGuard = 0, nTrain = 0, minDelay = 0;  // after the reference's int8_t narrowing
-  double *d_alpha = nullptr;
-  int32_t *d_delay = nullptr;
-  double *d_doppler = nullptr;
-  uint32_t *d_mask = nullptr, *d_cnt = nullptr, *d_off = nullptr, *d_n = nullptr;  // d_n[0..3] stage counts
-  double *d_buf[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};
-  uint8_t *d_keep = nullptr;
-  double2 *d_mapd = nullptr;  // host-map path (grown on demand)
+  DevBuf<double> d_alpha;
+  DevBuf<int32_t> d_delay;
+  DevBuf<double> d_doppler;
+  DevBuf<uint32_t> d_mask, d_cnt, d_off, d_n;  // d_n[0..3] stage counts
+  DevBuf<double> d_buf[2][3];
+  DevBuf<uint8_t> d_keep;
+  DevBuf<double2> d_mapd;  // host-map path (grown on demand)
   size_t mapd_cells = 0;
-  double *d_part = nullptr, *d_metrics = nullptr;
+  DevBuf<double> d_part, d_metrics;
   int nPart = 592;
   std::vector<int32_t> axes_delay;   // host copies of what d_delay / d_doppler hold
   std::vector<double> axes_doppler;
@@ -551,7 +551,7 @@ int b200dd_det_create(const b200dd_det_params *params, uint32_t max_doppler_bins
   *out = nullptr;
   if (max_doppler_bins == 0 || max_delay_bins == 0) return arg_fail("b200dd_det_create: empty map");
   if (max_delay_bins > 16384) return geom_fail("b200dd_det_create: more than 16384 delay bins unsupported");
-  b200dd_det *h = new (std::nothrow) b200dd_det();
+  Owned<b200dd_det> h(new (std::nothrow) b200dd_det(), b200dd_det_destroy);
   if (!h) return arg_fail("b200dd_det_create: out of host memory");
   h->p = *params;
   h->nGuard = (int8_t)params->n_guard;      // CfarDetector1D.h:46: int8_t parameters
@@ -561,63 +561,39 @@ int b200dd_det_create(const b200dd_det_params *params, uint32_t max_doppler_bins
   h->maxDel = max_delay_bins;
   const uint64_t cells = (uint64_t)max_doppler_bins * max_delay_bins;
   h->cap = (uint32_t)(cells < kMaxDetections ? cells : kMaxDetections);
-  auto fail = [&](int rc) { b200dd_det_destroy(h); return rc; };
-  int dev = params->device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    // alpha[n] = n (pfa^(-1/n) - 1), CfarDetector1D.cpp:76, same libm as the reference's host code
-    const int nt = h->nTrain > 0 ? h->nTrain : 0;
-    std::vector<double> alpha(2 * nt + 2, 0.0);
-    for (int n = 1; n <= 2 * nt; n++) alpha[n] = n * (pow(params->pfa, -1.0 / n) - 1);
-    B2_CUDA(cudaMalloc(&h->d_alpha, sizeof(double) * alpha.size()));
-    B2_CUDA(cudaMemcpy(h->d_alpha, alpha.data(), sizeof(double) * alpha.size(), cudaMemcpyHostToDevice));
-    B2_CUDA(cudaMalloc(&h->d_delay, sizeof(int32_t) * h->maxDel));
-    B2_CUDA(cudaMalloc(&h->d_doppler, sizeof(double) * h->maxDop));
-    const size_t words = (h->maxDel + 31) / 32;
-    B2_CUDA(cudaMalloc(&h->d_mask, sizeof(uint32_t) * words * h->maxDop));
-    B2_CUDA(cudaMalloc(&h->d_cnt, sizeof(uint32_t) * (h->maxDop + 1)));
-    B2_CUDA(cudaMalloc(&h->d_off, sizeof(uint32_t) * (h->maxDop + 1)));
-    B2_CUDA(cudaMalloc(&h->d_n, sizeof(uint32_t) * 4));
-    B2_CUDA(cudaMemset(h->d_n, 0, sizeof(uint32_t) * 4));
-    for (int b = 0; b < 2; b++)
-      for (int k = 0; k < 3; k++) B2_CUDA(cudaMalloc(&h->d_buf[b][k], sizeof(double) * h->cap));
-    B2_CUDA(cudaMalloc(&h->d_keep, h->cap));
-    B2_CUDA(cudaMalloc(&h->d_part, sizeof(double) * 2 * h->nPart));
-    B2_CUDA(cudaMalloc(&h->d_metrics, sizeof(double) * 2));
-    B2_CUDA(cudaFuncSetAttribute(cfar_flag_kernel<float2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * 16384)));  // per function, not per handle: always the supported maximum
-    B2_CUDA(cudaFuncSetAttribute(cfar_flag_kernel<double2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * 16384)));
-    return B200DD_OK;
-  };
-  int rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  if (int rc = resolve_device(params->device, &h->device)) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+  B2_CUDA(h->stream.create());
+  // alpha[n] = n (pfa^(-1/n) - 1), CfarDetector1D.cpp:76, same libm as the reference's host code
+  const int nt = h->nTrain > 0 ? h->nTrain : 0;
+  std::vector<double> alpha(2 * nt + 2, 0.0);
+  for (int n = 1; n <= 2 * nt; n++) alpha[n] = n * (pow(params->pfa, -1.0 / n) - 1);
+  B2_CUDA(h->d_alpha.alloc(alpha.size()));
+  B2_CUDA(cudaMemcpy(h->d_alpha, alpha.data(), sizeof(double) * alpha.size(), cudaMemcpyHostToDevice));
+  B2_CUDA(h->d_delay.alloc(h->maxDel));
+  B2_CUDA(h->d_doppler.alloc(h->maxDop));
+  const size_t words = (h->maxDel + 31) / 32;
+  B2_CUDA(h->d_mask.alloc(words * h->maxDop));
+  B2_CUDA(h->d_cnt.alloc(h->maxDop + 1));
+  B2_CUDA(h->d_off.alloc(h->maxDop + 1));
+  B2_CUDA(h->d_n.alloc(4));
+  B2_CUDA(cudaMemset(h->d_n, 0, sizeof(uint32_t) * 4));
+  for (auto &list : h->d_buf)
+    for (auto &b : list) B2_CUDA(b.alloc(h->cap));
+  B2_CUDA(h->d_keep.alloc(h->cap));
+  B2_CUDA(h->d_part.alloc(2 * h->nPart));
+  B2_CUDA(h->d_metrics.alloc(2));
+  B2_CUDA(cudaFuncSetAttribute(cfar_flag_kernel<float2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * 16384)));  // per function, not per handle: always the supported maximum
+  B2_CUDA(cudaFuncSetAttribute(cfar_flag_kernel<double2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * 16384)));
+  *out = h.release();
   return B200DD_OK;
 }
 
 void b200dd_det_destroy(b200dd_det *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_dev(h->d_alpha);
-    free_dev(h->d_delay);
-    free_dev(h->d_doppler);
-    free_dev(h->d_mask);
-    free_dev(h->d_cnt);
-    free_dev(h->d_off);
-    free_dev(h->d_n);
-    for (int b = 0; b < 2; b++)
-      for (int k = 0; k < 3; k++) free_dev(h->d_buf[b][k]);
-    free_dev(h->d_keep);
-    free_dev(h->d_mapd);
-    free_dev(h->d_part);
-    free_dev(h->d_metrics);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
@@ -625,7 +601,7 @@ int b200dd_det_set_metrics_device(b200dd_det *h, const void *d_map, uint32_t n_d
                                   void *stream) {
   if (!h || !d_map || !metrics) return arg_fail("b200dd_det_set_metrics_device: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   const size_t cells = (size_t)n_dop * n_del;
   int grid = (int)((cells + kBlock - 1) / kBlock);
   if (grid > h->nPart) grid = h->nPart;
@@ -647,7 +623,7 @@ int b200dd_det_process_device(b200dd_det *h, int last_stage, const void *d_map, 
   int rc = check_dims(h, n_dop, n_del);
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   int buf = 0, slot = 0;
   rc = run_chain<float2>(h, last_stage, (const float2 *)d_map, n_dop, n_del, delay, doppler, noise_power, nullptr, st, &buf, &slot);
   if (rc != B200DD_OK) return rc;
@@ -661,7 +637,7 @@ int b200dd_det_chain_device_async(b200dd_det *h, int last_stage, const void *d_m
   int rc = check_dims(h, n_dop, n_del);
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   const size_t cells = (size_t)n_dop * n_del;
   int grid = (int)((cells + kBlock - 1) / kBlock);
   if (grid > h->nPart) grid = h->nPart;
@@ -687,7 +663,7 @@ int b200dd_det_chain_fetch(b200dd_det *h, double *metrics, double *o_delay, doub
   if (!h) return arg_fail("b200dd_det_chain_fetch: null handle");
   if (cap && (!o_delay || !o_doppler || !o_snr)) return arg_fail("b200dd_det_chain_fetch: null output");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   if (metrics) B2_CUDA(cudaMemcpyAsync(metrics, h->d_metrics, sizeof(double) * 2, cudaMemcpyDeviceToHost, st));
   return fetch_results(h, h->chain_buf, h->chain_slot, o_delay, o_doppler, o_snr, cap, n_out, st, true);
 }
@@ -703,8 +679,7 @@ int b200dd_det_process_host(b200dd_det *h, int last_stage, const double *map, ui
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
   if (h->mapd_cells < (size_t)n_dop * n_del) {
-    free_dev(h->d_mapd);
-    B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * (size_t)n_dop * n_del));
+    B2_CUDA(h->d_mapd.alloc((size_t)n_dop * n_del));
     h->mapd_cells = (size_t)n_dop * n_del;
   }
   B2_CUDA(cudaMemcpyAsync(h->d_mapd, map, sizeof(double2) * (size_t)n_dop * n_del, cudaMemcpyHostToDevice, st));
@@ -753,8 +728,7 @@ int b200dd_det_interpolate_host(b200dd_det *h, const double *delay, const double
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
   if (h->mapd_cells < (size_t)n_dop * n_del) {
-    free_dev(h->d_mapd);
-    B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * (size_t)n_dop * n_del));
+    B2_CUDA(h->d_mapd.alloc((size_t)n_dop * n_del));
     h->mapd_cells = (size_t)n_dop * n_del;
   }
   B2_CUDA(cudaMemcpyAsync(h->d_mapd, map, sizeof(double2) * (size_t)n_dop * n_del, cudaMemcpyHostToDevice, st));

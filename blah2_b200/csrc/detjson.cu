@@ -219,21 +219,21 @@ const char *const kStashHead[4] = {"{\"timestamp\":[", "],\"delay\":[", "],\"dop
 
 struct b200dd_detjson {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   uint32_t fs = 0, ring_cap = 0, stash_tiles = 0;
   size_t max_bytes = 0, stash_max_bytes = 0;
   // per-CPI render
-  char *d_body = nullptr;
-  uint32_t *d_tile_len = nullptr, *d_tile_off = nullptr;  // [3 kDocTiles], [3 kDocTiles + 1]
-  DjInfo *d_info = nullptr;
-  DjRing *d_ring_state = nullptr;
+  DevBuf<char> d_body;
+  DevBuf<uint32_t> d_tile_len, d_tile_off;  // [3 kDocTiles], [3 kDocTiles + 1]
+  DevBuf<DjInfo> d_info;
+  DevBuf<DjRing> d_ring_state;
   bool pending = false;  // a render not fetched yet
   // stash
-  int32_t *d_ring = nullptr;  // [3][ring_cap]
-  char *d_stash = nullptr;
-  uint32_t *d_stile_len = nullptr, *d_stile_off = nullptr;
-  uint32_t *d_doc_first = nullptr, *d_doc_text = nullptr;
-  char *d_texts = nullptr;
+  DevBuf<int32_t> d_ring;  // [3][ring_cap]
+  DevBuf<char> d_stash;
+  DevBuf<uint32_t> d_stile_len, d_stile_off;
+  DevBuf<uint32_t> d_doc_first, d_doc_text;
+  DevBuf<char> d_texts;
   size_t first_alloc = 0, toff_alloc = 0, texts_alloc = 0;  // elements allocated
   struct Record {
     uint64_t ts, first;  // first: absolute entry number
@@ -294,12 +294,11 @@ int commit_shared(b200dd_detjson *h, uint64_t ts, uint32_t n, cudaStream_t st) {
 }
 
 // device array p of `have` elements grown to at least `need` (doubling), contents not kept
-template <class T> int grow(T *&p, size_t &have, size_t need) {
+template <class T> int grow(DevBuf<T> &p, size_t &have, size_t need) {
   if (need <= have) return B200DD_OK;
-  free_dev(p);
   have = 0;
   const size_t n = need * 2;
-  B2_CUDA(cudaMalloc(&p, sizeof(T) * n));
+  B2_CUDA(p.alloc(n));
   have = n;
   return B200DD_OK;
 }
@@ -318,12 +317,12 @@ int b2::detjson_share(b200dd_detjson *h, b200dd_detjson *hist) {
   const int rc = upload_ring_state(h, h->stream);  // {0, ring_cap}: every render stages at [0, n)
   if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaStreamSynchronize(h->stream));
-  free_dev(h->d_stash);  // the stash is rendered from hist
-  free_dev(h->d_stile_len);
-  free_dev(h->d_stile_off);
-  free_dev(h->d_doc_first);
-  free_dev(h->d_doc_text);
-  free_dev(h->d_texts);
+  h->d_stash.reset();  // the stash is rendered from hist
+  h->d_stile_len.reset();
+  h->d_stile_off.reset();
+  h->d_doc_first.reset();
+  h->d_doc_text.reset();
+  h->d_texts.reset();
   h->first_alloc = h->toff_alloc = h->texts_alloc = 0;
   h->hist = hist;
   return B200DD_OK;
@@ -351,9 +350,8 @@ int b200dd_detjson_create(uint32_t fs, uint32_t max_held, int32_t device, b200dd
   *out = nullptr;
   if (fs == 0) return arg_fail("b200dd_detjson_create: fs must be positive");
   if (max_held == 0 || max_held > kMaxHeld) return arg_fail("b200dd_detjson_create: max_held must be in [1, 2^25]");
-  b200dd_detjson *h = new (std::nothrow) b200dd_detjson();
+  Owned<b200dd_detjson> h(new (std::nothrow) b200dd_detjson(), b200dd_detjson_destroy);
   if (!h) return arg_fail("b200dd_detjson_create: out of host memory");
-  auto fail = [&](int rc) { b200dd_detjson_destroy(h); return rc; };
   h->fs = fs;
   h->ring_cap = max_held;
   h->stash_tiles = (max_held + kTile - 1) / kTile;
@@ -362,30 +360,22 @@ int b200dd_detjson_create(uint32_t fs, uint32_t max_held, int32_t device, b200dd
                  strlen(kDocHead[2]) + 2 + 3 * (size_t)kListCap * kDocItemMax;
   h->stash_max_bytes = strlen(kStashHead[0]) + strlen(kStashHead[1]) + strlen(kStashHead[2]) +
                        strlen(kStashHead[3]) + 2 + (size_t)max_held * (kStashItemMax + 3 * (jf::kMaxHundredthsText + 1));
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    B2_CUDA(cudaMalloc(&h->d_body, (3 * (size_t)kListCap * kDocItemMax + 15) & ~(size_t)15));
-    B2_CUDA(cudaMalloc(&h->d_tile_len, sizeof(uint32_t) * 3 * kDocTiles));
-    B2_CUDA(cudaMalloc(&h->d_tile_off, sizeof(uint32_t) * (3 * kDocTiles + 1)));
-    B2_CUDA(cudaMalloc(&h->d_info, sizeof(DjInfo)));
-    B2_CUDA(cudaMalloc(&h->d_ring_state, sizeof(DjRing)));
-    B2_CUDA(cudaMalloc(&h->d_ring, sizeof(int32_t) * 3 * (size_t)max_held));
-    B2_CUDA(cudaMalloc(&h->d_stash, (h->stash_max_bytes + 15) & ~(size_t)15));
-    B2_CUDA(cudaMalloc(&h->d_stile_len, sizeof(uint32_t) * 4 * h->stash_tiles));
-    B2_CUDA(cudaMalloc(&h->d_stile_off, sizeof(uint32_t) * (4 * h->stash_tiles + 1)));
-    const int rc = upload_ring_state(h, h->stream);
-    if (rc != B200DD_OK) return rc;
-    B2_CUDA(cudaStreamSynchronize(h->stream));  // the ring state is set before a render on another stream
-    return B200DD_OK;
-  };
-  const int rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  if (int rc = resolve_device(device, &h->device)) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+  B2_CUDA(h->stream.create());
+  B2_CUDA(h->d_body.alloc((3 * (size_t)kListCap * kDocItemMax + 15) & ~(size_t)15));
+  B2_CUDA(h->d_tile_len.alloc(3 * kDocTiles));
+  B2_CUDA(h->d_tile_off.alloc(3 * kDocTiles + 1));
+  B2_CUDA(h->d_info.alloc(1));
+  B2_CUDA(h->d_ring_state.alloc(1));
+  B2_CUDA(h->d_ring.alloc(3 * (size_t)max_held));
+  B2_CUDA(h->d_stash.alloc((h->stash_max_bytes + 15) & ~(size_t)15));
+  B2_CUDA(h->d_stile_len.alloc(4 * h->stash_tiles));
+  B2_CUDA(h->d_stile_off.alloc(4 * h->stash_tiles + 1));
+  if (int rc = upload_ring_state(h.get(), h->stream)) return rc;
+  B2_CUDA(cudaStreamSynchronize(h->stream));  // the ring state is set before a render on another stream
+  *out = h.release();
   return B200DD_OK;
 }
 
@@ -394,23 +384,8 @@ size_t b200dd_detjson_stash_max_bytes(const b200dd_detjson *h) { return h ? h->s
 
 void b200dd_detjson_destroy(b200dd_detjson *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_dev(h->d_body);
-    free_dev(h->d_tile_len);
-    free_dev(h->d_tile_off);
-    free_dev(h->d_info);
-    free_dev(h->d_ring_state);
-    free_dev(h->d_ring);
-    free_dev(h->d_stash);
-    free_dev(h->d_stile_len);
-    free_dev(h->d_stile_off);
-    free_dev(h->d_doc_first);
-    free_dev(h->d_doc_text);
-    free_dev(h->d_texts);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
@@ -418,7 +393,7 @@ int b200dd_detjson_render_device(b200dd_detjson *h, const double *d_delay, const
                                  const double *d_snr, const uint32_t *d_count, void *stream) {
   if (!h || !d_delay || !d_doppler || !d_snr || !d_count) return arg_fail("b200dd_detjson_render_device: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   DocArgs a;
   a.v[0] = d_delay; a.v[1] = d_doppler; a.v[2] = d_snr; a.count = d_count; a.fs = h->fs;
   a.ring = h->d_ring; a.ring_cap = h->ring_cap; a.rs = h->d_ring_state; a.info = h->d_info;
@@ -439,7 +414,7 @@ int b200dd_detjson_fetch(b200dd_detjson *h, uint64_t timestamp, char *out, size_
   if (!h || !out) return arg_fail("b200dd_detjson_fetch: null argument");
   if (!h->pending) return arg_fail("b200dd_detjson_fetch: nothing rendered since the last fetch");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   DjInfo info;
   uint32_t ends[3];  // where the delay, doppler and snr sections end in the body
   B2_CUDA(cudaMemcpyAsync(&info, h->d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
@@ -480,7 +455,7 @@ int b200dd_detjson_fetch_stash(b200dd_detjson *h, char *out, size_t cap, size_t 
   if (h->records.empty())  // detection.js:10, output = []
     return write_document("[]", 0, nullptr, nullptr, nullptr, out, cap, n_bytes, cap_msg, nullptr);
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   const uint32_t held = (uint32_t)(h->tail - h->head);
   std::vector<uint32_t> first, toff{0};
   std::string texts;

@@ -13,8 +13,8 @@
 using namespace b2;
 
 extern "C" int b200dd_bind_host_to_device(int32_t device, char *cpulist_out, int32_t cap) {
-  int dev = device;
-  if (dev < 0) B2_CUDA(cudaGetDevice(&dev));
+  int dev;
+  if (int rc = resolve_device(device, &dev)) return rc;
   char bus[32] = {0};
   B2_CUDA(cudaDeviceGetPCIBusId(bus, sizeof(bus), dev));
   for (char *p = bus; *p; p++) *p = (char)tolower(*p);

@@ -196,23 +196,23 @@ int check_metrics(const char *who, double mn, double mx, double mean, std::strin
 
 struct b200dd_iqjson {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   uint32_t n = 0, tiles = 0, stash_tiles = 0;
   std::string metric[3];     // min, max, mean as the document writes them
   std::string js_metric[3];  // ... and as /stash/iqdata re-prints them
   size_t max_bytes = 0, stash_max_bytes = 0;
   // per-CPI render
-  char *d_body = nullptr;
-  uint32_t *d_tile_len = nullptr, *d_tile_off = nullptr;  // [tiles], [tiles + 1]
-  int32_t *d_code = nullptr;                              // [n] text codes
-  IjInfo *d_info = nullptr;
-  uint32_t *d_row = nullptr;  // the uncommitted ring row
+  DevBuf<char> d_body;
+  DevBuf<uint32_t> d_tile_len, d_tile_off;  // [tiles], [tiles + 1]
+  DevBuf<int32_t> d_code;                   // [n] text codes
+  DevBuf<IjInfo> d_info;
+  DevBuf<uint32_t> d_row;     // the uncommitted ring row
   uint32_t row = 0;           // its host copy, the source of the upload after a commit
   bool pending = false;       // a render not fetched yet
   // stash
-  int32_t *d_ring = nullptr;  // [kRows][n]
-  char *d_stash = nullptr;
-  uint32_t *d_stile_len = nullptr, *d_stile_off = nullptr;  // [stash_tiles], [stash_tiles + 1]
+  DevBuf<int32_t> d_ring;  // [kRows][n]
+  DevBuf<char> d_stash;
+  DevBuf<uint32_t> d_stile_len, d_stile_off;  // [stash_tiles], [stash_tiles + 1]
   std::deque<std::string> ts_text;  // Number::toString of each held document's timestamp, oldest first
   uint32_t head = 0;                // ring row of the oldest held document
   // a share-set member (iqjson_share): its renders write ring row 0, its fetches commit into hist, the set's history
@@ -257,9 +257,9 @@ int b2::iqjson_share(b200dd_iqjson *h, b200dd_iqjson *hist) {
   h->pending = false;
   B2_CUDA(cudaMemcpyAsync(h->d_row, &h->row, sizeof(h->row), cudaMemcpyHostToDevice, h->stream));
   B2_CUDA(cudaStreamSynchronize(h->stream));
-  free_dev(h->d_stash);  // the stash is rendered from hist
-  free_dev(h->d_stile_len);
-  free_dev(h->d_stile_off);
+  h->d_stash.reset();  // the stash is rendered from hist
+  h->d_stile_len.reset();
+  h->d_stile_off.reset();
   h->hist = hist;
   return B200DD_OK;
 }
@@ -274,9 +274,8 @@ int b200dd_iqjson_create(uint32_t n_spectrum, double min, double max, double mea
   std::string metric[3];
   const int rc0 = check_metrics("b200dd_iqjson_create", min, max, mean, metric);
   if (rc0 != B200DD_OK) return rc0;
-  b200dd_iqjson *h = new (std::nothrow) b200dd_iqjson();
+  Owned<b200dd_iqjson> h(new (std::nothrow) b200dd_iqjson(), b200dd_iqjson_destroy);
   if (!h) return arg_fail("b200dd_iqjson_create: out of host memory");
-  auto fail = [&](int rc) { b200dd_iqjson_destroy(h); return rc; };
   h->n = n_spectrum;
   h->tiles = (n_spectrum + kDocTile - 1) / kDocTile;
   h->stash_tiles = (kDepth * n_spectrum + kTile - 1) / kTile;
@@ -291,30 +290,23 @@ int b200dd_iqjson_create(uint32_t n_spectrum, double min, double max, double mea
                       kDepth * 21 + h->js_metric[0].size() + h->js_metric[1].size() + h->js_metric[2].size() +
                       kDepth * 3;
   h->stash_max_bytes = head + (size_t)kDepth * n_spectrum * kStashItemMax + 2;
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    B2_CUDA(cudaMalloc(&h->d_body, ((size_t)n_spectrum * kDocItemMax + 15) & ~(size_t)15));
-    B2_CUDA(cudaMalloc(&h->d_tile_len, sizeof(uint32_t) * h->tiles));
-    B2_CUDA(cudaMalloc(&h->d_tile_off, sizeof(uint32_t) * (h->tiles + 1)));
-    B2_CUDA(cudaMalloc(&h->d_code, sizeof(int32_t) * n_spectrum));
-    B2_CUDA(cudaMalloc(&h->d_info, sizeof(IjInfo)));
-    B2_CUDA(cudaMalloc(&h->d_row, sizeof(uint32_t)));
-    B2_CUDA(cudaMalloc(&h->d_ring, sizeof(int32_t) * kRows * (size_t)n_spectrum));
-    B2_CUDA(cudaMalloc(&h->d_stash, ((size_t)kDepth * n_spectrum * kStashItemMax + 15) & ~(size_t)15));
-    B2_CUDA(cudaMalloc(&h->d_stile_len, sizeof(uint32_t) * h->stash_tiles));
-    B2_CUDA(cudaMalloc(&h->d_stile_off, sizeof(uint32_t) * (h->stash_tiles + 1)));
-    B2_CUDA(cudaMemsetAsync(h->d_row, 0, sizeof(uint32_t), h->stream));
-    B2_CUDA(cudaStreamSynchronize(h->stream));  // the row is set before a render on another stream
-    return B200DD_OK;
-  };
-  const int rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  if (int rc = resolve_device(device, &h->device)) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+  B2_CUDA(h->stream.create());
+  B2_CUDA(h->d_body.alloc(((size_t)n_spectrum * kDocItemMax + 15) & ~(size_t)15));
+  B2_CUDA(h->d_tile_len.alloc(h->tiles));
+  B2_CUDA(h->d_tile_off.alloc(h->tiles + 1));
+  B2_CUDA(h->d_code.alloc(n_spectrum));
+  B2_CUDA(h->d_info.alloc(1));
+  B2_CUDA(h->d_row.alloc(1));
+  B2_CUDA(h->d_ring.alloc(kRows * (size_t)n_spectrum));
+  B2_CUDA(h->d_stash.alloc(((size_t)kDepth * n_spectrum * kStashItemMax + 15) & ~(size_t)15));
+  B2_CUDA(h->d_stile_len.alloc(h->stash_tiles));
+  B2_CUDA(h->d_stile_off.alloc(h->stash_tiles + 1));
+  B2_CUDA(cudaMemsetAsync(h->d_row, 0, sizeof(uint32_t), h->stream));
+  B2_CUDA(cudaStreamSynchronize(h->stream));  // the row is set before a render on another stream
+  *out = h.release();
   return B200DD_OK;
 }
 
@@ -323,28 +315,15 @@ size_t b200dd_iqjson_stash_max_bytes(const b200dd_iqjson *h) { return h ? h->sta
 
 void b200dd_iqjson_destroy(b200dd_iqjson *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_dev(h->d_body);
-    free_dev(h->d_tile_len);
-    free_dev(h->d_tile_off);
-    free_dev(h->d_code);
-    free_dev(h->d_info);
-    free_dev(h->d_row);
-    free_dev(h->d_ring);
-    free_dev(h->d_stash);
-    free_dev(h->d_stile_len);
-    free_dev(h->d_stile_off);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
 int b200dd_iqjson_render_device(b200dd_iqjson *h, const void *d_spectrum, void *stream) {
   if (!h || !d_spectrum) return arg_fail("b200dd_iqjson_render_device: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   DocArgs a;
   a.spec = (const double2 *)d_spectrum; a.n = h->n; a.ring = h->d_ring; a.row = h->d_row; a.code = h->d_code; a.info = h->d_info;
   a.tile_len = h->d_tile_len; a.tile_off = h->d_tile_off; a.body = h->d_body;
@@ -364,7 +343,7 @@ int b200dd_iqjson_fetch(b200dd_iqjson *h, uint64_t timestamp, char *out, size_t 
   if (!h || !out) return arg_fail("b200dd_iqjson_fetch: null argument");
   if (!h->pending) return arg_fail("b200dd_iqjson_fetch: nothing rendered since the last fetch");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   IjInfo info;
   B2_CUDA(cudaMemcpyAsync(&info, h->d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
@@ -388,7 +367,7 @@ int b200dd_iqjson_fetch_stash(b200dd_iqjson *h, char *out, size_t cap, size_t *n
   if (h->ts_text.empty())  // iqdata.js:8, output = []
     return write_document("[]", 0, nullptr, nullptr, nullptr, out, cap, n_bytes, cap_msg, nullptr);
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   const uint32_t held = (uint32_t)h->ts_text.size();
   std::string hdr = "{\"timestamp\":[";
   for (uint32_t i = 0; i < held; i++) hdr += (i ? "," : "") + h->ts_text[i];
@@ -440,7 +419,7 @@ int b200dd_iqjson_render_host(const double *spectrum, uint32_t n, double min, do
 int b200dd_iqjson_debug_bin_values(b200dd_iqjson *h, const void *d_spectrum, void *d_out, void *stream) {
   if (!h || !d_spectrum || !d_out) return arg_fail("b200dd_iqjson_debug_bin_values: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   ij_values_kernel<<<(h->n + 255) / 256, 256, 0, st>>>((const double2 *)d_spectrum, h->n, (double *)d_out);
   B2_LAUNCH_CHECK();
   return B200DD_OK;

@@ -55,31 +55,24 @@ int join_texts(const std::string &who, const char *text, int stride, const int *
 }
 
 template <int STRIDE, class FMT> int format_on_device(const double *v, uint32_t n, char *text, int *len, int32_t device) {
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__);
+  int dev;
+  if (int rc = resolve_device(device, &dev)) return rc;
   DeviceGuard guard(dev);
   if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
   if (n == 0) return B200DD_OK;
-  double *d_v = nullptr;
-  char *d_text = nullptr;
-  int *d_len = nullptr;
-  auto body = [&]() -> int {
-    B2_CUDA(cudaMalloc(&d_v, sizeof(double) * n));
-    B2_CUDA(cudaMalloc(&d_text, (size_t)n * STRIDE));
-    B2_CUDA(cudaMalloc(&d_len, sizeof(int) * n));
-    B2_CUDA(cudaMemcpy(d_v, v, sizeof(double) * n, cudaMemcpyHostToDevice));
-    const uint32_t blocks = (n + 255) / 256 < 132 * 16 ? (n + 255) / 256 : 132 * 16;
-    format_kernel<STRIDE, FMT><<<blocks, 256>>>(d_v, n, d_text, d_len);
-    B2_LAUNCH_CHECK();
-    B2_CUDA(cudaMemcpy(text, d_text, (size_t)n * STRIDE, cudaMemcpyDeviceToHost));
-    B2_CUDA(cudaMemcpy(len, d_len, sizeof(int) * n, cudaMemcpyDeviceToHost));
-    return B200DD_OK;
-  };
-  const int rc = body();
-  free_dev(d_v);
-  free_dev(d_text);
-  free_dev(d_len);
-  return rc;
+  DevBuf<double> d_v;
+  DevBuf<char> d_text;
+  DevBuf<int> d_len;
+  B2_CUDA(d_v.alloc(n));
+  B2_CUDA(d_text.alloc((size_t)n * STRIDE));
+  B2_CUDA(d_len.alloc(n));
+  B2_CUDA(cudaMemcpy(d_v, v, sizeof(double) * n, cudaMemcpyHostToDevice));
+  const uint32_t blocks = (n + 255) / 256 < 132 * 16 ? (n + 255) / 256 : 132 * 16;
+  format_kernel<STRIDE, FMT><<<blocks, 256>>>(d_v, n, d_text, d_len);
+  B2_LAUNCH_CHECK();
+  B2_CUDA(cudaMemcpy(text, d_text, (size_t)n * STRIDE, cudaMemcpyDeviceToHost));
+  B2_CUDA(cudaMemcpy(len, d_len, sizeof(int) * n, cudaMemcpyDeviceToHost));
+  return B200DD_OK;
 }
 
 // The format_doubles entries of `who`: FMT's text (at most STRIDE bytes) of each of n doubles, comma-separated, made

@@ -88,16 +88,16 @@ template <class TMAP> __global__ void mj_cell_values_kernel(const TMAP *map, siz
 
 struct b200dd_mapjson {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   uint32_t nDop = 0, nDel = 0, nTiles = 0;
   size_t cells = 0;
   std::string delay_txt, doppler_txt;  // the two axis arrays as the client receives them
   bool axes_ok = true;                 // false: a Doppler value has no text, every document fails
   size_t body_max = 0, max_bytes = 0;
-  char *d_body = nullptr;
-  uint32_t *d_tile_len = nullptr, *d_tile_off = nullptr;
-  uint32_t *d_info = nullptr;  // [0] body bytes, [1] non-finite flag
-  double2 *d_maph = nullptr;   // render_host staging
+  DevBuf<char> d_body;
+  DevBuf<uint32_t> d_tile_len, d_tile_off;
+  DevBuf<uint32_t> d_info;   // [0] body bytes, [1] non-finite flag
+  DevBuf<double2> d_maph;    // render_host staging
   // what the last render left for fetch
   bool rendered = false;
   double noise = 0.0, maxp = 0.0;
@@ -147,9 +147,8 @@ int b200dd_mapjson_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, 
   *out = nullptr;
   if (n_dop == 0 || n_del == 0) return arg_fail("b200dd_mapjson_create: empty map");
   if (fs == 0) return arg_fail("b200dd_mapjson_create: fs must be positive");
-  b200dd_mapjson *h = new (std::nothrow) b200dd_mapjson();
+  Owned<b200dd_mapjson> h(new (std::nothrow) b200dd_mapjson(), b200dd_mapjson_destroy);
   if (!h) return arg_fail("b200dd_mapjson_create: out of host memory");
-  auto fail = [&](int rc) { b200dd_mapjson_destroy(h); return rc; };
   h->nDop = n_dop;
   h->nDel = n_del;
   h->cells = (size_t)n_dop * n_del;
@@ -162,25 +161,18 @@ int b200dd_mapjson_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, 
   // body: every cell's text is at most kMaxText bytes, plus n_del - 1 commas and two brackets per row, plus a
   // comma between rows
   h->body_max = h->cells * jf::kMaxText + (size_t)n_dop * (n_del + 1) + (n_dop - 1);
-  if (h->body_max > 0xFFFFFFF0ull) return fail(geom_fail("b200dd_mapjson_create: map too large for 32-bit text offsets"));
+  if (h->body_max > 0xFFFFFFF0ull) return geom_fail("b200dd_mapjson_create: map too large for 32-bit text offsets");
   const std::string widest(jf::kMaxText, '0');
-  h->max_bytes = compose_header(h, "18446744073709551615", widest, widest).size() + h->body_max + 2;
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    B2_CUDA(cudaMalloc(&h->d_body, (h->body_max + 15) & ~(size_t)15));
-    B2_CUDA(cudaMalloc(&h->d_tile_len, sizeof(uint32_t) * h->nTiles));
-    B2_CUDA(cudaMalloc(&h->d_tile_off, sizeof(uint32_t) * (h->nTiles + 1)));
-    B2_CUDA(cudaMalloc(&h->d_info, sizeof(uint32_t) * 2));
-    return B200DD_OK;
-  };
-  const int rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  h->max_bytes = compose_header(h.get(), "18446744073709551615", widest, widest).size() + h->body_max + 2;
+  if (int rc = resolve_device(device, &h->device)) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+  B2_CUDA(h->stream.create());
+  B2_CUDA(h->d_body.alloc((h->body_max + 15) & ~(size_t)15));
+  B2_CUDA(h->d_tile_len.alloc(h->nTiles));
+  B2_CUDA(h->d_tile_off.alloc(h->nTiles + 1));
+  B2_CUDA(h->d_info.alloc(2));
+  *out = h.release();
   return B200DD_OK;
 }
 
@@ -188,16 +180,8 @@ size_t b200dd_mapjson_max_bytes(const b200dd_mapjson *h) { return h ? h->max_byt
 
 void b200dd_mapjson_destroy(b200dd_mapjson *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_dev(h->d_body);
-    free_dev(h->d_tile_len);
-    free_dev(h->d_tile_off);
-    free_dev(h->d_info);
-    free_dev(h->d_maph);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
@@ -205,7 +189,7 @@ int b200dd_mapjson_render_device(b200dd_mapjson *h, const void *d_map, int is_f6
                                  double max_power, void *stream) {
   if (!h || !d_map) return arg_fail("b200dd_mapjson_render_device: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   h->rendered = true;
   h->noise = noise_power;
   h->maxp = max_power;
@@ -219,7 +203,7 @@ int b200dd_mapjson_fetch(b200dd_mapjson *h, uint64_t timestamp, char *out, size_
   if (!h || !out) return arg_fail("b200dd_mapjson_fetch: null argument");
   if (!h->rendered) return arg_fail("b200dd_mapjson_fetch: nothing rendered");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   uint32_t info[2] = {0, 0};
   double m[2] = {h->noise, h->maxp};
   B2_CUDA(cudaMemcpyAsync(info, h->d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
@@ -241,7 +225,7 @@ int b200dd_mapjson_render_host(b200dd_mapjson *h, const double *map, double nois
   if (n_bytes) *n_bytes = 0;
   if (!h || !map || !out) return arg_fail("b200dd_mapjson_render_host: null argument");
   DeviceGuard guard(h->device);
-  if (!h->d_maph) B2_CUDA(cudaMalloc(&h->d_maph, sizeof(double2) * h->cells));
+  if (!h->d_maph) B2_CUDA(h->d_maph.alloc(h->cells));
   B2_CUDA(cudaMemcpyAsync(h->d_maph, map, sizeof(double2) * h->cells, cudaMemcpyHostToDevice, h->stream));
   const int rc = b200dd_mapjson_render_device(h, h->d_maph, 1, noise_power, max_power, h->stream);
   if (rc != B200DD_OK) return rc;
@@ -252,7 +236,7 @@ int b200dd_mapjson_debug_cell_values(b200dd_mapjson *h, const void *d_map, int i
                                      void *stream) {
   if (!h || !d_map || !d_out) return arg_fail("b200dd_mapjson_debug_cell_values: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   const int blocks = 132 * 8;
   if (is_f64)
     mj_cell_values_kernel<double2><<<blocks, 256, 0, st>>>((const double2 *)d_map, h->cells, noise_power, (double *)d_out);

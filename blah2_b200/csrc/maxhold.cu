@@ -126,18 +126,18 @@ __global__ void __launch_bounds__(kTextThreads) mh_write_kernel(RenderArgs a) {
 
 struct b200dd_maxhold {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   uint32_t nDop = 0, nDel = 0, nTiles = 0;
   size_t cells = 0;
   std::string delay_txt, doppler_txt;  // the two axis arrays as JSON.stringify prints them
   bool axes_ok = true;                 // false: an axis value has no text, every document fails
   size_t body_max = 0, max_bytes = 0;
-  int32_t *d_ring = nullptr;  // [kSlots][cells] hundredths
-  int32_t *d_held = nullptr;  // [cells]
-  MhState *d_state = nullptr;
-  char *d_body = nullptr;
-  uint32_t *d_tile_len = nullptr, *d_tile_off = nullptr;
-  uint32_t *d_total = nullptr;
+  DevBuf<int32_t> d_ring;  // [kSlots][cells] hundredths
+  DevBuf<int32_t> d_held;  // [cells]
+  DevBuf<MhState> d_state;
+  DevBuf<char> d_body;
+  DevBuf<uint32_t> d_tile_len, d_tile_off;
+  DevBuf<uint32_t> d_total;
 };
 
 namespace {
@@ -182,9 +182,8 @@ int b200dd_maxhold_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, 
   *out = nullptr;
   if (n_dop == 0 || n_del == 0) return arg_fail("b200dd_maxhold_create: empty map");
   if (fs == 0) return arg_fail("b200dd_maxhold_create: fs must be positive");
-  b200dd_maxhold *h = new (std::nothrow) b200dd_maxhold();
+  Owned<b200dd_maxhold> h(new (std::nothrow) b200dd_maxhold(), b200dd_maxhold_destroy);
   if (!h) return arg_fail("b200dd_maxhold_create: out of host memory");
-  auto fail = [&](int rc) { b200dd_maxhold_destroy(h); return rc; };
   h->nDop = n_dop;
   h->nDel = n_del;
   h->cells = (size_t)n_dop * n_del;
@@ -195,31 +194,24 @@ int b200dd_maxhold_create(uint32_t n_dop, uint32_t n_del, const int32_t *delay, 
   h->axes_ok = numbers_text(km.data(), n_del, false, true, h->delay_txt) &&
                numbers_text(doppler, n_dop, true, true, h->doppler_txt);
   h->body_max = h->cells * jf::kMaxHundredthsText + (size_t)n_dop * (n_del + 1) + (n_dop - 1);
-  if (h->body_max > 0xFFFFFFF0ull) return fail(geom_fail("b200dd_maxhold_create: map too large for 32-bit text offsets"));
+  if (h->body_max > 0xFFFFFFF0ull) return geom_fail("b200dd_maxhold_create: map too large for 32-bit text offsets");
   // the longest texts: a timestamp, and a metric (Number::toString of a double is at most 25 bytes)
   const std::string widest(25, '0');
-  h->max_bytes = compose_header(h, "18446744073709552000", widest, widest).size() + h->body_max + 2;
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    B2_CUDA(cudaMalloc(&h->d_ring, sizeof(int32_t) * kSlots * h->cells));
-    B2_CUDA(cudaMalloc(&h->d_held, sizeof(int32_t) * h->cells));
-    B2_CUDA(cudaMalloc(&h->d_state, sizeof(MhState)));
-    B2_CUDA(cudaMemsetAsync(h->d_state, 0, sizeof(MhState), h->stream));
-    B2_CUDA(cudaMalloc(&h->d_body, (h->body_max + 15) & ~(size_t)15));
-    B2_CUDA(cudaMalloc(&h->d_tile_len, sizeof(uint32_t) * h->nTiles));
-    B2_CUDA(cudaMalloc(&h->d_tile_off, sizeof(uint32_t) * (h->nTiles + 1)));
-    B2_CUDA(cudaMalloc(&h->d_total, sizeof(uint32_t)));
-    B2_CUDA(cudaStreamSynchronize(h->stream));  // the state is cleared before a push on another stream
-    return B200DD_OK;
-  };
-  const int rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  h->max_bytes = compose_header(h.get(), "18446744073709552000", widest, widest).size() + h->body_max + 2;
+  if (int rc = resolve_device(device, &h->device)) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+  B2_CUDA(h->stream.create());
+  B2_CUDA(h->d_ring.alloc(kSlots * h->cells));
+  B2_CUDA(h->d_held.alloc(h->cells));
+  B2_CUDA(h->d_state.alloc(1));
+  B2_CUDA(cudaMemsetAsync(h->d_state, 0, sizeof(MhState), h->stream));
+  B2_CUDA(h->d_body.alloc((h->body_max + 15) & ~(size_t)15));
+  B2_CUDA(h->d_tile_len.alloc(h->nTiles));
+  B2_CUDA(h->d_tile_off.alloc(h->nTiles + 1));
+  B2_CUDA(h->d_total.alloc(1));
+  B2_CUDA(cudaStreamSynchronize(h->stream));  // the state is cleared before a push on another stream
+  *out = h.release();
   return B200DD_OK;
 }
 
@@ -227,18 +219,8 @@ size_t b200dd_maxhold_max_bytes(const b200dd_maxhold *h) { return h ? h->max_byt
 
 void b200dd_maxhold_destroy(b200dd_maxhold *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_dev(h->d_ring);
-    free_dev(h->d_held);
-    free_dev(h->d_state);
-    free_dev(h->d_body);
-    free_dev(h->d_tile_len);
-    free_dev(h->d_tile_off);
-    free_dev(h->d_total);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
@@ -248,7 +230,7 @@ int b200dd_maxhold_push_device(b200dd_maxhold *h, const void *d_map, int is_f64,
   if (jf::is_finite(noise_power) && fabs(noise_power) > kNoiseBound)
     return arg_fail("b200dd_maxhold_push_device: |noise_power| > 1e7 dB");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   return enqueue_push(h, d_map, is_f64 != 0, noise_power, max_power, nullptr, nullptr, st);
 }
 
@@ -256,7 +238,7 @@ int b200dd_maxhold_fetch(b200dd_maxhold *h, uint64_t timestamp, char *out, size_
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_maxhold_fetch: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   MhState s;
   B2_CUDA(cudaMemcpyAsync(&s, h->d_state, sizeof(s), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));

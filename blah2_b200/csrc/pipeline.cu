@@ -125,7 +125,7 @@ struct ShareSet {
   b200dd_tracker *tr = nullptr;
   TimingHistory *tm = nullptr;  // host state: its commits need no event
   int64_t mh_last = -1, dj_last = -1, ij_last = -1, tr_last = -1, tm_last = -1;  // the CPI each one took last
-  cudaEvent_t ev = nullptr;
+  Event ev;
   bool ev_recorded = false;
 };
 
@@ -152,7 +152,7 @@ struct LastCpi {
 struct b200dd_pipeline {
   b200dd_pipeline_params p;
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   b200dd_caf *caf = nullptr;
   b200dd_wh *wh = nullptr;
   b200dd_det *det = nullptr;
@@ -167,20 +167,20 @@ struct b200dd_pipeline {
   bool tm_on = false;               // the submits enqueue stamps
   TimingHistory *tm = nullptr;
   uint64_t tm_t_start = 0;
-  uint64_t *d_tm = nullptr;         // the last submit's stamps, TmSlot
+  DevBuf<uint64_t> d_tm;            // the last submit's stamps, TmSlot
   std::vector<const char *> tm_names;  // behind the last document written
   std::vector<double> tm_values;
   uint32_t spec_bins = 0, spec_nfft = 0;
   b200dd_caf_geometry g;
   std::vector<int32_t> delay;
   std::vector<double> doppler;
-  float2 *d_yf = nullptr;                    // filtered surveillance channel (device path)
-  double2 *d_xd = nullptr, *d_yd = nullptr;  // host path staging
-  float2 *d_xf = nullptr, *d_yf2 = nullptr;
-  double2 *d_mapd = nullptr;
-  float2 *d_map = nullptr;
-  short4 *d_iq16 = nullptr;  // int16 ingest staging
-  int8_t *d_x8 = nullptr, *d_y8 = nullptr;  // int8 ingest staging, 2 N bytes per channel
+  DevBuf<float2> d_yf;         // filtered surveillance channel (device path)
+  DevBuf<double2> d_xd, d_yd;  // host path staging
+  DevBuf<float2> d_xf, d_yf2;
+  DevBuf<double2> d_mapd;
+  DevBuf<float2> d_map;
+  DevBuf<short4> d_iq16;       // int16 ingest staging
+  DevBuf<int8_t> d_x8, d_y8;   // int8 ingest staging, 2 N bytes per channel
   LastCpi last;
   // CUDA-graph replay of the device chain (b200dd_pipeline_submit_device): one instantiated graph per
   // (d_x, d_y, d_map) triple given to b200dd_pipeline_prepare_device
@@ -248,40 +248,33 @@ extern "C" {
 int b200dd_pipeline_create(const b200dd_pipeline_params *params, b200dd_pipeline **out) {
   if (!params || !out) return arg_fail("b200dd_pipeline_create: null argument");
   *out = nullptr;
-  b200dd_pipeline *h = new (std::nothrow) b200dd_pipeline();
+  Owned<b200dd_pipeline> h(new (std::nothrow) b200dd_pipeline(), b200dd_pipeline_destroy);
   if (!h) return arg_fail("b200dd_pipeline_create: out of host memory");
   h->p = *params;
-  auto fail = [&](int rc) { b200dd_pipeline_destroy(h); return rc; };
-  int dev = params->caf.device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
+  if (int rc = resolve_device(params->caf.device, &h->device)) return rc;
+  const int dev = h->device;
   DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
   b200dd_caf_params cp = params->caf;
   cp.device = dev;
   int rc = b200dd_caf_create(&cp, &h->caf);
-  if (rc != B200DD_OK) return fail(rc);
+  if (rc != B200DD_OK) return rc;
   b200dd_caf_get_geometry(h->caf, &h->g);
   h->delay.resize(h->g.n_delay_bins);
   h->doppler.resize(h->g.n_doppler_bins);
   b200dd_caf_get_axes(h->caf, h->delay.data(), h->doppler.data());
   if (params->clutter_enable) {
     rc = b200dd_wh_create(params->clutter_delay_min, params->clutter_delay_max, params->caf.n_samples, dev, &h->wh);
-    if (rc != B200DD_OK) return fail(rc);
+    if (rc != B200DD_OK) return rc;
   }
   b200dd_det_params dp = params->det;
   dp.device = dev;
   rc = b200dd_det_create(&dp, h->g.n_doppler_bins, h->g.n_delay_bins, &h->det);  // also serves set_metrics
-  if (rc != B200DD_OK) return fail(rc);
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    B2_CUDA(cudaMalloc(&h->d_map, sizeof(float2) * (size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
-    if (h->wh) B2_CUDA(cudaMalloc(&h->d_yf, sizeof(float2) * params->caf.n_samples));
-    return B200DD_OK;
-  };
-  rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  if (rc != B200DD_OK) return rc;
+  B2_CUDA(h->stream.create());
+  B2_CUDA(h->d_map.alloc((size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
+  if (h->wh) B2_CUDA(h->d_yf.alloc(params->caf.n_samples));
+  *out = h.release();
   return B200DD_OK;
 }
 
@@ -289,34 +282,20 @@ static void set_leave(b200dd_pipeline *h);
 
 void b200dd_pipeline_destroy(b200dd_pipeline *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    set_leave(h);
-    b200dd_caf_destroy(h->caf);
-    b200dd_wh_destroy(h->wh);
-    pipeline_drop_graphs(h);
-    b200dd_det_destroy(h->det);
-    b200dd_spectrum_destroy(h->spec);
-    b200dd_iqjson_destroy(h->ij);
-    b200dd_mapjson_destroy(h->mj);
-    b200dd_maxhold_destroy(h->mh);
-    b200dd_detjson_destroy(h->dj);
-    b200dd_tracker_destroy(h->tr);
-    timing_history_destroy(h->tm);
-    free_dev(h->d_tm);
-    free_dev(h->d_yf);
-    free_dev(h->d_xd);
-    free_dev(h->d_yd);
-    free_dev(h->d_xf);
-    free_dev(h->d_yf2);
-    free_dev(h->d_mapd);
-    free_dev(h->d_map);
-    free_dev(h->d_iq16);
-    free_dev(h->d_x8);
-    free_dev(h->d_y8);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
+  set_leave(h);
+  b200dd_caf_destroy(h->caf);
+  b200dd_wh_destroy(h->wh);
+  pipeline_drop_graphs(h);
+  b200dd_det_destroy(h->det);
+  b200dd_spectrum_destroy(h->spec);
+  b200dd_iqjson_destroy(h->ij);
+  b200dd_mapjson_destroy(h->mj);
+  b200dd_maxhold_destroy(h->mh);
+  b200dd_detjson_destroy(h->dj);
+  b200dd_tracker_destroy(h->tr);
+  timing_history_destroy(h->tm);
   delete h;
 }
 
@@ -597,14 +576,14 @@ static int host_counts(const b200dd_pipeline *h, uint32_t n, uint32_t *need, uin
 // (complex64 samples are copied straight into x and y)
 static int host_staging(b200dd_pipeline *h, HostFormat fmt, bool map_out) {
   const size_t N = h->p.caf.n_samples;
-  if (!h->d_xf) B2_CUDA(cudaMalloc(&h->d_xf, sizeof(float2) * N));
-  if (!h->d_yf2) B2_CUDA(cudaMalloc(&h->d_yf2, sizeof(float2) * N));
-  if (map_out && !h->d_mapd) B2_CUDA(cudaMalloc(&h->d_mapd, sizeof(double2) * (size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
-  if (fmt == kC128 && !h->d_xd) B2_CUDA(cudaMalloc(&h->d_xd, sizeof(double2) * N));
-  if (fmt == kC128 && !h->d_yd) B2_CUDA(cudaMalloc(&h->d_yd, sizeof(double2) * N));
-  if (fmt == kInt16 && !h->d_iq16) B2_CUDA(cudaMalloc(&h->d_iq16, sizeof(short4) * N));
-  if (fmt == kCi8 && !h->d_x8) B2_CUDA(cudaMalloc(&h->d_x8, 2 * N));
-  if (fmt == kCi8 && !h->d_y8) B2_CUDA(cudaMalloc(&h->d_y8, 2 * N));
+  if (!h->d_xf) B2_CUDA(h->d_xf.alloc(N));
+  if (!h->d_yf2) B2_CUDA(h->d_yf2.alloc(N));
+  if (map_out && !h->d_mapd) B2_CUDA(h->d_mapd.alloc((size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
+  if (fmt == kC128 && !h->d_xd) B2_CUDA(h->d_xd.alloc(N));
+  if (fmt == kC128 && !h->d_yd) B2_CUDA(h->d_yd.alloc(N));
+  if (fmt == kInt16 && !h->d_iq16) B2_CUDA(h->d_iq16.alloc(N));
+  if (fmt == kCi8 && !h->d_x8) B2_CUDA(h->d_x8.alloc(2 * N));
+  if (fmt == kCi8 && !h->d_y8) B2_CUDA(h->d_y8.alloc(2 * N));
   return B200DD_OK;
 }
 
@@ -1014,7 +993,7 @@ int b200dd_pipeline_enable_timing_json(b200dd_pipeline *h, uint64_t t_start, siz
   int rc = stage_reset(h, h->tm, timing_history_destroy, kTimingBit);
   if (rc != B200DD_OK) return rc;
   if (!h->d_tm) {
-    B2_CUDA(cudaMalloc(&h->d_tm, sizeof(uint64_t) * kTmSlots));
+    B2_CUDA(h->d_tm.alloc(kTmSlots));
     B2_CUDA(cudaMemset(h->d_tm, 0, sizeof(uint64_t) * kTmSlots));
   }
   h->tm_t_start = t_start;
@@ -1175,8 +1154,7 @@ static void set_free(ShareSet *s) {
   b200dd_iqjson_destroy(s->ij);
   b200dd_tracker_destroy(s->tr);
   timing_history_destroy(s->tm);
-  if (s->ev) cudaEventDestroy(s->ev);
-  delete s;
+  delete s;  // under the guard: the event goes with it
 }
 
 // a member being destroyed leaves its set; the last one frees it (its stream is synchronised: nothing is in flight)
@@ -1203,25 +1181,19 @@ int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
   }
   b200dd_pipeline *h0 = members[0];
   DeviceGuard guard(h0->device);
-  ShareSet *s = new (std::nothrow) ShareSet();
-  if (!s) return arg_fail("b200dd_pipeline_share_history: out of host memory");
-  s->device = h0->device;
-  auto body = [&]() -> int {
-    for (uint32_t i = 0; i < n; i++) B2_CUDA(cudaStreamSynchronize(members[i]->stream));
-    B2_CUDA(cudaEventCreateWithFlags(&s->ev, cudaEventDisableTiming));
-    int rc = h0->mh ? maxhold_create(h0, &s->mh) : B200DD_OK;
-    if (rc == B200DD_OK && h0->dj) rc = detjson_create(h0, &s->dj);
-    if (rc == B200DD_OK && h0->ij) rc = iqjson_create(h0, &s->ij);
-    if (rc == B200DD_OK && h0->tr) rc = tracker_create(h0, &s->tr);
-    if (rc == B200DD_OK && h0->tm_on && !(s->tm = timing_history_create(h0->tm_t_start)))
-      rc = arg_fail("b200dd_pipeline_share_history: out of host memory");
-    return rc;
-  };
-  const int rc = body();
-  if (rc != B200DD_OK) {
-    set_free(s);
-    return rc;
-  }
+  Owned<ShareSet> set(new (std::nothrow) ShareSet(), set_free);
+  if (!set) return arg_fail("b200dd_pipeline_share_history: out of host memory");
+  set->device = h0->device;
+  for (uint32_t i = 0; i < n; i++) B2_CUDA(cudaStreamSynchronize(members[i]->stream));
+  B2_CUDA(set->ev.create(cudaEventDisableTiming));
+  int rc = h0->mh ? maxhold_create(h0, &set->mh) : B200DD_OK;
+  if (rc == B200DD_OK && h0->dj) rc = detjson_create(h0, &set->dj);
+  if (rc == B200DD_OK && h0->ij) rc = iqjson_create(h0, &set->ij);
+  if (rc == B200DD_OK && h0->tr) rc = tracker_create(h0, &set->tr);
+  if (rc == B200DD_OK && h0->tm_on && !(set->tm = timing_history_create(h0->tm_t_start)))
+    rc = arg_fail("b200dd_pipeline_share_history: out of host memory");
+  if (rc != B200DD_OK) return rc;
+  ShareSet *s = set.release();
   // from here on the members change: each one's renders stage for the set's histories, its own window and tracker go
   int first = B200DD_OK;  // only a CUDA error can fail here; every member joins all the same
   for (uint32_t i = 0; i < n; i++) {

@@ -244,14 +244,14 @@ double2 unit_phase(uint64_t num, uint64_t den) {  // exp(-2 pi i num / den), num
 
 struct b200dd_spectrum {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   uint32_t n = 0, decimation = 0, nSpectrum = 0, nfft = 0;
   double bandwidth = 0.0;
   uint32_t rowsPerChunk = 0, nChunks = 0;    // 8-byte-load fold (any nSpectrum / alignment, double2 input)
   uint32_t rowsPerChunk2 = 0, nChunks2 = 0;  // two-columns-per-thread fold
-  double2 *d_t1 = nullptr, *d_t2 = nullptr, *d_w = nullptr, *d_part = nullptr, *d_g = nullptr, *d_out = nullptr;
-  double2 *d_xd = nullptr;  // host-path staging
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+  DevBuf<double2> d_t1, d_t2, d_w, d_part, d_g, d_out;
+  DevBuf<double2> d_xd;  // host-path staging
+  Event ev[3];
   std::vector<double> frequency;
 };
 
@@ -356,25 +356,18 @@ int b200dd_spectrum_plan(uint32_t n, double bandwidth, b200dd_spectrum_geometry 
 int b200dd_spectrum_create(uint32_t n, double bandwidth, int32_t device, b200dd_spectrum **out) {
   if (!out) return arg_fail("b200dd_spectrum_create: null argument");
   *out = nullptr;
-  b200dd_spectrum *h = new (std::nothrow) b200dd_spectrum();
+  Owned<b200dd_spectrum> h(new (std::nothrow) b200dd_spectrum(), b200dd_spectrum_destroy);
   if (!h) return arg_fail("b200dd_spectrum_create: out of host memory");
-  {
-    const int rc0 = spectrum_host_plan(n, bandwidth, h);
-    if (rc0 != B200DD_OK) { delete h; return rc0; }
-  }
+  if (int rc = spectrum_host_plan(n, bandwidth, h.get())) return rc;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     cudaGetLastError();
-    delete h;
     set_last_error("b200dd_spectrum_create: no CUDA device (there is no CPU fallback)");
     return B200DD_ERR_CUDA;
   }
-  auto fail = [&](int rc) { b200dd_spectrum_destroy(h); return rc; };
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
+  if (int rc = resolve_device(device, &h->device)) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
   const uint32_t decimation = h->decimation, nSpectrum = h->nSpectrum, nfft = h->nfft;
   // phase tables (long double on the host, exact integer residues)
   const uint64_t k0 = (uint64_t)(nfft / 2) + 1;  // :46 int(nfft / 2) + 1
@@ -384,46 +377,29 @@ int b200dd_spectrum_create(uint32_t n, double bandwidth, int32_t device, b200dd_
     t2[r] = unit_phase((k0 * r) % nfft, nfft);
     w[r] = unit_phase(r, nSpectrum);
   }
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    for (auto &e : h->ev) B2_CUDA(cudaEventCreate(&e));
-    B2_CUDA(cudaMalloc(&h->d_t1, sizeof(double2) * decimation));
-    B2_CUDA(cudaMalloc(&h->d_t2, sizeof(double2) * nSpectrum));
-    B2_CUDA(cudaMalloc(&h->d_w, sizeof(double2) * nSpectrum));
-    B2_CUDA(cudaMalloc(&h->d_part, sizeof(double2) * (size_t)(h->nChunks > h->nChunks2 ? h->nChunks : h->nChunks2) * nSpectrum));
-    B2_CUDA(cudaMalloc(&h->d_g, sizeof(double2) * nSpectrum));
-    B2_CUDA(cudaMalloc(&h->d_out, sizeof(double2) * nSpectrum));
-    B2_CUDA(cudaMemcpy(h->d_t1, t1.data(), sizeof(double2) * decimation, cudaMemcpyHostToDevice));
-    B2_CUDA(cudaMemcpy(h->d_t2, t2.data(), sizeof(double2) * nSpectrum, cudaMemcpyHostToDevice));
-    B2_CUDA(cudaMemcpy(h->d_w, w.data(), sizeof(double2) * nSpectrum, cudaMemcpyHostToDevice));
-    // per function, not per handle: always the largest g any handle stages (12288 bins, 196608 B + 4 KB static),
-    // so that creating a smaller handle never lowers the limit a live larger one launches with
-    B2_CUDA(cudaFuncSetAttribute(spec_dft_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)(sizeof(double2) * (size_t)DFT_SMEM_BINS)));
-    return B200DD_OK;
-  };
-  const int rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  B2_CUDA(h->stream.create());
+  for (auto &e : h->ev) B2_CUDA(e.create());
+  B2_CUDA(h->d_t1.alloc(decimation));
+  B2_CUDA(h->d_t2.alloc(nSpectrum));
+  B2_CUDA(h->d_w.alloc(nSpectrum));
+  B2_CUDA(h->d_part.alloc((size_t)(h->nChunks > h->nChunks2 ? h->nChunks : h->nChunks2) * nSpectrum));
+  B2_CUDA(h->d_g.alloc(nSpectrum));
+  B2_CUDA(h->d_out.alloc(nSpectrum));
+  B2_CUDA(cudaMemcpy(h->d_t1, t1.data(), sizeof(double2) * decimation, cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(h->d_t2, t2.data(), sizeof(double2) * nSpectrum, cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(h->d_w, w.data(), sizeof(double2) * nSpectrum, cudaMemcpyHostToDevice));
+  // per function, not per handle: always the largest g any handle stages (12288 bins, 196608 B + 4 KB static),
+  // so that creating a smaller handle never lowers the limit a live larger one launches with
+  B2_CUDA(cudaFuncSetAttribute(spec_dft_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)(sizeof(double2) * (size_t)DFT_SMEM_BINS)));
+  *out = h.release();
   return B200DD_OK;
 }
 
 void b200dd_spectrum_destroy(b200dd_spectrum *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_dev(h->d_t1);
-    free_dev(h->d_t2);
-    free_dev(h->d_w);
-    free_dev(h->d_part);
-    free_dev(h->d_g);
-    free_dev(h->d_out);
-    free_dev(h->d_xd);
-    for (auto &e : h->ev)
-      if (e) cudaEventDestroy(e);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
@@ -451,7 +427,7 @@ int b200dd_spectrum_process_device(b200dd_spectrum *h, const void *d_x, uint32_t
   if (!h || !d_x) return arg_fail("b200dd_spectrum_process_device: null argument");
   if (n < h->nfft) return arg_fail("b200dd_spectrum_process_device: fewer than nfft samples");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   return run_spectrum<float2>(h, (const float2 *)d_x, d_spectrum ? (double2 *)d_spectrum : h->d_out, st, false);
 }
 
@@ -459,7 +435,7 @@ int b200dd_spectrum_process_device_f64(b200dd_spectrum *h, const void *d_x, uint
   if (!h || !d_x) return arg_fail("b200dd_spectrum_process_device_f64: null argument");
   if (n < h->nfft) return arg_fail("b200dd_spectrum_process_device_f64: fewer than nfft samples");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   return run_spectrum<double2>(h, (const double2 *)d_x, d_spectrum ? (double2 *)d_spectrum : h->d_out, st, false);
 }
 
@@ -468,7 +444,7 @@ int b200dd_spectrum_profile_device(b200dd_spectrum *h, const void *d_x, uint32_t
   if (!h || !d_x || !ms_fold || !ms_rest) return arg_fail("b200dd_spectrum_profile_device: null argument");
   if (n < h->nfft) return arg_fail("b200dd_spectrum_profile_device: fewer than nfft samples");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   const int rc = run_spectrum<float2>(h, (const float2 *)d_x, h->d_out, st, true);
   if (rc != B200DD_OK) return rc;
   B2_CUDA(cudaStreamSynchronize(st));
@@ -480,7 +456,7 @@ int b200dd_spectrum_profile_device(b200dd_spectrum *h, const void *d_x, uint32_t
 int b200dd_spectrum_fetch(b200dd_spectrum *h, double *spectrum_out, void *stream) {
   if (!h || !spectrum_out) return arg_fail("b200dd_spectrum_fetch: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   B2_CUDA(cudaMemcpyAsync(spectrum_out, h->d_out, sizeof(double2) * h->nSpectrum, cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   return B200DD_OK;
@@ -490,7 +466,7 @@ int b200dd_spectrum_process_host(b200dd_spectrum *h, const double *x, uint32_t n
   if (!h || !x || !spectrum_out) return arg_fail("b200dd_spectrum_process_host: null argument");
   if (n < h->nfft) return arg_fail("b200dd_spectrum_process_host: fewer than nfft samples");
   DeviceGuard guard(h->device);
-  if (!h->d_xd) B2_CUDA(cudaMalloc(&h->d_xd, sizeof(double2) * (size_t)(h->nfft ? h->nfft : 1)));
+  if (!h->d_xd) B2_CUDA(h->d_xd.alloc((size_t)(h->nfft ? h->nfft : 1)));
   B2_CUDA(cudaMemcpyAsync(h->d_xd, x, sizeof(double2) * (size_t)h->nfft, cudaMemcpyHostToDevice, h->stream));
   const int rc = run_spectrum<double2>(h, h->d_xd, h->d_out, h->stream, false);
   if (rc != B200DD_OK) return rc;

@@ -411,50 +411,23 @@ size_t slot_bytes(uint32_t H) { return 16 * (size_t)H + 4 * (size_t)((H + 15) / 
 
 struct b200dd_tracker {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   b200dd_tracker_params p{};
   uint32_t slots = 0, H = 0, W = 0, tiles = 0, nh = 0;
   size_t max_bytes = 0;
-  TrArgs a{};
+  TrArgs a{};      // the kernels' view of the arrays below
   RenderArgs r{};
+  DevBuf<TrState> d_s;
+  DevBuf<uint32_t> d_order, d_order_tmp, d_free_list, d_counter, d_id, d_len, d_st;
+  DevBuf<double> d_cur_delay, d_cur_doppler, d_acc, d_hd, d_hf, d_acc_init;
+  DevBuf<TrInfo> d_info;
+  DevBuf<uint32_t> d_item_len, d_tile_len, d_tile_off;
+  DevBuf<char> d_body;
   size_t body_alloc = 0;
-  double *d_in = nullptr;  // process_host staging: delay, doppler
-  uint32_t *d_in_count = nullptr;
+  DevBuf<double> d_in;  // process_host staging: delay, doppler
+  DevBuf<uint32_t> d_in_count;
   size_t in_alloc = 0;
 };
-
-namespace {
-
-void free_all(b200dd_tracker *h) {
-  TrArgs &a = h->a;
-  free_dev(a.s);
-  free_dev(a.order);
-  free_dev(a.order_tmp);
-  free_dev(a.free_list);
-  free_dev(a.counter);
-  free_dev(a.cur_delay);
-  free_dev(a.cur_doppler);
-  free_dev(a.acc);
-  free_dev(a.id);
-  free_dev(a.len);
-  free_dev(a.hd);
-  free_dev(a.hf);
-  free_dev(a.st);
-  double *ai = const_cast<double *>(a.acc_init);
-  free_dev(ai);
-  a.acc_init = nullptr;
-  free_dev(h->r.info);
-  free_dev(h->r.item_len);
-  free_dev(h->r.tile_len);
-  uint32_t *to = const_cast<uint32_t *>(h->r.tile_off);
-  free_dev(to);
-  h->r.tile_off = nullptr;
-  free_dev(h->r.body);
-  free_dev(h->d_in);
-  free_dev(h->d_in_count);
-}
-
-}  // namespace
 
 extern "C" {
 
@@ -476,9 +449,8 @@ int b200dd_tracker_create(const b200dd_tracker_params *params, uint32_t max_trac
   *out = nullptr;
   int rc = check_params(params, max_tracks, max_history, "b200dd_tracker_create");
   if (rc != B200DD_OK) return rc;
-  b200dd_tracker *h = new (std::nothrow) b200dd_tracker();
+  Owned<b200dd_tracker> h(new (std::nothrow) b200dd_tracker(), b200dd_tracker_destroy);
   if (!h) return arg_fail("b200dd_tracker_create: out of host memory");
-  auto fail = [&](int e) { b200dd_tracker_destroy(h); return e; };
   std::vector<double> acc;
   acc_hypotheses(params->cpi, params->max_acc_init, &acc);
   h->p = *params;
@@ -488,42 +460,36 @@ int b200dd_tracker_create(const b200dd_tracker_params *params, uint32_t max_trac
   h->tiles = (max_tracks + kThreads - 1) / kThreads;
   h->nh = (uint32_t)acc.size();
   h->max_bytes = kHeadBound + (size_t)max_tracks * item_bound(max_history);
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
+  if ((rc = resolve_device(device, &h->device))) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
   TrArgs &a = h->a;
+  RenderArgs &r = h->r;
   const size_t S = max_tracks;
-  auto body = [&]() -> int {
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    B2_CUDA(cudaMalloc(&a.s, sizeof(TrState)));
-    B2_CUDA(cudaMalloc(&a.order, sizeof(uint32_t) * S));
-    B2_CUDA(cudaMalloc(&a.order_tmp, sizeof(uint32_t) * S));
-    B2_CUDA(cudaMalloc(&a.free_list, sizeof(uint32_t) * S));
-    B2_CUDA(cudaMalloc(&a.counter, sizeof(uint32_t) * S));
-    B2_CUDA(cudaMalloc(&a.cur_delay, sizeof(double) * S));
-    B2_CUDA(cudaMalloc(&a.cur_doppler, sizeof(double) * S));
-    B2_CUDA(cudaMalloc(&a.acc, sizeof(double) * S));
-    B2_CUDA(cudaMalloc(&a.id, sizeof(uint32_t) * S));
-    B2_CUDA(cudaMalloc(&a.len, sizeof(uint32_t) * S));
-    B2_CUDA(cudaMalloc(&a.hd, sizeof(double) * S * h->H));
-    B2_CUDA(cudaMalloc(&a.hf, sizeof(double) * S * h->H));
-    B2_CUDA(cudaMalloc(&a.st, sizeof(uint32_t) * S * h->W));
-    double *ai = nullptr;
-    B2_CUDA(cudaMalloc(&ai, sizeof(double) * acc.size()));
-    a.acc_init = ai;
-    B2_CUDA(cudaMemcpy(ai, acc.data(), sizeof(double) * acc.size(), cudaMemcpyHostToDevice));
-    B2_CUDA(cudaMalloc(&h->r.info, sizeof(TrInfo)));
-    B2_CUDA(cudaMalloc(&h->r.item_len, sizeof(uint32_t) * S));
-    B2_CUDA(cudaMalloc(&h->r.tile_len, sizeof(uint32_t) * h->tiles));
-    uint32_t *to = nullptr;
-    B2_CUDA(cudaMalloc(&to, sizeof(uint32_t) * (h->tiles + 1)));
-    h->r.tile_off = to;
-    return B200DD_OK;
-  };
-  rc = body();
-  if (rc != B200DD_OK) return fail(rc);
+  B2_CUDA(h->stream.create());
+  B2_CUDA(h->d_s.alloc(1));
+  B2_CUDA(h->d_order.alloc(S));
+  B2_CUDA(h->d_order_tmp.alloc(S));
+  B2_CUDA(h->d_free_list.alloc(S));
+  B2_CUDA(h->d_counter.alloc(S));
+  B2_CUDA(h->d_cur_delay.alloc(S));
+  B2_CUDA(h->d_cur_doppler.alloc(S));
+  B2_CUDA(h->d_acc.alloc(S));
+  B2_CUDA(h->d_id.alloc(S));
+  B2_CUDA(h->d_len.alloc(S));
+  B2_CUDA(h->d_hd.alloc(S * h->H));
+  B2_CUDA(h->d_hf.alloc(S * h->H));
+  B2_CUDA(h->d_st.alloc(S * h->W));
+  B2_CUDA(h->d_acc_init.alloc(acc.size()));
+  B2_CUDA(cudaMemcpy(h->d_acc_init, acc.data(), sizeof(double) * acc.size(), cudaMemcpyHostToDevice));
+  B2_CUDA(h->d_info.alloc(1));
+  B2_CUDA(h->d_item_len.alloc(S));
+  B2_CUDA(h->d_tile_len.alloc(h->tiles));
+  B2_CUDA(h->d_tile_off.alloc(h->tiles + 1));
+  a.s = h->d_s; a.order = h->d_order; a.order_tmp = h->d_order_tmp; a.free_list = h->d_free_list;
+  a.counter = h->d_counter; a.cur_delay = h->d_cur_delay; a.cur_doppler = h->d_cur_doppler; a.acc = h->d_acc;
+  a.id = h->d_id; a.len = h->d_len; a.hd = h->d_hd; a.hf = h->d_hf; a.st = h->d_st; a.acc_init = h->d_acc_init;
+  r.info = h->d_info; r.item_len = h->d_item_len; r.tile_len = h->d_tile_len; r.tile_off = h->d_tile_off;
   const double c = (double)299792458u;  // Constants::c, blah2.cpp:193-194
   a.nh = h->nh;
   a.slots = max_tracks;
@@ -536,20 +502,15 @@ int b200dd_tracker_create(const b200dd_tracker_params *params, uint32_t max_trac
   a.dop_hi = 0.0 + 1 * (1 / params->cpi);
   a.range_res = c / params->fs;
   a.lambda = c / params->fc;
-  rc = b200dd_tracker_reset(h);
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  if ((rc = b200dd_tracker_reset(h.get()))) return rc;
+  *out = h.release();
   return B200DD_OK;
 }
 
 void b200dd_tracker_destroy(b200dd_tracker *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_all(h);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
@@ -570,7 +531,7 @@ int b200dd_tracker_process_device(b200dd_tracker *h, const double *d_delay, cons
   (void)d_snr;  // the Detection's SNR enters no track value and no document
   if (!h || !d_delay || !d_doppler || !d_count) return arg_fail("b200dd_tracker_process_device: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   tr_update_kernel<<<1, kUpdThreads, 0, st>>>(h->a, d_delay, d_doppler, d_count, timestamp);
   B2_LAUNCH_CHECK();
   tr_append_kernel<<<kAppendBlocks, kThreads, 0, st>>>(h->a, d_delay, d_doppler);
@@ -583,13 +544,12 @@ int b200dd_tracker_process_host(b200dd_tracker *h, const double *delay, const do
   (void)snr;
   if (!h || (n && (!delay || !doppler))) return arg_fail("b200dd_tracker_process_host: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  if (!h->d_in_count) B2_CUDA(cudaMalloc(&h->d_in_count, sizeof(uint32_t)));
+  cudaStream_t st = stream_or(stream, h->stream);
+  if (!h->d_in_count) B2_CUDA(h->d_in_count.alloc(1));
   if ((size_t)n > h->in_alloc) {
     B2_CUDA(cudaStreamSynchronize(st));
-    free_dev(h->d_in);
     h->in_alloc = 0;
-    B2_CUDA(cudaMalloc(&h->d_in, sizeof(double) * 2 * (size_t)n));
+    B2_CUDA(h->d_in.alloc(2 * (size_t)n));
     h->in_alloc = n;
   }
   // pageable sources: each copy has taken the host data when it returns
@@ -598,7 +558,7 @@ int b200dd_tracker_process_host(b200dd_tracker *h, const double *delay, const do
     B2_CUDA(cudaMemcpyAsync(h->d_in + h->in_alloc, doppler, sizeof(double) * n, cudaMemcpyHostToDevice, st));
   }
   B2_CUDA(cudaMemcpyAsync(h->d_in_count, &n, sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-  const double *dd = h->d_in ? h->d_in : (const double *)h->d_in_count;  // n = 0: never read
+  const double *dd = h->d_in ? h->d_in.get() : (const double *)h->d_in_count.get();  // n = 0: never read
   const double *df = h->d_in ? h->d_in + h->in_alloc : dd;
   return b200dd_tracker_process_device(h, dd, df, nullptr, h->d_in_count, timestamp, st);
 }
@@ -608,11 +568,11 @@ int b200dd_tracker_fetch(b200dd_tracker *h, uint64_t timestamp, char *out, size_
   if (n_bytes) *n_bytes = 0;
   if (!h || !out) return arg_fail("b200dd_tracker_fetch: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   B2_CUDA(cudaMemsetAsync(h->r.info, 0, sizeof(TrInfo), st));
   tr_len_kernel<<<h->tiles, kThreads, 0, st>>>(h->a, h->r);
   B2_LAUNCH_CHECK();
-  scan_kernel<<<1, 1024, 0, st>>>(h->r.tile_len, const_cast<uint32_t *>(h->r.tile_off), (int)h->tiles, &h->r.info->body);
+  scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)h->tiles, &h->d_info->body);
   B2_LAUNCH_CHECK();
   TrState s;
   TrInfo info;
@@ -641,10 +601,10 @@ int b200dd_tracker_fetch(b200dd_tracker *h, uint64_t timestamp, char *out, size_
     return B200DD_ERR_CAPACITY;
   }
   if (info.body > h->body_alloc) {
-    free_dev(h->r.body);
     h->body_alloc = 0;
     const size_t want = std::min(h->max_bytes, (size_t)info.body * 2);
-    B2_CUDA(cudaMalloc(&h->r.body, want));
+    B2_CUDA(h->d_body.alloc(want));
+    h->r.body = h->d_body;
     h->body_alloc = want;
   }
   memcpy(out, hdr.data(), hdr.size());

@@ -26,38 +26,31 @@ __global__ void __launch_bounds__(256) fp64_fma_kernel(int iters, double *sink) 
 
 extern "C" int b200dd_ubench_fp64_tflops(int32_t device, double *tflops) {
   if (!tflops) return arg_fail("b200dd_ubench_fp64_tflops: null argument");
-  int dev = device;
-  if (dev < 0) B2_CUDA(cudaGetDevice(&dev));
+  int dev;
+  if (int rc = resolve_device(device, &dev)) return rc;
   DeviceGuard guard(dev);
   if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
   int sms = 0;
   B2_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int grid = sms * 8, iters = 4096;
-  double *sink = nullptr;
-  B2_CUDA(cudaMalloc(&sink, sizeof(double) * (size_t)grid * 256));
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  auto body = [&]() -> int {
-    B2_CUDA(cudaEventCreate(&e0));
-    B2_CUDA(cudaEventCreate(&e1));
-    fp64_fma_kernel<<<grid, 256>>>(64, sink);
+  DevBuf<double> sink;
+  B2_CUDA(sink.alloc((size_t)grid * 256));
+  Event e0, e1;
+  B2_CUDA(e0.create());
+  B2_CUDA(e1.create());
+  fp64_fma_kernel<<<grid, 256>>>(64, sink);
+  B2_LAUNCH_CHECK();
+  float best = 1e30f;
+  for (int t = 0; t < 5; t++) {
+    B2_CUDA(cudaEventRecord(e0));
+    fp64_fma_kernel<<<grid, 256>>>(iters, sink);
     B2_LAUNCH_CHECK();
-    float best = 1e30f;
-    for (int t = 0; t < 5; t++) {
-      B2_CUDA(cudaEventRecord(e0));
-      fp64_fma_kernel<<<grid, 256>>>(iters, sink);
-      B2_LAUNCH_CHECK();
-      B2_CUDA(cudaEventRecord(e1));
-      B2_CUDA(cudaEventSynchronize(e1));
-      float ms = 0.f;
-      B2_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-      if (ms < best) best = ms;
-    }
-    *tflops = 2.0 * 8.0 * iters * (double)grid * 256.0 / (best * 1e-3) / 1e12;
-    return B200DD_OK;
-  };
-  const int rc = body();
-  if (e0) cudaEventDestroy(e0);
-  if (e1) cudaEventDestroy(e1);
-  cudaFree(sink);
-  return rc;
+    B2_CUDA(cudaEventRecord(e1));
+    B2_CUDA(cudaEventSynchronize(e1));
+    float ms = 0.f;
+    B2_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    if (ms < best) best = ms;
+  }
+  *tflops = 2.0 * 8.0 * iters * (double)grid * 256.0 / (best * 1e-3) / 1e12;
+  return B200DD_OK;
 }

@@ -1303,7 +1303,7 @@ struct b200dd_wh {
   uint32_t N = 0;
   int nBins = 0;
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   int log2m_c = 12, log2m_a = 12;  // FFT lengths of the correlation / filter stages
   int L = 0, nSeg = 0, segPerCta = 1, gridCorr = 1;  // correlation stage
   int Lout = 0, gridApply = 1, ctasApply = 1;       // filter stage: blocks, persistent CTAs
@@ -1314,16 +1314,16 @@ struct b200dd_wh {
   size_t solveSmem = 0;
   int partResident = 1;  // resident CTAs per SM of the partitioned filter kernel
   Span span;
-  double2 *d_tw_c = nullptr, *d_tw_a = nullptr, *d_partial = nullptr, *d_a = nullptr, *d_b = nullptr, *d_w = nullptr, *d_what = nullptr;
-  int *d_status = nullptr;
-  int *d_next_block = nullptr;  // work queue of the persistent filter CTAs
-  double2 *d_xd = nullptr, *d_yd = nullptr;  // host path staging (complex128)
+  DevBuf<double2> d_tw_c, d_tw_a, d_partial, d_a, d_b, d_w, d_what;
+  DevBuf<int> d_status;
+  DevBuf<int> d_next_block;  // work queue of the persistent filter CTAs
+  DevBuf<double2> d_xd, d_yd;  // host path staging (complex128)
   int num_sms = 132;
   // chunk mode (one CPI split over several GPUs): this handle filters the samples [c0, c0 + nc) of an N-sample signal
   bool chunked = false;
   uint32_t c0 = 0, nc = 0;
   int haloXL = 0, haloXR = 0, haloYR = 0;
-  double2 *d_ab = nullptr;  // [2][nBins] this chunk's correlation sums (reduced over its CTAs)
+  DevBuf<double2> d_ab;  // [2][nBins] this chunk's correlation sums (reduced over its CTAs)
 };
 
 namespace {
@@ -1414,7 +1414,7 @@ int wh_launch_solve(b200dd_wh *h, cudaStream_t st) {
 }
 
 template <class TIN> int wh_dispatch(b200dd_wh *h, const void *x, const void *y, void *y_out, cudaStream_t st,
-                                     cudaEvent_t *ev = nullptr) {
+                                     const Event *ev = nullptr) {
   if (ev) B2_CUDA(cudaEventRecord(ev[0], st));
   int rc = with_log2m(h->log2m_c, [&](auto l) { return wh_launch_corr<decltype(l)::value, TIN>(h, x, y, st); });
   if (rc != B200DD_OK) return rc;
@@ -1577,7 +1577,7 @@ static int wh_create_impl(int32_t delay_min, int32_t delay_max, uint32_t n_sampl
   if (nb < 1) return geom_fail("b200dd_wh_create: delayMax - delayMin must be >= 1");
   if (nb > kMaxBins) return geom_fail("b200dd_wh_create: more than 4096 filter taps unsupported");
   if ((uint64_t)nb > n_samples) return geom_fail("b200dd_wh_create: more taps than samples");
-  b200dd_wh *h = new (std::nothrow) b200dd_wh();
+  Owned<b200dd_wh> h(new (std::nothrow) b200dd_wh(), b200dd_wh_destroy);
   if (!h) return arg_fail("b200dd_wh_create: out of host memory");
   h->delayMin = delay_min;
   h->delayMax = delay_max;
@@ -1592,86 +1592,62 @@ static int wh_create_impl(int32_t delay_min, int32_t delay_max, uint32_t n_sampl
     h->haloXR = (int)nb - 1 + sh;                               // the correlations reach forward nBins - 1 samples of xs
     h->haloYR = (int)nb - 1;
     if ((uint32_t)(nb + sh) > chunk_len && n_samples != chunk_len)
-      { delete h; return geom_fail("b200dd_wh_create_chunk: a chunk must be longer than the filter (the halo comes from ONE neighbour)"); }
+      return geom_fail("b200dd_wh_create_chunk: a chunk must be longer than the filter (the halo comes from ONE neighbour)");
   }
-  auto fail = [&](int rc) { b200dd_wh_destroy(h); return rc; };
-  int dev = device;
-  if (dev < 0 && cudaGetDevice(&dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDevice", __FILE__, __LINE__));
-  h->device = dev;
-  DeviceGuard guard(dev);
-  if (!guard.ok) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
+  if (int rc = resolve_device(device, &h->device)) return rc;
+  DeviceGuard guard(h->device);
+  if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaGetDeviceProperties", __FILE__, __LINE__));
+  if (cudaGetDeviceProperties(&prop, h->device) != cudaSuccess) return cuda_fail(cudaGetLastError(), "cudaGetDeviceProperties", __FILE__, __LINE__);
   h->num_sms = prop.multiProcessorCount;
   if (h->nBins > 3585) {  // resident CTAs of the partitioned filter: what its compiled register count allows
     int r = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, wh_apply_part_kernel<kPartLog2M, float2>,
                                                       dit::Plan3<kPartLog2M>::NT, fft_smem<kPartLog2M>()) != cudaSuccess)
-      return fail(cuda_fail(cudaGetLastError(), "cudaOccupancyMaxActiveBlocksPerMultiprocessor", __FILE__, __LINE__));
+      return cuda_fail(cudaGetLastError(), "cudaOccupancyMaxActiveBlocksPerMultiprocessor", __FILE__, __LINE__);
     h->partResident = r < 1 ? 1 : r;
   }
-  wh_plan(h);
-  if (!h->log2m_c || !h->log2m_a) return fail(geom_fail("b200dd_wh_create: no FFT plan (needs nSamples >= 512, and nSamples >= 4096 above 3585 taps)"));
-  auto body = [&]() -> int {
-    const int rc = wh_set_smem_limits(h);
-    if (rc != B200DD_OK) return rc;
-    B2_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    const int Mc = 1 << h->log2m_c, M = 1 << h->log2m_a;
-    auto twc = twiddle_table_f64(Mc), twa = twiddle_table_f64(M);
-    B2_CUDA(cudaMalloc(&h->d_tw_c, sizeof(double2) * Mc));
-    B2_CUDA(cudaMemcpy(h->d_tw_c, twc.data(), sizeof(double2) * Mc, cudaMemcpyHostToDevice));
-    B2_CUDA(cudaMalloc(&h->d_tw_a, sizeof(double2) * M));
-    B2_CUDA(cudaMemcpy(h->d_tw_a, twa.data(), sizeof(double2) * M, cudaMemcpyHostToDevice));
-    B2_CUDA(cudaMalloc(&h->d_partial, sizeof(double2) * (size_t)h->gridCorr * 2 * h->nBins));
-    B2_CUDA(cudaMalloc(&h->d_a, sizeof(double2) * h->nBins));
-    B2_CUDA(cudaMalloc(&h->d_b, sizeof(double2) * h->nBins));
-    B2_CUDA(cudaMalloc(&h->d_w, sizeof(double2) * h->nBins));
-    B2_CUDA(cudaMalloc(&h->d_what, sizeof(double2) * M * h->parts));
-    B2_CUDA(cudaMalloc(&h->d_status, sizeof(int)));
-    B2_CUDA(cudaMemset(h->d_status, 0, sizeof(int)));
-    B2_CUDA(cudaMalloc(&h->d_next_block, sizeof(int)));
-    if (h->chunked) B2_CUDA(cudaMalloc(&h->d_ab, sizeof(double2) * 2 * h->nBins));
-    return B200DD_OK;
-  };
-  int rc = body();
-  if (rc != B200DD_OK) return fail(rc);
-  *out = h;
+  wh_plan(h.get());
+  if (!h->log2m_c || !h->log2m_a) return geom_fail("b200dd_wh_create: no FFT plan (needs nSamples >= 512, and nSamples >= 4096 above 3585 taps)");
+  if (int rc = wh_set_smem_limits(h.get())) return rc;
+  B2_CUDA(h->stream.create());
+  const int Mc = 1 << h->log2m_c, M = 1 << h->log2m_a;
+  auto twc = twiddle_table_f64(Mc), twa = twiddle_table_f64(M);
+  B2_CUDA(h->d_tw_c.alloc(Mc));
+  B2_CUDA(cudaMemcpy(h->d_tw_c, twc.data(), sizeof(double2) * Mc, cudaMemcpyHostToDevice));
+  B2_CUDA(h->d_tw_a.alloc(M));
+  B2_CUDA(cudaMemcpy(h->d_tw_a, twa.data(), sizeof(double2) * M, cudaMemcpyHostToDevice));
+  B2_CUDA(h->d_partial.alloc((size_t)h->gridCorr * 2 * h->nBins));
+  B2_CUDA(h->d_a.alloc(h->nBins));
+  B2_CUDA(h->d_b.alloc(h->nBins));
+  B2_CUDA(h->d_w.alloc(h->nBins));
+  B2_CUDA(h->d_what.alloc(M * h->parts));
+  B2_CUDA(h->d_status.alloc(1));
+  B2_CUDA(cudaMemset(h->d_status, 0, sizeof(int)));
+  B2_CUDA(h->d_next_block.alloc(1));
+  if (h->chunked) B2_CUDA(h->d_ab.alloc(2 * h->nBins));
+  *out = h.release();
   return B200DD_OK;
 }
 
 void b200dd_wh_destroy(b200dd_wh *h) {
   if (!h) return;
-  {
-    DeviceGuard guard(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    free_dev(h->d_tw_c);
-    free_dev(h->d_tw_a);
-    free_dev(h->d_partial);
-    free_dev(h->d_a);
-    free_dev(h->d_b);
-    free_dev(h->d_w);
-    free_dev(h->d_what);
-    free_dev(h->d_status);
-    free_dev(h->d_next_block);
-    free_dev(h->d_ab);
-    free_dev(h->d_xd);
-    free_dev(h->d_yd);
-    if (h->stream) cudaStreamDestroy(h->stream);
-  }
+  DeviceGuard guard(h->device);  // held while the members free
+  if (h->stream) cudaStreamSynchronize(h->stream);
   delete h;
 }
 
 int b200dd_wh_process_device(b200dd_wh *h, const void *d_x, const void *d_y, void *d_y_out, void *stream) {
   if (!h || !d_x || !d_y || !d_y_out) return arg_fail("b200dd_wh_process_device: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   return wh_dispatch<float2>(h, d_x, d_y, d_y_out, st);
 }
 
 int b200dd_wh_process_device_f64(b200dd_wh *h, const void *d_x, const void *d_y, void *d_y_out, void *stream) {
   if (!h || !d_x || !d_y || !d_y_out) return arg_fail("b200dd_wh_process_device_f64: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   return wh_dispatch<double2>(h, d_x, d_y, d_y_out, st);
 }
 
@@ -1687,7 +1663,7 @@ int b200dd_wh_chunk_corr_device(b200dd_wh *h, const void *d_x_loc, const void *d
   if (!h || !d_x_loc || !d_y_loc || !d_ab) return arg_fail("b200dd_wh_chunk_corr_device: null argument");
   if (!h->chunked) return arg_fail("b200dd_wh_chunk_corr_device: not a chunk handle");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   // virtual pointers indexed by the GLOBAL sample number
   const float2 *xv = (const float2 *)d_x_loc - ((long long)h->c0 - h->haloXL);
   const float2 *yv = (const float2 *)d_y_loc - (long long)h->c0;
@@ -1704,7 +1680,7 @@ int b200dd_wh_chunk_filter_device(b200dd_wh *h, const void *d_ab, const void *d_
   if (!h || !d_ab || !d_x_loc || !d_y_loc || !d_y_out) return arg_fail("b200dd_wh_chunk_filter_device: null argument");
   if (!h->chunked) return arg_fail("b200dd_wh_chunk_filter_device: not a chunk handle");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  cudaStream_t st = stream_or(stream, h->stream);
   if (d_ab != (const void *)h->d_ab)
     B2_CUDA(cudaMemcpyAsync(h->d_ab, d_ab, sizeof(double2) * 2 * h->nBins, cudaMemcpyDeviceToDevice, st));
   int rc = wh_launch_solve(h, st);  // replicated on every GPU: identical sums in, identical weights out
@@ -1719,21 +1695,18 @@ int b200dd_wh_profile_device(b200dd_wh *h, const void *d_x, const void *d_y, voi
                              float *ms_corr, float *ms_solve, float *ms_apply) {
   if (!h || !d_x || !d_y || !d_y_out || !ms_corr || !ms_solve || !ms_apply) return arg_fail("b200dd_wh_profile_device: null argument");
   DeviceGuard guard(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  cudaEvent_t ev[4];
-  for (int i = 0; i < 4; i++) B2_CUDA(cudaEventCreate(&ev[i]));
-  int rc = wh_dispatch<float2>(h, d_x, d_y, d_y_out, st, ev);
-  if (rc == B200DD_OK) {
-    B2_CUDA(cudaEventSynchronize(ev[3]));
-    B2_CUDA(cudaEventElapsedTime(ms_corr, ev[0], ev[1]));
-    B2_CUDA(cudaEventElapsedTime(ms_solve, ev[1], ev[2]));
-    B2_CUDA(cudaEventElapsedTime(ms_apply, ev[2], ev[3]));  // weight spectrum + overlap-save filter
-  }
-  for (int i = 0; i < 4; i++) cudaEventDestroy(ev[i]);
-  return rc;
+  cudaStream_t st = stream_or(stream, h->stream);
+  Event ev[4];
+  for (auto &e : ev) B2_CUDA(e.create());
+  if (int rc = wh_dispatch<float2>(h, d_x, d_y, d_y_out, st, ev)) return rc;
+  B2_CUDA(cudaEventSynchronize(ev[3]));
+  B2_CUDA(cudaEventElapsedTime(ms_corr, ev[0], ev[1]));
+  B2_CUDA(cudaEventElapsedTime(ms_solve, ev[1], ev[2]));
+  B2_CUDA(cudaEventElapsedTime(ms_apply, ev[2], ev[3]));  // weight spectrum + overlap-save filter
+  return B200DD_OK;
 }
 
-const int *b200dd_wh_device_status(b200dd_wh *h) { return h ? h->d_status : nullptr; }
+const int *b200dd_wh_device_status(b200dd_wh *h) { return h ? h->d_status.get() : nullptr; }
 
 int b200dd_wh_last_status(b200dd_wh *h) {
   if (!h) return arg_fail("b200dd_wh_last_status: null handle");
@@ -1749,8 +1722,8 @@ int b200dd_wh_process_host(b200dd_wh *h, const double *x, double *y) {
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
   if (!h->d_xd) {
-    B2_CUDA(cudaMalloc(&h->d_xd, sizeof(double2) * h->N));
-    B2_CUDA(cudaMalloc(&h->d_yd, sizeof(double2) * h->N));
+    B2_CUDA(h->d_xd.alloc(h->N));
+    B2_CUDA(h->d_yd.alloc(h->N));
   }
   B2_CUDA(cudaMemcpyAsync(h->d_xd, x, sizeof(double2) * h->N, cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemcpyAsync(h->d_yd, y, sizeof(double2) * h->N, cudaMemcpyHostToDevice, st));

@@ -77,9 +77,32 @@ def _channel_count(name, x, y, dtypes, per_instant):
     return counts[0]
 
 
-class Ambiguity:
+class _Handle:
+    """Owner of one C-ABI handle: ``_lib`` and ``_h`` are set by the subclass's constructor, ``_destroy`` names the
+    library function that frees ``_h``."""
+    _destroy = None
+
+    def close(self):
+        if getattr(self, "_h", None):
+            getattr(self._lib, self._destroy)(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _st(stream):
+        """The stream argument of a call: the caller's stream, or NULL for the handle's own."""
+        return capi.ptr(stream or None)
+
+
+class Ambiguity(_Handle):
     """Ambiguity(delayMin, delayMax, dopplerMin, dopplerMax, fs, n, roundHamming=False)
     -- src/process/ambiguity/Ambiguity.h:34."""
+    _destroy = "b200dd_caf_destroy"
 
     def __init__(self, delayMin, delayMax, dopplerMin, dopplerMax, fs, n, roundHamming=False, device=-1):
         lib = capi.load()
@@ -140,34 +163,34 @@ class Ambiguity:
         Asynchronous.  Returns None; result in d_map (or the handle's internal map)."""
         n = d_x.numel() if hasattr(d_x, "numel") else self.geometry.n_used
         capi.check(self._lib.b200dd_caf_process_device(self._h, capi.ptr(d_x), capi.ptr(d_y), int(n),
-                                                       capi.ptr(d_map), capi.ptr(stream) if stream else None))
+                                                       capi.ptr(d_map), self._st(stream)))
 
     def range_device(self, d_x, d_y, batch0, n_batches, d_R, stream=None):
         """Range stage on batches [batch0, batch0+n_batches): d_x, d_y hold exactly those batches."""
         capi.check(self._lib.b200dd_caf_range_device(self._h, capi.ptr(d_x), capi.ptr(d_y), int(batch0), int(n_batches),
-                                                     capi.ptr(d_R), capi.ptr(stream) if stream else None))
+                                                     capi.ptr(d_R), self._st(stream)))
 
     def doppler_device(self, d_R, col0, n_cols, d_map_tile, stream=None):
         """Doppler stage on delay columns [col0, col0+n_cols) of the complete range matrix d_R."""
         capi.check(self._lib.b200dd_caf_doppler_device(self._h, capi.ptr(d_R), int(col0), int(n_cols),
-                                                       capi.ptr(d_map_tile), capi.ptr(stream) if stream else None))
+                                                       capi.ptr(d_map_tile), self._st(stream)))
 
     def place_tile(self, d_tile, col0, n_cols, d_map, stream=None):
         """Tile [nDop][n_cols] -> delay columns [col0, col0 + n_cols) of the row-major map d_map."""
         capi.check(self._lib.b200dd_caf_place_tile_device(self._h, capi.ptr(d_tile), int(col0), int(n_cols), capi.ptr(d_map),
-                                                          capi.ptr(stream) if stream else None))
+                                                          self._st(stream)))
 
     def place_tiles(self, d_tiles, n_tiles, d_map, stream=None):
         """All gathered tiles of an equal column split (shard.block_range) -> the row-major map, one kernel."""
         capi.check(self._lib.b200dd_caf_place_tiles_device(self._h, capi.ptr(d_tiles), int(n_tiles), capi.ptr(d_map),
-                                                           capi.ptr(stream) if stream else None))
+                                                           self._st(stream)))
 
     def profile_device(self, d_x, d_y, d_map=None, stream=None):
         """(ms_range, ms_doppler): CUDA-event durations of the two CAF kernels for one CPI."""
         a, b = C.c_float(), C.c_float()
         n = d_x.numel() if hasattr(d_x, "numel") else self.geometry.n_used
         capi.check(self._lib.b200dd_caf_profile_device(self._h, capi.ptr(d_x), capi.ptr(d_y), int(n), capi.ptr(d_map),
-                                                       capi.ptr(stream) if stream else None, C.byref(a), C.byref(b)))
+                                                       self._st(stream), C.byref(a), C.byref(b)))
         return a.value, b.value
 
     def debug_range_matrix(self):
@@ -182,20 +205,10 @@ class Ambiguity:
     def stream_ptr(self) -> int:
         return int(self._lib.b200dd_caf_stream(self._h) or 0)
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_caf_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class WienerHopf:
+class WienerHopf(_Handle):
     """WienerHopf(delayMin, delayMax, nSamples) -- src/process/clutter/WienerHopf.h:68."""
+    _destroy = "b200dd_wh_destroy"
 
     def __init__(self, delayMin, delayMax, nSamples, device=-1):
         lib = capi.load()
@@ -221,13 +234,13 @@ class WienerHopf:
     def process_device(self, d_x, d_y, d_y_out=None, stream=None):
         out = d_y if d_y_out is None else d_y_out
         capi.check(self._lib.b200dd_wh_process_device(self._h, capi.ptr(d_x), capi.ptr(d_y), capi.ptr(out),
-                                                      capi.ptr(stream) if stream else None))
+                                                      self._st(stream)))
 
     def profile_device(self, d_x, d_y, d_y_out, stream=None):
         """(ms_corr, ms_solve, ms_apply): CUDA-event durations of the filter's stages."""
         a, b, c = C.c_float(), C.c_float(), C.c_float()
         capi.check(self._lib.b200dd_wh_profile_device(self._h, capi.ptr(d_x), capi.ptr(d_y), capi.ptr(d_y_out),
-                                                      capi.ptr(stream) if stream else None, C.byref(a), C.byref(b),
+                                                      self._st(stream), C.byref(a), C.byref(b),
                                                       C.byref(c)))
         return a.value, b.value, c.value
 
@@ -242,22 +255,12 @@ class WienerHopf:
         capi.check(self._lib.b200dd_wh_debug_weights(self._h, capi.ptr(w), capi.ptr(a), capi.ptr(b)))
         return w, a, b
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_wh_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class WienerHopfChunk:
+class WienerHopfChunk(_Handle):
     """The clutter filter on ONE CHUNK of a CPI that is split over several GPUs (SURVEY.md s8e row 3; C ABI
     b200dd_wh_create_chunk).  Device path only (complex64 CUDA tensors).  x_loc / y_loc are the chunk plus the
     halos `halos()` reports; blah2_b200.shard.wienerhopf_single_cpi_sharded drives it across ranks."""
+    _destroy = "b200dd_wh_destroy"
 
     def __init__(self, delayMin, delayMax, nSamples, chunk_begin, chunk_len, device=-1):
         lib = capi.load()
@@ -279,13 +282,13 @@ class WienerHopfChunk:
         """d_ab (complex128 CUDA tensor, 2 nBins) <- this chunk's share of (a, b)."""
         assert d_x_loc.numel() == self.x_left + self.chunk_len + self.x_right and d_y_loc.numel() == self.chunk_len + self.y_right
         capi.check(self._lib.b200dd_wh_chunk_corr_device(self._h, capi.ptr(d_x_loc), capi.ptr(d_y_loc), capi.ptr(d_ab),
-                                                         capi.ptr(stream) if stream else None))
+                                                         self._st(stream)))
 
     def filter_device(self, d_ab, d_x_loc, d_y_loc, d_y_out, stream=None):
         """Replicated solve on the summed d_ab, then the chunk's chunk_len filtered samples into d_y_out."""
         assert d_y_out.numel() == self.chunk_len
         capi.check(self._lib.b200dd_wh_chunk_filter_device(self._h, capi.ptr(d_ab), capi.ptr(d_x_loc), capi.ptr(d_y_loc),
-                                                           capi.ptr(d_y_out), capi.ptr(stream) if stream else None))
+                                                           capi.ptr(d_y_out), self._st(stream)))
 
     def last_status(self) -> bool:
         rc = capi.check(self._lib.b200dd_wh_last_status(self._h), allow=(capi.FILTER_FAILED,))
@@ -299,23 +302,13 @@ class WienerHopfChunk:
         capi.check(self._lib.b200dd_wh_debug_weights(self._h, capi.ptr(w), capi.ptr(a), capi.ptr(b)))
         return w, a, b
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_wh_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class SpectrumAnalyser:
+class SpectrumAnalyser(_Handle):
     """SpectrumAnalyser(n, bandwidth) -- src/process/spectrum/SpectrumAnalyser.h:48.
 
     ``process(x)`` returns ``(spectrum, frequency)``: the two vectors the reference hands to
     ``IqData::update_spectrum`` / ``update_frequency`` (SpectrumAnalyser.cpp:55,68)."""
+    _destroy = "b200dd_spectrum_destroy"
 
     def __init__(self, n, bandwidth, device=-1):
         lib = capi.load()
@@ -342,35 +335,25 @@ class SpectrumAnalyser:
         n = d_x.numel()
         f64 = getattr(d_x, "element_size", lambda: 8)() == 16
         fn = self._lib.b200dd_spectrum_process_device_f64 if f64 else self._lib.b200dd_spectrum_process_device
-        capi.check(fn(self._h, capi.ptr(d_x), int(n), capi.ptr(d_spectrum), capi.ptr(stream) if stream else None))
+        capi.check(fn(self._h, capi.ptr(d_x), int(n), capi.ptr(d_spectrum), self._st(stream)))
 
     def fetch(self, stream=None):
         out = np.empty(self.nSpectrum, dtype=np.complex128)
-        capi.check(self._lib.b200dd_spectrum_fetch(self._h, capi.ptr(out), capi.ptr(stream) if stream else None))
+        capi.check(self._lib.b200dd_spectrum_fetch(self._h, capi.ptr(out), self._st(stream)))
         return out
 
     def profile_device(self, d_x, stream=None):
         """(ms_fold, ms_rest): CUDA-event durations of the folding pass and of reduction + DFT."""
         a, b = C.c_float(), C.c_float()
         capi.check(self._lib.b200dd_spectrum_profile_device(self._h, capi.ptr(d_x), int(d_x.numel()),
-                                                            capi.ptr(stream) if stream else None, C.byref(a),
+                                                            self._st(stream), C.byref(a),
                                                             C.byref(b)))
         return a.value, b.value
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_spectrum_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class _DetHandle:
+class _DetHandle(_Handle):
     """One b200dd_det handle shared by the three detection classes of a pipeline."""
+    _destroy = "b200dd_det_destroy"
 
     def __init__(self, pfa=1e-5, nGuard=0, nTrain=0, minDelay=0, minDoppler=0.0, nCentroidDelay=0,
                  nCentroidDoppler=0, resolutionDoppler=1.0, doDelay=True, doDoppler=True, max_doppler_bins=8192,
@@ -408,14 +391,14 @@ class _DetHandle:
         capi.check(self._lib.b200dd_det_process_device(self._h, last_stage, capi.ptr(d_map), int(nDop), int(nDel),
                                                        capi.ptr(delay), capi.ptr(doppler), float(noisePower),
                                                        capi.ptr(od), capi.ptr(of), capi.ptr(os_), self.cap,
-                                                       C.byref(n), capi.ptr(stream) if stream else None))
+                                                       C.byref(n), self._st(stream)))
         k = n.value
         return Detection(od[:k].copy(), of[:k].copy(), os_[:k].copy())
 
     def set_metrics_device(self, d_map, nDop, nDel, stream=None):
         out = np.empty(2, dtype=np.float64)
         capi.check(self._lib.b200dd_det_set_metrics_device(self._h, capi.ptr(d_map), int(nDop), int(nDel),
-                                                           capi.ptr(out), capi.ptr(stream) if stream else None))
+                                                           capi.ptr(out), self._st(stream)))
         return float(out[0]), float(out[1])
 
     def centroid(self, det: Detection) -> Detection:
@@ -446,17 +429,6 @@ class _DetHandle:
                                                          capi.ptr(od), capi.ptr(of), capi.ptr(os_), cap, C.byref(n)))
         k = n.value
         return Detection(od[:k].copy(), of[:k].copy(), os_[:k].copy())
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_det_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class CfarDetector1D:
@@ -505,10 +477,11 @@ def set_metrics(m: Map) -> Map:
     return m
 
 
-class MapJson:
+class MapJson(_Handle):
     """The map document of blah2.cpp:303-304 for maps of one shape: ``render_host`` for a complex128 host map,
     ``render_device`` + ``fetch`` for a device map (float2 / complex64, or complex128).  Raises B200ddError with
     code ERR_NONFINITE for a map cell with |z| = 0, inf or NaN, which has no JSON text."""
+    _destroy = "b200dd_mapjson_destroy"
 
     def __init__(self, delay, doppler, fs, device=-1):
         lib = capi.load()
@@ -536,12 +509,12 @@ class MapJson:
         import torch
         f64 = d_map.dtype in (torch.complex128, torch.float64)
         capi.check(self._lib.b200dd_mapjson_render_device(self._h, capi.ptr(d_map), int(f64), float(noisePower),
-                                                          float(maxPower), capi.ptr(stream) if stream else None))
+                                                          float(maxPower), self._st(stream)))
 
     def fetch(self, timestamp, stream=None) -> bytes:
         n = C.c_size_t()
         capi.check(self._lib.b200dd_mapjson_fetch(self._h, int(timestamp), capi.ptr(self._out), self._out.size,
-                                                  C.byref(n), capi.ptr(stream) if stream else None))
+                                                  C.byref(n), self._st(stream)))
         return self._out[:n.value].tobytes()
 
     def cell_values(self, d_map, noisePower):
@@ -554,24 +527,14 @@ class MapJson:
         torch.cuda.synchronize(d_map.device)
         return out.cpu().numpy()
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_mapjson_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class MaxHold:
+class MaxHold(_Handle):
     """The max-hold map document blah2's API serves at /stash/map (api/stash/maxhold.js): per cell the maximum
     over the last 20 accepted CPIs, with the latest one's header.  ``push_device`` adds a CPI's device map
     (complex64 or complex128) with its set_metrics values; ``fetch`` renders the document.  ``fetch`` raises
     B200ddError with code ERR_NONFINITE when the last push was rejected (a cell or metric without JSON text) and
     ERR_ARG when nothing is held yet."""
+    _destroy = "b200dd_maxhold_destroy"
 
     def __init__(self, delay, doppler, fs, device=-1):
         lib = capi.load()
@@ -589,33 +552,23 @@ class MaxHold:
         import torch
         f64 = d_map.dtype in (torch.complex128, torch.float64)
         capi.check(self._lib.b200dd_maxhold_push_device(self._h, capi.ptr(d_map), int(f64), float(noisePower),
-                                                        float(maxPower), capi.ptr(stream) if stream else None))
+                                                        float(maxPower), self._st(stream)))
 
     def fetch(self, timestamp, stream=None) -> bytes:
         n = C.c_size_t()
         capi.check(self._lib.b200dd_maxhold_fetch(self._h, int(timestamp), capi.ptr(self._out), self._out.size,
-                                                  C.byref(n), capi.ptr(stream) if stream else None))
+                                                  C.byref(n), self._st(stream)))
         return self._out[:n.value].tobytes()
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_maxhold_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class DetectionJson:
+class DetectionJson(_Handle):
     """The detection document of blah2.cpp:312-317 and the API's /stash/detection history (api/stash/detection.js)
     of up to ``max_held`` detections.  ``render_device`` renders a device detection list (float64 tensors, the count
     in a uint32 / int32 device word); ``fetch`` writes its document and commits it to the history;
     ``fetch_stash`` writes the history.  ``render_host`` needs no handle and no device.  Raises B200ddError with code
     ERR_NONFINITE for a value without JSON text, ERR_CAPACITY for more than 2^18 detections or an overflowed history
     (see include/b200dd.h)."""
+    _destroy = "b200dd_detjson_destroy"
 
     def __init__(self, fs, max_held=1 << 20, device=-1):
         lib = capi.load()
@@ -632,18 +585,18 @@ class DetectionJson:
         """Asynchronous: the three lists are float64 device tensors, d_count a one-word device tensor."""
         capi.check(self._lib.b200dd_detjson_render_device(self._h, capi.ptr(d_delay), capi.ptr(d_doppler),
                                                           capi.ptr(d_snr), capi.ptr(d_count),
-                                                          capi.ptr(stream) if stream else None))
+                                                          self._st(stream)))
 
     def fetch(self, timestamp, stream=None) -> bytes:
         n = C.c_size_t()
         capi.check(self._lib.b200dd_detjson_fetch(self._h, int(timestamp), capi.ptr(self._out), self._out.size,
-                                                  C.byref(n), capi.ptr(stream) if stream else None))
+                                                  C.byref(n), self._st(stream)))
         return self._out[:n.value].tobytes()
 
     def fetch_stash(self, stream=None) -> bytes:
         n = C.c_size_t()
         capi.check(self._lib.b200dd_detjson_fetch_stash(self._h, capi.ptr(self._stash), self._stash.size, C.byref(n),
-                                                        capi.ptr(stream) if stream else None))
+                                                        self._st(stream)))
         return self._stash[:n.value].tobytes()
 
     @staticmethod
@@ -659,25 +612,15 @@ class DetectionJson:
                                                   int(timestamp), int(fs), capi.ptr(out), out.size, C.byref(n)))
         return out[:n.value].tobytes()
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_detjson_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class IqDataJson:
+class IqDataJson(_Handle):
     """The IQ-data document of blah2.cpp:299-300 (IqData::to_json of the spectrum) and the API's /stash/iqdata history
     of the last 20 documents (api/stash/iqdata.js).  ``min``, ``max`` and ``mean`` are the IqData members the document
     carries (blah2 never assigns them); they must be finite.  ``render_device`` renders a device spectrum (a complex128
     tensor of ``n_spectrum`` bins); ``fetch`` writes its document and commits it to the history; ``fetch_stash`` writes
     the history.  ``render_host`` needs no handle and no device.  Raises B200ddError with code ERR_NONFINITE for a
     bin that is zero, infinite or NaN (see include/b200dd.h)."""
+    _destroy = "b200dd_iqjson_destroy"
 
     def __init__(self, n_spectrum, min, max, mean, device=-1):
         lib = capi.load()
@@ -695,18 +638,18 @@ class IqDataJson:
     def render_device(self, d_spectrum, stream=None):
         """Asynchronous: d_spectrum is a complex128 device tensor of n_spectrum bins."""
         capi.check(self._lib.b200dd_iqjson_render_device(self._h, capi.ptr(d_spectrum),
-                                                         capi.ptr(stream) if stream else None))
+                                                         self._st(stream)))
 
     def fetch(self, timestamp, stream=None) -> bytes:
         n = C.c_size_t()
         capi.check(self._lib.b200dd_iqjson_fetch(self._h, int(timestamp), capi.ptr(self._out), self._out.size,
-                                                 C.byref(n), capi.ptr(stream) if stream else None))
+                                                 C.byref(n), self._st(stream)))
         return self._out[:n.value].tobytes()
 
     def fetch_stash(self, stream=None) -> bytes:
         n = C.c_size_t()
         capi.check(self._lib.b200dd_iqjson_fetch_stash(self._h, capi.ptr(self._stash), self._stash.size, C.byref(n),
-                                                       capi.ptr(stream) if stream else None))
+                                                       self._st(stream)))
         return self._stash[:n.value].tobytes()
 
     def bin_values(self, d_spectrum):
@@ -727,17 +670,6 @@ class IqDataJson:
         capi.check(lib.b200dd_iqjson_render_host(capi.ptr(s), s.size, float(min), float(max), float(mean),
                                                  int(timestamp), capi.ptr(out), out.size, C.byref(n)))
         return out[:n.value].tobytes()
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_iqjson_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def timing_render_host(t_start, t_now, n, names, values) -> bytes:
@@ -765,12 +697,13 @@ def _fetch_growing(buf, call):
     return buf, buf[:n].tobytes()
 
 
-class Tracker:
+class Tracker(_Handle):
     """blah2's Tracker (src/process/tracker/Tracker.cpp) with its tracks on the device, named like the reference's
     constructor Tracker(m, n, nDelete, cpi, maxAccInit, rangeRes, lambda) with rangeRes = c / fs and lambda = c / fc
     given as fs and fc (blah2.cpp:193-195).  ``process_device`` / ``process_host`` run Tracker::process on one CPI's
     detections; ``fetch`` returns Track::to_json(timestamp).  ``max_tracks`` and ``max_history`` bound the state: past
     them fetch raises ERR_CAPACITY until ``reset``.  A non-finite track value raises ERR_NONFINITE at fetch."""
+    _destroy = "b200dd_tracker_destroy"
 
     def __init__(self, m, n, nDelete, cpi, maxAcc, fs, fc, max_tracks=1 << 16, max_history=64, device=-1):
         lib = capi.load()
@@ -786,7 +719,7 @@ class Tracker:
         """Asynchronous: the lists are float64 device tensors, d_count a one-word device tensor."""
         capi.check(self._lib.b200dd_tracker_process_device(self._h, capi.ptr(d_delay), capi.ptr(d_doppler),
                                                            capi.ptr(d_snr), capi.ptr(d_count), int(timestamp),
-                                                           capi.ptr(stream) if stream else None))
+                                                           self._st(stream)))
 
     def process_host(self, delay, doppler, snr, timestamp, stream=None):
         v = [np.ascontiguousarray(np.asarray(a, dtype=np.float64).ravel()) for a in (delay, doppler, snr)]
@@ -794,13 +727,13 @@ class Tracker:
             raise ValueError("delay, doppler and snr differ in length")
         capi.check(self._lib.b200dd_tracker_process_host(self._h, capi.ptr(v[0]), capi.ptr(v[1]), capi.ptr(v[2]),
                                                          v[0].size, int(timestamp),
-                                                         capi.ptr(stream) if stream else None))
+                                                         self._st(stream)))
 
     def fetch(self, timestamp, stream=None) -> bytes:
         def call(buf):
             n = C.c_size_t()
             rc = self._lib.b200dd_tracker_fetch(self._h, int(timestamp), capi.ptr(buf), buf.size, C.byref(n),
-                                                capi.ptr(stream) if stream else None)
+                                                self._st(stream))
             return rc, n.value
         self._out, doc = _fetch_growing(self._out, call)
         return doc
@@ -808,22 +741,12 @@ class Tracker:
     def reset(self):
         capi.check(self._lib.b200dd_tracker_reset(self._h))
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_tracker_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class Pipeline:
+class Pipeline(_Handle):
     """One CPI through the body of the reference's process thread (src/blah2.cpp:268-287):
     [WienerHopf] -> Ambiguity -> Map::set_metrics -> [CfarDetector1D -> Centroid -> Interpolate],
     intermediates resident on the device.  Parameters are named like config/config.yml."""
+    _destroy = "b200dd_pipeline_destroy"
 
     def __init__(self, delayMin, delayMax, dopplerMin, dopplerMax, fs, nSamples, roundHamming=True, clutter=None,
                  detection=None, device=-1, max_detections=4096, spectrum_bandwidth=None, map_json=False,
@@ -1063,28 +986,17 @@ class Pipeline:
     def submit_device(self, d_x, d_y, d_map=None, stream=None):
         n = d_x.numel() if hasattr(d_x, "numel") else self.n_samples
         capi.check(self._lib.b200dd_pipeline_submit_device(self._h, capi.ptr(d_x), capi.ptr(d_y), int(n),
-                                                           capi.ptr(d_map), capi.ptr(stream) if stream else None))
+                                                           capi.ptr(d_map), self._st(stream)))
 
     def prepare_device(self, d_x, d_y, d_map=None, stream=None):
         """Plan creation for submit_device on this buffer triple (records the CUDA graph of the chain now)."""
         n = d_x.numel() if hasattr(d_x, "numel") else self.n_samples
         capi.check(self._lib.b200dd_pipeline_prepare_device(self._h, capi.ptr(d_x), capi.ptr(d_y), int(n),
-                                                            capi.ptr(d_map), capi.ptr(stream) if stream else None))
+                                                            capi.ptr(d_map), self._st(stream)))
 
     def fetch(self, stream=None):
         res = capi.CpiResult()
         capi.check(self._lib.b200dd_pipeline_fetch(self._h, C.byref(res), capi.ptr(self._od), capi.ptr(self._of),
                                                    capi.ptr(self._os), self.cap,
-                                                   capi.ptr(stream) if stream else None), allow=(capi.ERR_CAPACITY,))
+                                                   self._st(stream)), allow=(capi.ERR_CAPACITY,))
         return self._result(res)
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_pipeline_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

@@ -12,13 +12,16 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from .process import _Handle
 
-class Comm:
+
+class Comm(_Handle):
     """The C-ABI communicator (include/b200dd.h b200dd_comm_*: NCCL issued from C on its own stream).
 
     One per process / GPU.  The 128-byte NCCL id is created on rank 0 and handed to the other ranks through
     torch.distributed's default process group (any backend) -- plumbing; the data path below never touches torch.
     """
+    _destroy = "b200dd_comm_destroy"
 
     def __init__(self, rank: int, world: int, device: int):
         from . import capi
@@ -93,17 +96,6 @@ class Comm:
 
     def sync(self):
         self._capi.check(self._lib.b200dd_comm_sync(self._h))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.b200dd_comm_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def cpi_indices(n_cpis: int, rank: int, world: int) -> list[int]:
