@@ -186,6 +186,9 @@ SIGNATURES = [
                                             C.c_uint32, _VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("b200dd_timing_max_bytes", C.c_size_t, []),
     ("b200dd_pipeline_share_history", C.c_int, [_VP, C.c_uint32]),
+    ("b200dd_pipeline_enable_export", C.c_int, [_VP, C.c_uint32, C.POINTER(C.c_size_t)]),
+    ("b200dd_pipeline_export_record", C.c_int, [_VP, C.POINTER(_VP)]),
+    ("b200dd_pipeline_submit_record", C.c_int, [_VP, _VP, _VP]),
     ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),
     ("b200dd_mapjson_destroy", None, [_VP]),

@@ -178,6 +178,10 @@ struct DetDeviceList {
   uint32_t cap;
 };
 int det_device_list(b200dd_det *h, DetDeviceList *out);
+// det.cu: makes the handle's last async chain one that ran through `last_stage` (0: set_metrics only) on the device
+// noisePower, without launching anything: b200dd_det_chain_fetch and det_device_list then read the metrics words,
+// stage counts and list that such a chain leaves, whatever the caller writes there (a CPI computed elsewhere).
+void det_adopt_chain(b200dd_det *h, int last_stage);
 // detjson.cu: a render recorded in a graph was replayed (true), or the pipeline dropped the CPI's document (false).
 void detjson_mark_rendered(b200dd_detjson *h, bool rendered);
 // detjson.cu: B200DD_OK when no Interpolate result on these axes -- delay within one bin of the delay axis, Doppler

@@ -761,6 +761,12 @@ int b200dd_det_interpolate_host(b200dd_det *h, const double *delay, const double
 // the device word pair {noisePower, maxPower} that the async chain's set_metrics writes (for the map-JSON stage)
 const double *b2::det_device_metrics(b200dd_det *h) { return h->d_metrics; }
 
+void b2::det_adopt_chain(b200dd_det *h, int last_stage) {
+  // where run_chain leaves its results with the device noisePower (the tail kernel's buffers and count slots)
+  h->chain_buf = last_stage >= B200DD_DET_CENTROID && last_stage < B200DD_DET_INTERPOLATE ? 1 : 0;
+  h->chain_slot = last_stage >= B200DD_DET_INTERPOLATE ? 2 : (last_stage >= B200DD_DET_CENTROID ? 1 : -1);
+}
+
 int b2::det_device_list(b200dd_det *h, DetDeviceList *out) {
   if (h->chain_slot < 0) return arg_fail("det_device_list: the last chain ran no detection stage");
   out->delay = h->d_buf[h->chain_buf][0];

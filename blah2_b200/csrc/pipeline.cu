@@ -2,10 +2,12 @@
 // intermediates resident in HBM (the body of the reference's process thread, src/blah2.cpp:268-287).
 // Composes the per-class handles of caf.cu / wh.cu / det.cu / spectrum.cu / iqjson.cu / mapjson.cu / maxhold.cu / detjson.cu /
 // tracker.cu through their C ABI, and timing.cu's stamps and history; the only kernels
-// defined here are the host entry points' conversions: complex128 <-> complex64 and the int16 / int8 ingest.
+// defined here are the host entry points' conversions (complex128 <-> complex64, the int16 / int8 ingest) and the
+// CPI record's pack and unpack.
 #include "common.cuh"
 
 #include <algorithm>
+#include <cstring>
 #include <new>
 #include <string>
 #include <vector>
@@ -108,6 +110,121 @@ enum StageBit : unsigned {
   kShareBits = kIqBit | kMaxholdBit | kDetBit | kTrackBit | kTimingBit,  // the stages a share set takes over
 };
 
+// ---- CPI record (b200dd_pipeline_enable_export / _submit_record): one fixed-size device buffer per CPI holding
+// everything the fetches read besides the map.  Layout, each section 16-byte aligned, present as its stage is:
+//   RecHeader | uint64_t stamps[kTmSlots] (timing) | double2 spectrum[n_spectrum] (spectrum) |
+//   double delay[max_det], doppler[max_det], snr[max_det] (detection; slots past the count are zero)
+constexpr uint32_t kRecVersion = 1;
+constexpr uint32_t kRecMaxDetections = 1u << 18;  // the detection list's capacity (det.cu)
+
+struct RecHeader {
+  uint32_t version;
+  uint32_t path;            // TmPath of the submit: what the timing document counts as extract_buffer
+  uint64_t fingerprint;     // record_fingerprint of the exporting pipeline
+  uint64_t bytes;           // the record's size
+  uint32_t max_detections;  // detection slots
+  int32_t filter_status;    // the clutter filter's status word (0 without the filter)
+  uint32_t cfar_count;      // CFAR's count: above the list capacity, the CPI's list is invalid (CFAR overflow)
+  uint32_t count;           // the final list's length
+  uint32_t overflow;        // count > max_detections: only the first max_detections detections travelled
+  uint32_t pad;
+  double metrics[2];        // set_metrics: noisePower, maxPower
+};
+static_assert(sizeof(RecHeader) == 64, "the record header is 64 bytes");
+
+struct RecordLayout {
+  uint32_t max_det = 0, n_spec = 0;  // n_spec: 0 without the spectrum stage
+  bool timing = false, detection = false;
+  size_t off_tm = 0, off_spec = 0, off_det = 0, bytes = 0;
+};
+
+// The pipeline's words a chain leaves (written by its stages, read by its fetches): what the pack kernel copies into
+// the record and the unpack kernel writes back.  A null pointer is a stage the pipeline does not run.
+struct RecordArgs {
+  unsigned char *rec;
+  RecordLayout L;
+  uint64_t fingerprint;
+  uint32_t path;
+  uint32_t det_cap;
+  int *status;
+  double *metrics;
+  uint32_t *cfar, *count;
+  double *list[3];
+  uint64_t *stamps;
+  double2 *spectrum;
+};
+
+__global__ void __launch_bounds__(256) pl_pack_kernel(RecordArgs a) {
+  const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+  const uint32_t count = a.count ? *a.count : 0u, kept = min(count, a.L.max_det);
+  if (tid == 0) {
+    RecHeader h;
+    h.version = kRecVersion;
+    h.path = a.path;
+    h.fingerprint = a.fingerprint;
+    h.bytes = a.L.bytes;
+    h.max_detections = a.L.max_det;
+    h.filter_status = a.status ? *a.status : 0;
+    h.cfar_count = a.cfar ? *a.cfar : 0u;
+    h.count = count;
+    h.overflow = count > a.L.max_det ? 1u : 0u;
+    h.pad = 0;
+    h.metrics[0] = a.metrics[0];
+    h.metrics[1] = a.metrics[1];
+    *reinterpret_cast<RecHeader *>(a.rec) = h;
+  }
+  if (a.stamps) {
+    uint64_t *t = reinterpret_cast<uint64_t *>(a.rec + a.L.off_tm);
+    for (uint32_t i = tid; i < kTmSlots; i += stride) t[i] = a.stamps[i];
+  }
+  if (a.spectrum) {
+    double2 *s = reinterpret_cast<double2 *>(a.rec + a.L.off_spec);
+    for (uint32_t i = tid; i < a.L.n_spec; i += stride) s[i] = a.spectrum[i];
+  }
+  if (a.count) {
+    double *d = reinterpret_cast<double *>(a.rec + a.L.off_det);
+    for (uint32_t i = tid; i < a.L.max_det; i += stride) {
+      const bool in = i < kept;
+      d[i] = in ? a.list[0][i] : 0.0;
+      d[a.L.max_det + i] = in ? a.list[1][i] : 0.0;
+      d[2 * (size_t)a.L.max_det + i] = in ? a.list[2][i] : 0.0;
+    }
+  }
+}
+
+// The inverse of pl_pack_kernel into an importing pipeline's words.  A record overflow leaves CFAR's count above the
+// list capacity, so that every fetch treats it as a CFAR overflow.  The tracker's stamps stay the importer's own.
+__global__ void __launch_bounds__(256) pl_unpack_kernel(RecordArgs a) {
+  const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+  const RecHeader *h = reinterpret_cast<const RecHeader *>(a.rec);
+  const uint32_t kept = min(h->count, a.L.max_det);
+  if (tid == 0) {
+    a.metrics[0] = h->metrics[0];
+    a.metrics[1] = h->metrics[1];
+    if (a.status) *a.status = h->filter_status;
+    if (a.count) {
+      *a.cfar = h->overflow ? max(h->cfar_count, a.det_cap + 1u) : h->cfar_count;
+      *a.count = kept;
+    }
+  }
+  if (a.stamps) {
+    const uint64_t *t = reinterpret_cast<const uint64_t *>(a.rec + a.L.off_tm);
+    for (uint32_t i = tid; i < kTmTracker0; i += stride) a.stamps[i] = t[i];
+  }
+  if (a.spectrum) {
+    const double2 *s = reinterpret_cast<const double2 *>(a.rec + a.L.off_spec);
+    for (uint32_t i = tid; i < a.L.n_spec; i += stride) a.spectrum[i] = s[i];
+  }
+  if (a.count) {
+    const double *d = reinterpret_cast<const double *>(a.rec + a.L.off_det);
+    for (uint32_t i = tid; i < kept; i += stride) {
+      a.list[0][i] = d[i];
+      a.list[1][i] = d[a.L.max_det + i];
+      a.list[2][i] = d[2 * (size_t)a.L.max_det + i];
+    }
+  }
+}
+
 }  // namespace
 
 // The stateful stages of a share set (b200dd_pipeline_share_history): one max-hold window, one detection history,
@@ -199,6 +316,12 @@ struct b200dd_pipeline {
   b200dd_tracker_params tr_params{};
   uint32_t tr_max_tracks = 0, tr_max_history = 0;
   ShareSet *set = nullptr;  // share-set membership: the stateful stages above are null and the set's are used
+  // CPI export (b200dd_pipeline_enable_export): every submit packs its record into d_rec; exp_max == 0 is off
+  uint32_t exp_max = 0;
+  RecordLayout exp_layout;
+  uint64_t exp_fingerprint = 0;
+  DevBuf<unsigned char> d_rec;
+  bool exp_valid = false;  // d_rec holds the last submit's record
 };
 
 static void pipeline_drop_graphs(b200dd_pipeline *h) {
@@ -342,6 +465,109 @@ static int tm_stamp(b200dd_pipeline *h, int slot, void *st) {
   return h->tm_on ? timing_stamp(h->d_tm + slot, (cudaStream_t)st) : B200DD_OK;
 }
 
+// The record layout of `h`'s stages with max_det detection slots.
+static RecordLayout record_layout(const b200dd_pipeline *h, uint32_t max_det) {
+  auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+  RecordLayout L;
+  L.timing = h->tm_on;
+  L.detection = h->p.detection_enable != 0;
+  L.n_spec = h->spec ? h->spec_bins : 0;
+  L.max_det = max_det;
+  L.off_tm = sizeof(RecHeader);
+  L.off_spec = up16(L.off_tm + (L.timing ? sizeof(uint64_t) * kTmSlots : 0));
+  L.off_det = up16(L.off_spec + sizeof(double2) * L.n_spec);
+  L.bytes = up16(L.off_det + (L.detection ? 3 * sizeof(double) * (size_t)max_det : 0));
+  return L;
+}
+
+// FNV-1a over everything that shapes a record's products: the CAF, clutter-filter and detection parameters (not the
+// device), the spectrum stage, the timing stage and the layout.  Exporter and importer must agree on it.
+static uint64_t record_fingerprint(const b200dd_pipeline *h, const RecordLayout &L) {
+  uint64_t f = 1469598103934665603ull;
+  auto mix = [&f](uint64_t v) {
+    for (int i = 0; i < 8; i++) {
+      f ^= (v >> (8 * i)) & 0xFFu;
+      f *= 1099511628211ull;
+    }
+  };
+  auto mixd = [&mix](double d) {
+    uint64_t v;
+    memcpy(&v, &d, sizeof v);
+    mix(v);
+  };
+  const b200dd_caf_params &c = h->p.caf;
+  const b200dd_det_params &d = h->p.det;
+  mix(kRecVersion);
+  mix((uint64_t)(int64_t)c.delay_min); mix((uint64_t)(int64_t)c.delay_max);
+  mix((uint64_t)(int64_t)c.doppler_min); mix((uint64_t)(int64_t)c.doppler_max);
+  mix(c.fs); mix(c.n_samples); mix((uint64_t)c.round_hamming);
+  mix((uint64_t)h->p.clutter_enable);
+  if (h->p.clutter_enable) { mix((uint64_t)(int64_t)h->p.clutter_delay_min); mix((uint64_t)(int64_t)h->p.clutter_delay_max); }
+  mix((uint64_t)h->p.detection_enable);
+  if (h->p.detection_enable) {
+    mixd(d.pfa); mix((uint64_t)(int64_t)d.n_guard); mix((uint64_t)(int64_t)d.n_train); mix((uint64_t)(int64_t)d.min_delay);
+    mixd(d.min_doppler); mix((uint64_t)(int64_t)d.n_centroid_delay); mix((uint64_t)(int64_t)d.n_centroid_doppler);
+    mixd(d.resolution_doppler); mix((uint64_t)(int64_t)d.interp_delay); mix((uint64_t)(int64_t)d.interp_doppler);
+  }
+  mix(L.n_spec);
+  if (L.n_spec) mixd(h->spec_bandwidth);
+  mix(L.timing ? 1 : 0);
+  mix(L.max_det);
+  mix(L.bytes);
+  return f;
+}
+
+// The record `rec` of layout L and `h`'s words it travels between: the stages' device buffers, which the pack kernel
+// reads and the unpack kernel writes (the pipeline owns those stages).
+static int record_args(b200dd_pipeline *h, const void *rec, const RecordLayout &L, uint64_t fingerprint, int path,
+                       RecordArgs *a) {
+  *a = RecordArgs{};
+  a->rec = (unsigned char *)rec;
+  a->L = L;
+  a->fingerprint = fingerprint;
+  a->path = (uint32_t)path;
+  a->status = h->wh ? const_cast<int *>(b200dd_wh_device_status(h->wh)) : nullptr;
+  a->metrics = const_cast<double *>(det_device_metrics(h->det));
+  if (L.detection) {
+    DetDeviceList l;
+    const int rc = det_device_list(h->det, &l);
+    if (rc != B200DD_OK) return rc;
+    a->cfar = const_cast<uint32_t *>(l.cfar_count);
+    a->count = const_cast<uint32_t *>(l.count);
+    a->list[0] = const_cast<double *>(l.delay);
+    a->list[1] = const_cast<double *>(l.doppler);
+    a->list[2] = const_cast<double *>(l.snr);
+    a->det_cap = l.cap;
+  }
+  if (L.timing) a->stamps = h->d_tm;
+  if (L.n_spec) a->spectrum = (double2 *)const_cast<void *>(spectrum_device_output(h->spec));
+  return B200DD_OK;
+}
+
+static int record_grid(const RecordLayout &L) { return grid_for(std::max<uint32_t>({L.max_det, L.n_spec, (uint32_t)kTmSlots})); }
+
+// the export's layout, fingerprint and buffer for the stages `h` has now (enable_export, and enabling the spectrum or
+// timing stage while export is on: both synchronise the stream and drop the graphs first)
+static int export_layout(b200dd_pipeline *h) {
+  const RecordLayout L = record_layout(h, h->exp_max);
+  if (!h->d_rec || L.bytes != h->exp_layout.bytes) B2_CUDA(h->d_rec.alloc(L.bytes));
+  h->exp_layout = L;
+  h->exp_fingerprint = record_fingerprint(h, L);
+  h->exp_valid = false;
+  return B200DD_OK;
+}
+
+// the pack kernel of the CPI just enqueued on `st` (nothing when export is off)
+static int export_pack(b200dd_pipeline *h, int path, void *st) {
+  if (!h->exp_max) return B200DD_OK;
+  RecordArgs a;
+  const int rc = record_args(h, h->d_rec, h->exp_layout, h->exp_fingerprint, path, &a);
+  if (rc != B200DD_OK) return rc;
+  pl_pack_kernel<<<record_grid(h->exp_layout), 256, 0, (cudaStream_t)st>>>(a);
+  B2_LAUNCH_CHECK();
+  return B200DD_OK;
+}
+
 // after the spectrum kernels on `st`: the IQ-data document of their output, from the spectrum's own buffer, and the
 // spectrum's closing stamp
 static int pipeline_enqueue_after_spectrum(b200dd_pipeline *h, void *st) {
@@ -352,8 +578,10 @@ static int pipeline_enqueue_after_spectrum(b200dd_pipeline *h, void *st) {
   return tm_stamp(h, kTmSpectrum, st);
 }
 
-// the CAF of x and y into `map`, set_metrics and the detection stages, then the products after them, on `st`
-static int pipeline_enqueue_tail(b200dd_pipeline *h, const void *x, const void *y, uint32_t n, float2 *map, void *st) {
+// the CAF of x and y into `map`, set_metrics and the detection stages, then the products after them and, with export
+// on, the record of a submit that came in by `path` (TmPath), on `st`
+static int pipeline_enqueue_tail(b200dd_pipeline *h, const void *x, const void *y, uint32_t n, float2 *map, int path,
+                                 void *st) {
   int rc = b200dd_caf_process_device(h->caf, x, y, n, map, st);
   if (rc != B200DD_OK) return rc;
   // Map::set_metrics runs after every Ambiguity::process, detection or not (blah2.cpp:278-279): stage 0 = metrics only
@@ -363,11 +591,13 @@ static int pipeline_enqueue_tail(b200dd_pipeline *h, const void *x, const void *
   if (rc == B200DD_OK && h->p.detection_enable) rc = tm_stamp(h, kTmDetector, st);
   if (rc == B200DD_OK) rc = pipeline_enqueue_products(h, map, st);
   if (rc == B200DD_OK) rc = tm_stamp(h, kTmOutput, st);
+  if (rc == B200DD_OK) rc = export_pack(h, path, st);
   return rc;
 }
 
 // the kernels of one CPI on device-resident IQ, enqueued on `st` (also what a graph capture records)
-static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map, void *st) {
+static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
+                                   int path, void *st) {
   const void *y = d_y;
   int rc = tm_stamp(h, kTmChain, st);
   if (rc != B200DD_OK) return rc;
@@ -383,7 +613,7 @@ static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const vo
     if (rc != B200DD_OK) return rc;
     y = h->d_yf;
   }
-  return pipeline_enqueue_tail(h, d_x, y, n, d_map ? (float2 *)d_map : h->d_map, st);
+  return pipeline_enqueue_tail(h, d_x, y, n, d_map ? (float2 *)d_map : h->d_map, path, st);
 }
 
 // After a submit enqueued its CPI on `st`, eagerly or as a graph replay, with map `map` (null: the pipeline's own):
@@ -407,6 +637,7 @@ static void pipeline_submitted(b200dd_pipeline *h, int path, void *st, const voi
   // an eager render marks its document itself; a replayed one cannot
   if (h->dj) detjson_mark_rendered(h->dj, true);
   if (h->ij) iqjson_mark_rendered(h->ij, true);
+  h->exp_valid = h->exp_max != 0;
 }
 
 static const b200dd_pipeline::GraphEntry *pipeline_find_graph(const b200dd_pipeline *h, const void *d_x, const void *d_y,
@@ -427,10 +658,11 @@ static int member_may_submit(const b200dd_pipeline *h, const char *msg) {
 // Replay pays off in a submit -> fetch -> submit loop; in a deep queue of CPIs enqueued ahead eager launches can be
 // faster, so replay is opt-in per triple (b200dd_pipeline_prepare_device).
 static int pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
-                                  void *st) {
+                                  int path, void *st) {
   DeviceGuard guard(h->device);
-  const b200dd_pipeline::GraphEntry *g = pipeline_find_graph(h, d_x, d_y, n, d_map);
-  if (!g) return pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
+  // a graph records b200dd_pipeline_submit_device's chain, whose record says so
+  const b200dd_pipeline::GraphEntry *g = path == kTmDevice ? pipeline_find_graph(h, d_x, d_y, n, d_map) : nullptr;
+  if (!g) return pipeline_enqueue_device(h, d_x, d_y, n, d_map, path, st);
   B2_CUDA(cudaGraphLaunch(g->exec, (cudaStream_t)st));
   return B200DD_OK;
 }
@@ -442,7 +674,7 @@ int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
   int rc = member_may_submit(h, "b200dd_pipeline_submit_device: the share-set member's last CPI is not fetched yet");
   if (rc != B200DD_OK) return rc;
   void *st = stream ? stream : (void *)h->stream;
-  rc = pipeline_submit_device(h, d_x, d_y, n, d_map, st);
+  rc = pipeline_submit_device(h, d_x, d_y, n, d_map, kTmDevice, st);
   if (rc == B200DD_OK) pipeline_submitted(h, kTmDevice, st, d_map);
   return rc;
 }
@@ -458,13 +690,13 @@ int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const vo
     // the eager run sets up what a capture must not do (uploads the axes, sizes scratch buffers); it is a CPI
     int rc = member_may_submit(h, "b200dd_pipeline_prepare_device: the share-set member's last CPI is not fetched yet");
     if (rc != B200DD_OK) return rc;
-    rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
+    rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, kTmDevice, st);
     if (rc != B200DD_OK) return rc;
     pipeline_submitted(h, kTmDevice, st, d_map);
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     if (cudaStreamBeginCapture((cudaStream_t)st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-      rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, st);
+      rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, kTmDevice, st);
       const cudaError_t ce = cudaStreamEndCapture((cudaStream_t)st, &graph);
       if (rc == B200DD_OK && ce == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) != cudaSuccess) exec = nullptr;
       if (graph) cudaGraphDestroy(graph);
@@ -631,7 +863,7 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
   pl_narrow_kernel<<<grid_for(need), 256, 0, st>>>(h->d_yd, h->d_yf2, need);
   B2_LAUNCH_CHECK();
   rc = tm_stamp(h, kTmNarrow, st);
-  if (rc == B200DD_OK) rc = pipeline_enqueue_tail(h, h->d_xf, h->d_yf2, need, h->d_map, st);
+  if (rc == B200DD_OK) rc = pipeline_enqueue_tail(h, h->d_xf, h->d_yf2, need, h->d_map, kTmHost, st);
   if (rc == B200DD_OK) rc = host_submitted(h, kTmHost, map_out);
   return rc;
 }
@@ -655,7 +887,7 @@ static int host_ingest(b200dd_pipeline *h, const char *entry, HostFormat fmt, ui
   rc = host_staging(h, fmt, map_out != nullptr);
   if (rc == B200DD_OK) rc = tm_stamp(h, kTmExtract0, h->stream);
   if (rc == B200DD_OK) rc = ingest(need_x);
-  if (rc == B200DD_OK) rc = pipeline_submit_device(h, h->d_xf, h->d_yf2, need_x, h->d_map, h->stream);
+  if (rc == B200DD_OK) rc = pipeline_submit_device(h, h->d_xf, h->d_yf2, need_x, h->d_map, kTmIngest, h->stream);
   if (rc == B200DD_OK) rc = host_submitted(h, kTmIngest, map_out);
   return rc;
 }
@@ -733,7 +965,7 @@ int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32
   h->spec_nfft = sg.nfft;
   h->spec_bandwidth = bandwidth;
   if (n_spectrum) *n_spectrum = sg.n_spectrum;
-  return B200DD_OK;
+  return h->exp_max ? export_layout(h) : B200DD_OK;
 }
 
 int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectrum_out, uint32_t cap) {
@@ -1005,7 +1237,7 @@ int b200dd_pipeline_enable_timing_json(b200dd_pipeline *h, uint64_t t_start, siz
   det_set_metrics_stamp(h->det, h->d_tm + kTmAmbiguity);
   if (doc_bytes) *doc_bytes = timing_doc_max_bytes();
   if (stash_bytes) *stash_bytes = timing_stash_max_bytes();
-  return B200DD_OK;
+  return h->exp_max ? export_layout(h) : B200DD_OK;
 }
 
 // blah2's stage names and values of the last submit (blah2.cpp:251-338), from its device stamps
@@ -1112,6 +1344,63 @@ int b200dd_pipeline_process_host(b200dd_pipeline *h, const double *x, const doub
   int rc = b200dd_pipeline_submit_host(h, x, y, n, map_out);
   if (rc != B200DD_OK) return rc;
   return b200dd_pipeline_fetch(h, result, o_delay, o_doppler, o_snr, cap, h->stream);
+}
+
+int b200dd_pipeline_enable_export(b200dd_pipeline *h, uint32_t max_detections, size_t *record_bytes) {
+  if (record_bytes) *record_bytes = 0;
+  if (max_detections == 0 || max_detections > kRecMaxDetections)
+    return arg_fail("b200dd_pipeline_enable_export: max_detections outside [1, 2^18]");
+  if (!h) return arg_fail("b200dd_pipeline_enable_export: null handle");
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaStreamSynchronize(h->stream));
+  pipeline_drop_graphs(h);  // they do not pack the record
+  h->exp_max = max_detections;
+  const int rc = export_layout(h);
+  if (rc != B200DD_OK) {
+    h->exp_max = 0;
+    return rc;
+  }
+  if (record_bytes) *record_bytes = h->exp_layout.bytes;
+  return B200DD_OK;
+}
+
+int b200dd_pipeline_export_record(b200dd_pipeline *h, const void **d_record) {
+  if (d_record) *d_record = nullptr;
+  if (!h || !d_record) return arg_fail("b200dd_pipeline_export_record: null argument");
+  if (!h->exp_max) return arg_fail("b200dd_pipeline_export_record: export is not enabled");
+  if (!h->exp_valid) return arg_fail("b200dd_pipeline_export_record: no CPI submitted since export was enabled");
+  *d_record = h->d_rec;
+  return B200DD_OK;
+}
+
+int b200dd_pipeline_submit_record(b200dd_pipeline *h, const void *d_record, const void *d_map) {
+  if (!h || !d_record || !d_map) return arg_fail("b200dd_pipeline_submit_record: null argument");
+  int rc = member_may_submit(h, "b200dd_pipeline_submit_record: the share-set member's last CPI is not fetched yet");
+  if (rc != B200DD_OK) return rc;
+  DeviceGuard guard(h->device);
+  cudaStream_t st = h->stream;
+  RecHeader hd;
+  B2_CUDA(cudaMemcpyAsync(&hd, d_record, sizeof(hd), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  if (hd.version != kRecVersion) return arg_fail("b200dd_pipeline_submit_record: not a CPI record of this version");
+  if (hd.max_detections == 0 || hd.max_detections > kRecMaxDetections || hd.path < kTmHost || hd.path > kTmDevice)
+    return arg_fail("b200dd_pipeline_submit_record: not a CPI record");
+  const RecordLayout L = record_layout(h, hd.max_detections);
+  if (hd.bytes != L.bytes || hd.fingerprint != record_fingerprint(h, L))
+    return arg_fail("b200dd_pipeline_submit_record: the record comes from a pipeline of other parameters or stages");
+  det_adopt_chain(h->det, h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0);
+  RecordArgs a;
+  rc = record_args(h, d_record, L, hd.fingerprint, (int)hd.path, &a);
+  if (rc != B200DD_OK) return rc;
+  pl_unpack_kernel<<<record_grid(L), 256, 0, st>>>(a);
+  B2_LAUNCH_CHECK();
+  // the renders a submit runs after its chain, on the imported words and the gathered map
+  if (h->ij) rc = b200dd_iqjson_render_device(h->ij, spectrum_device_output(h->spec), st);
+  if (rc == B200DD_OK) rc = pipeline_enqueue_products(h, (float2 *)const_cast<void *>(d_map), st);
+  if (rc != B200DD_OK) return rc;
+  pipeline_submitted(h, (int)hd.path, st, d_map);
+  h->exp_valid = false;  // the import packed nothing
+  return B200DD_OK;
 }
 
 

@@ -742,6 +742,22 @@ class Tracker(_Handle):
         capi.check(self._lib.b200dd_tracker_reset(self._h))
 
 
+def record_bytes(max_detections, n_spectrum=0, timing=False, detection=True) -> int:
+    """The size of a pipeline's CPI record (b200dd_pipeline_enable_export): a 64-byte header, 80 bytes of stage stamps
+    with the timing stage, 16 bytes per spectrum bin with the spectrum stage and 24 bytes per detection slot with
+    detection, rounded up to 16 bytes."""
+    n = 64 + (80 if timing else 0) + 16 * int(n_spectrum) + (24 * int(max_detections) if detection else 0)
+    return (n + 15) // 16 * 16
+
+
+class _DeviceBytes:
+    """A device byte range as torch.as_tensor takes it (__cuda_array_interface__), without a copy."""
+
+    def __init__(self, ptr, nbytes):
+        self.__cuda_array_interface__ = {"shape": (int(nbytes),), "typestr": "|u1", "data": (int(ptr), False),
+                                         "version": 3}
+
+
 class Pipeline(_Handle):
     """One CPI through the body of the reference's process thread (src/blah2.cpp:268-287):
     [WienerHopf] -> Ambiguity -> Map::set_metrics -> [CfarDetector1D -> Centroid -> Interpolate],
@@ -886,6 +902,8 @@ class Pipeline(_Handle):
         self.timing_json_max_bytes, self.timing_stash_max_bytes = int(db.value), int(sb.value)
         self._tmjson = np.empty(self.timing_json_max_bytes, dtype=np.uint8)
         self._tmstash = np.empty(self.timing_stash_max_bytes, dtype=np.uint8)
+        if getattr(self, "export_max_detections", 0):  # the record now carries the stamps
+            self.enable_export(self.export_max_detections)
 
     def fetch_timing_json(self, timestamp) -> bytes:
         """The timing document of the last fetched CPI with tNow = ``timestamp`` (call after fetch() and, with the
@@ -921,6 +939,31 @@ class Pipeline(_Handle):
         pipes = list(pipes)
         arr = (C.c_void_p * max(len(pipes), 1))(*[p._h for p in pipes])
         capi.check(capi.load().b200dd_pipeline_share_history(arr, len(pipes)))
+
+    def enable_export(self, max_detections=4096) -> int:
+        """Every CPI submitted from now on also packs its record: everything the fetches read besides the map, in
+        one fixed-size device buffer (b200dd_pipeline_enable_export).  Detections past ``max_detections`` (1 .. 2^18)
+        do not travel: such a CPI imports as a CFAR overflow.  Returns the record's size in bytes, kept as
+        ``record_bytes`` (enable_timing_json afterwards packs the stamps too and updates it)."""
+        nb = C.c_size_t()
+        capi.check(self._lib.b200dd_pipeline_enable_export(self._h, int(max_detections), C.byref(nb)))
+        self.export_max_detections, self.record_bytes = int(max_detections), int(nb.value)
+        return self.record_bytes
+
+    def export_record(self):
+        """The last submit's record as a uint8 CUDA tensor of ``record_bytes`` that views the pipeline's buffer: valid
+        until the next submit, written on that submit's stream."""
+        import torch
+        p = C.c_void_p()
+        capi.check(self._lib.b200dd_pipeline_export_record(self._h, C.byref(p)))
+        return torch.as_tensor(_DeviceBytes(int(p.value), self.record_bytes))
+
+    def submit_record(self, d_record, d_map):
+        """Takes the CPI another pipeline of the same parameters and spectrum / timing stages exported: its record
+        and its complex64 map (device buffers, complete when this is called).  Then fetch() and every fetch_* behave
+        as after a submit; d_map must stay untouched until fetch().  Raises B200ddError (ERR_ARG) for a record of
+        other parameters or stages."""
+        capi.check(self._lib.b200dd_pipeline_submit_record(self._h, capi.ptr(d_record), capi.ptr(d_map)))
 
     def fetch_spectrum(self):
         """Spectrum of the reference channel of the last submitted CPI (complex128, nSpectrum bins)."""

@@ -124,6 +124,52 @@ def gather_maps(local_maps: torch.Tensor, n_cpis: int, rank: int, world: int, ds
     return out
 
 
+class IndependentCpiPlan:
+    """Independent CPIs over the ranks with every product on rank ``dst`` (BASELINE config 4).
+
+    Rank r computes the CPIs c = r, r + world, ... (cpi_indices); each CPI's record (Pipeline.export_record) and map
+    travel to ``dst`` in one round of two gathers per ``world`` CPIs (``comm.gather_async``), and ``dst`` hands them to
+    ``consume`` in CPI order, c = 0, 1, 2, ..., which submits them to its importing pipeline(s)
+    (Pipeline.submit_record) and fetches.  ``comm`` is a Comm on GPUs, a TorchComm in the CPU tests.
+
+    Receive buffers form a ring of ``depth`` rounds: a round's buffers are gathered into again ``depth`` rounds later,
+    so by then every CPI consumed from them must have been fetched (fetch() ends a CPI's reads of its map).  Importers
+    that keep CPIs unfetched across rounds (a share set) need a deeper ring."""
+
+    def __init__(self, comm, record_bytes: int, map_shape, device, depth: int = 1, dst: int = 0):
+        self.comm, self.dst, self.depth = comm, dst, int(depth)
+        shape = tuple(map_shape)
+        # what a rank without a CPI in the last round sends: the gathers are collective
+        self.pad_record = torch.zeros(int(record_bytes), dtype=torch.uint8, device=device)
+        self.pad_map = torch.zeros(shape, dtype=torch.complex64, device=device)
+        self.recv_record = self.recv_map = None
+        if comm.rank == dst:
+            self.recv_record = torch.empty((self.depth, comm.world, int(record_bytes)), dtype=torch.uint8, device=device)
+            self.recv_map = torch.empty((self.depth, comm.world) + shape, dtype=torch.complex64, device=device)
+
+    def run(self, n_cpis: int, compute, consume, after=None):
+        """CPIs 0 .. n_cpis - 1.  On every rank, ``compute(c)`` enqueues CPI c on the stream ``after`` (None: the
+        caller's ordering is synchronous) and returns its (record, map) tensors; the next round's compute is enqueued
+        after this round's gathers have read them.  On ``dst``, ``consume(c, record, map)`` gets every CPI in order,
+        its buffers complete."""
+        comm, rank, world, dst = self.comm, self.comm.rank, self.comm.world, self.dst
+        for k in range((n_cpis + world - 1) // world):
+            # the last round's gathers have read what compute overwrites
+            comm.join(after) if after is not None else comm.sync()
+            c = k * world + rank
+            record, m = compute(c) if c < n_cpis else (self.pad_record, self.pad_map)
+            s = k % self.depth
+            root = rank == dst
+            comm.gather_async(record, self.recv_record[s] if root else None, dst, after=after)
+            comm.gather_async(m, self.recv_map[s] if root else None, dst, after=None)
+            if not root:
+                continue
+            comm.sync()                             # submit_record reads each record's header on the host
+            for r in range(world):
+                if k * world + r < n_cpis:
+                    consume(k * world + r, self.recv_record[s, r], self.recv_map[s, r])
+
+
 # ------------------------------------------------------------------------------------------
 # ONE large CPI split over the ranks (BASELINE config 5)
 # ------------------------------------------------------------------------------------------
@@ -208,6 +254,13 @@ class TorchComm:
     @staticmethod
     def _bytes(t):
         return torch.view_as_real(t).reshape(-1) if t.is_complex() else t.reshape(-1)
+
+    def gather_async(self, send, recv, dst=0, after=None):
+        got = [torch.empty_like(self._bytes(send)) for _ in range(self.world)] if self.rank == dst else None
+        dist.gather(self._bytes(send).contiguous(), got, dst=dst)
+        if self.rank == dst:
+            for r in range(self.world):
+                self._bytes(recv[r]).copy_(got[r])
 
     def gatherv_async(self, send, recv, sizes, offsets, dst=0, after=None):
         es = send.element_size()

@@ -871,6 +871,47 @@ B200DD_API int b200dd_pipeline_debug_timing_values(b200dd_pipeline *h, const cha
  * history; its stamps stay per member, and its documents follow the same commit rule as the histories. */
 B200DD_API int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n);
 
+/* CPI records: independent CPIs over GPUs with every product on one rank.  A pipeline that computes a CPI exports
+ * it as one fixed-size device record holding everything its fetches read besides the map: the clutter-filter status,
+ * set_metrics' noisePower and maxPower, CFAR's count, the detection list, the spectrum (spectrum stage) and the
+ * timing stamps (timing stage).  Another pipeline, created with the same parameters and spectrum / timing stages,
+ * on any GPU, takes the record and the map as if it had run the CPI itself: every fetch, stash, the tracker and the
+ * share-set rules apply unchanged.  The record's layout is private to the library; only its size is public.
+ *
+ * enable_export: from now on every submit (submit_device eager or graph-replayed, submit_host, _rspduo, _ci8,
+ * _cf32, and prepare_device's runs) ends its chain with one pack kernel that writes the CPI's record into a device
+ * buffer the pipeline owns.  max_detections (1 .. 2^18) detection slots of 24 bytes each bound the record:
+ * *record_bytes (nullable) = 64 + 80 with the timing stage + 16 nSpectrum with the spectrum stage + 24
+ * max_detections with detection, rounded up to 16.  A CPI with more detections than slots carries the first
+ * max_detections and is marked as overflowed.  Enabling the spectrum or timing stage later changes the layout;
+ * *record_bytes is then b200dd_pipeline_export_record's buffer size from the next submit on.  Recorded graphs are
+ * dropped (prepare_device records them again).  Without this call nothing is enqueued: every submit runs the
+ * kernels it ran before.  B200DD_ERR_ARG: max_detections out of range, null handle.
+ *
+ * export_record: *d_record = the device record of the last submit.  It stays valid until the next submit on this
+ * pipeline and is written on the stream that submit ran on (b200dd_pipeline_stream for the host submits).
+ * B200DD_ERR_ARG when export is not enabled or nothing was submitted since.
+ *
+ * submit_record: the importing pipeline takes the CPI of record d_record and float2 map d_map (nDoppler x nDelay,
+ * the exporter's map bytes): on b200dd_pipeline_stream(h) it writes the record into its own detection list,
+ * metrics and status words, spectrum and stamps, then runs the renders a submit runs after the map -- the map
+ * document body on d_map, the IQ-data and detection documents, and the max-hold push (at fetch for a share-set
+ * member).  Both buffers must be complete, or ordered before that stream's work, at the call: it reads the record's
+ * header synchronously.  d_map must stay untouched until b200dd_pipeline_fetch, as a share-set member's map does.
+ * Afterwards b200dd_pipeline_fetch, fetch_spectrum and every fetch_*_json / fetch_*_stash behave as after a submit:
+ *  - a failed clutter-filter solve imports as B200DD_FILTER_FAILED: nothing is committed, nCpi does not step;
+ *  - a CFAR overflow imports as that overflow;
+ *  - a record overflow behaves as a CFAR overflow: fetch and fetch_detection_json return B200DD_ERR_CAPACITY,
+ *    nothing enters the detection history and the tracker skips the CPI;
+ *  - the timing document's stage times come from the exporter's stamps (differences between stamps of one GPU);
+ *    `tracker` is measured here, at the track fetch.
+ * Importers may be share-set members (the set's rules apply, the import counts as a submit).  B200DD_ERR_ARG,
+ * nothing enqueued: a null argument, not a record of this version, a record from a pipeline whose parameters or
+ * spectrum / timing stages differ, a share-set member whose last CPI is not fetched. */
+B200DD_API int b200dd_pipeline_enable_export(b200dd_pipeline *h, uint32_t max_detections, size_t *record_bytes);
+B200DD_API int b200dd_pipeline_export_record(b200dd_pipeline *h, const void **d_record);
+B200DD_API int b200dd_pipeline_submit_record(b200dd_pipeline *h, const void *d_record, const void *d_map);
+
 /* ------------------------------------------------------------------------------------------------
  * Inter-GPU exchanges (one process per GPU, NCCL over NVLink / NVSwitch).  The reference has no
  * distributed code; these serve the two shardings of SURVEY.md s8(e): independent CPIs round-robin
