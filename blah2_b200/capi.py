@@ -21,6 +21,10 @@ ERR_CUDA = 3
 ERR_CAPACITY = 4
 ERR_NONFINITE = 5
 FILTER_FAILED = 10
+# b200dd_pipeline_stamp's boundaries
+STAMP_CHAIN = 0
+STAMP_SPECTRUM = 1
+STAMP_CLUTTER = 2
 
 DET_CFAR = 1
 DET_CENTROID = 2
@@ -142,6 +146,8 @@ SIGNATURES = [
     ("b200dd_spectrum_process_host", C.c_int, [_VP, _VP, C.c_uint32, _VP]),
     ("b200dd_spectrum_process_device", C.c_int, [_VP, _VP, C.c_uint32, _VP, _VP]),
     ("b200dd_spectrum_process_device_f64", C.c_int, [_VP, _VP, C.c_uint32, _VP, _VP]),
+    ("b200dd_spectrum_fold_slice_device", C.c_int, [_VP, _VP, C.c_uint32, C.c_uint32, _VP, _VP]),
+    ("b200dd_spectrum_finish_device", C.c_int, [_VP, _VP, C.c_uint32, _VP, _VP]),
     ("b200dd_spectrum_fetch", C.c_int, [_VP, _VP, _VP]),
     ("b200dd_spectrum_profile_device", C.c_int, [_VP, _VP, C.c_uint32, _VP, C.POINTER(C.c_float),
                                                  C.POINTER(C.c_float)]),
@@ -189,6 +195,8 @@ SIGNATURES = [
     ("b200dd_pipeline_enable_export", C.c_int, [_VP, C.c_uint32, C.POINTER(C.c_size_t)]),
     ("b200dd_pipeline_export_record", C.c_int, [_VP, C.POINTER(_VP)]),
     ("b200dd_pipeline_submit_record", C.c_int, [_VP, _VP, _VP]),
+    ("b200dd_pipeline_submit_map", C.c_int, [_VP, _VP, _VP, _VP, C.c_uint32, _VP]),
+    ("b200dd_pipeline_stamp", C.c_int, [_VP, C.c_int, _VP]),
     ("b200dd_mapjson_create", C.c_int, [C.c_uint32, C.c_uint32, _VP, _VP, C.c_uint32, C.c_int32, C.POINTER(_VP)]),
     ("b200dd_mapjson_max_bytes", C.c_size_t, [_VP]),
     ("b200dd_mapjson_destroy", None, [_VP]),

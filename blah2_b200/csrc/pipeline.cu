@@ -287,6 +287,7 @@ struct b200dd_pipeline {
   DevBuf<uint64_t> d_tm;            // the last submit's stamps, TmSlot
   std::vector<const char *> tm_names;  // behind the last document written
   std::vector<double> tm_values;
+  unsigned tm_pre = 0;              // b200dd_pipeline_stamp: the boundaries stamped since the last submit, 1 << slot
   uint32_t spec_bins = 0, spec_nfft = 0;
   b200dd_caf_geometry g;
   std::vector<int32_t> delay;
@@ -578,19 +579,24 @@ static int pipeline_enqueue_after_spectrum(b200dd_pipeline *h, void *st) {
   return tm_stamp(h, kTmSpectrum, st);
 }
 
-// the CAF of x and y into `map`, set_metrics and the detection stages, then the products after them and, with export
-// on, the record of a submit that came in by `path` (TmPath), on `st`
-static int pipeline_enqueue_tail(b200dd_pipeline *h, const void *x, const void *y, uint32_t n, float2 *map, int path,
-                                 void *st) {
-  int rc = b200dd_caf_process_device(h->caf, x, y, n, map, st);
-  if (rc != B200DD_OK) return rc;
+// set_metrics and the detection stages on the CPI's `map`, then the products after them, on `st`
+static int pipeline_enqueue_after_map(b200dd_pipeline *h, float2 *map, void *st) {
   // Map::set_metrics runs after every Ambiguity::process, detection or not (blah2.cpp:278-279): stage 0 = metrics only
   const int last = h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0;
-  rc = b200dd_det_chain_device_async(h->det, last, map, h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(),
-                                     h->doppler.data(), st);
+  int rc = b200dd_det_chain_device_async(h->det, last, map, h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(),
+                                         h->doppler.data(), st);
   if (rc == B200DD_OK && h->p.detection_enable) rc = tm_stamp(h, kTmDetector, st);
   if (rc == B200DD_OK) rc = pipeline_enqueue_products(h, map, st);
   if (rc == B200DD_OK) rc = tm_stamp(h, kTmOutput, st);
+  return rc;
+}
+
+// the CAF of x and y into `map`, everything after it and, with export on, the record of a submit that came in by
+// `path` (TmPath), on `st`
+static int pipeline_enqueue_tail(b200dd_pipeline *h, const void *x, const void *y, uint32_t n, float2 *map, int path,
+                                 void *st) {
+  int rc = b200dd_caf_process_device(h->caf, x, y, n, map, st);
+  if (rc == B200DD_OK) rc = pipeline_enqueue_after_map(h, map, st);
   if (rc == B200DD_OK) rc = export_pack(h, path, st);
   return rc;
 }
@@ -638,6 +644,7 @@ static void pipeline_submitted(b200dd_pipeline *h, int path, void *st, const voi
   if (h->dj) detjson_mark_rendered(h->dj, true);
   if (h->ij) iqjson_mark_rendered(h->ij, true);
   h->exp_valid = h->exp_max != 0;
+  h->tm_pre = 0;
 }
 
 static const b200dd_pipeline::GraphEntry *pipeline_find_graph(const b200dd_pipeline *h, const void *d_x, const void *d_y,
@@ -1400,6 +1407,46 @@ int b200dd_pipeline_submit_record(b200dd_pipeline *h, const void *d_record, cons
   if (rc != B200DD_OK) return rc;
   pipeline_submitted(h, (int)hd.path, st, d_map);
   h->exp_valid = false;  // the import packed nothing
+  return B200DD_OK;
+}
+
+int b200dd_pipeline_stamp(b200dd_pipeline *h, int slot, void *stream) {
+  if (!h) return arg_fail("b200dd_pipeline_stamp: null handle");
+  static const int slots[] = {kTmChain, kTmSpectrum, kTmClutter};  // B200DD_STAMP_CHAIN, _SPECTRUM, _CLUTTER
+  if (slot < B200DD_STAMP_CHAIN || slot > B200DD_STAMP_CLUTTER) return arg_fail("b200dd_pipeline_stamp: not a boundary slot");
+  if (!h->tm_on) return B200DD_OK;
+  DeviceGuard guard(h->device);
+  const int rc = tm_stamp(h, slots[slot], stream ? stream : (void *)h->stream);
+  if (rc == B200DD_OK) h->tm_pre |= 1u << slot;
+  return rc;
+}
+
+int b200dd_pipeline_submit_map(b200dd_pipeline *h, const void *d_map, const int *d_filter_status,
+                               const void *d_spectrum_parts, uint32_t n_parts, void *stream) {
+  if (!h || !d_map) return arg_fail("b200dd_pipeline_submit_map: null argument");
+  if (!h->wh != !d_filter_status)
+    return arg_fail("b200dd_pipeline_submit_map: a clutter-filter status is required iff the clutter filter is enabled");
+  if (h->spec ? (!d_spectrum_parts || n_parts == 0) : (d_spectrum_parts || n_parts))
+    return arg_fail("b200dd_pipeline_submit_map: spectrum parts are required iff the spectrum stage is enabled");
+  int rc = member_may_submit(h, "b200dd_pipeline_submit_map: the share-set member's last CPI is not fetched yet");
+  if (rc != B200DD_OK) return rc;
+  DeviceGuard guard(h->device);
+  void *st = stream ? stream : (void *)h->stream;
+  static const int slots[] = {kTmChain, kTmSpectrum, kTmClutter};
+  for (int i = 0; i < 3 && rc == B200DD_OK; i++)
+    if (!(h->tm_pre & (1u << i))) rc = tm_stamp(h, slots[i], st);
+  if (rc == B200DD_OK && h->spec) {
+    rc = b200dd_spectrum_finish_device(h->spec, d_spectrum_parts, n_parts, nullptr, st);
+    if (rc == B200DD_OK && h->ij) rc = b200dd_iqjson_render_device(h->ij, spectrum_device_output(h->spec), st);
+  }
+  if (rc != B200DD_OK) return rc;
+  if (h->wh)
+    B2_CUDA(cudaMemcpyAsync(const_cast<int *>(b200dd_wh_device_status(h->wh)), d_filter_status, sizeof(int),
+                            cudaMemcpyDeviceToDevice, (cudaStream_t)st));
+  rc = pipeline_enqueue_after_map(h, (float2 *)const_cast<void *>(d_map), st);
+  if (rc != B200DD_OK) return rc;
+  pipeline_submitted(h, kTmDevice, st, d_map);
+  h->exp_valid = false;  // nothing was packed
   return B200DD_OK;
 }
 

@@ -18,8 +18,14 @@
 //   K_S1  spec_fold_kernel<TIN> / spec_fold2_kernel   x (float2 / double2) -> per-chunk column sums  part[chunk][r]
 //   K_S2  spec_reduce_kernel      g[r] = t2[r] * sum_chunk part[chunk][r]        (fixed order: deterministic)
 //   K_S3  spec_dft_kernel         spectrum[m] = sum_r g[r] W^(r m)               (direct; phases = table seeds + running product)
+//
+// The fold is a sum over samples, so it also runs on a SLICE [sample0, end) of the CPI held by one GPU
+// (b200dd_spectrum_fold_slice_device): K_S1 over the slice's rows, then K_S2 without the t2 phase sums its chunks into
+// one part of nSpectrum column sums.  b200dd_spectrum_finish_device is K_S2 with t2 over the parts of all slices, then
+// K_S3.  A slice's interior is whole rows of its local buffer; only its first and last rows are masked.
 #include "common.cuh"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <new>
@@ -48,21 +54,48 @@ __device__ __forceinline__ void zfma(double2 &acc, double2 v, double2 w) {
   acc.y = fma(v.y, w.x, acc.y);
 }
 
+// The samples a fold reads: global sample g = q nSpec + r of the CPI (q < dec, r < nSpec) is x[g - sample0] for
+// sample0 <= g < end.  The kernels walk BANDS of nSpec samples, band q = [q nSpec + shift, (q + 1) nSpec + shift):
+// rows of the CPI, shifted by one sample when the two-column kernel pairs columns (2j + 1, 2j + 2) (odd sample0).
+// Bands [qa, qb) hold samples of the slice; bands [fa, fb) hold nothing else, so their loads need no mask.  Chunk
+// c of the launch covers bands [qa + c rows, qa + (c + 1) rows).  A whole CPI (sample0 = 0, end = nfft) is
+// qa = fa = 0, qb = fb = dec: no band is masked.
+struct FoldSpan {
+  uint32_t sample0;
+  uint64_t end;
+  uint32_t qa, qb, fa, fb;
+  uint32_t rowsPerChunk;
+};
+
+// chunk bands [q0, q1) split into masked [q0, lo), whole [lo, hi), masked [hi, q1): ascending, each band once
+__device__ __forceinline__ void fold_bands(const FoldSpan &sp, uint32_t &q0, uint32_t &q1, uint32_t &lo, uint32_t &hi) {
+  q0 = sp.qa + blockIdx.y * sp.rowsPerChunk;
+  q1 = min(sp.qb, q0 + sp.rowsPerChunk);
+  lo = min(max(sp.fa, q0), q1);
+  hi = max(lo, min(sp.fb, q1));
+}
+
 // K_S1.  grid (ceil(nSpec / 128), nChunks); thread = one column r, rows q in [q0, q1) of this chunk.  A warp's load
 // of one row is 32 consecutive samples (256 B / 512 B, whole sectors); FOLD_UNROLL independent rows are in flight
 // per thread.  The row phase t1[q] is warp-uniform (one broadcast load).  Sum order: q ascending.
 template <class TIN>
 __global__ void __launch_bounds__(FOLD_THREADS) spec_fold_kernel(const TIN *__restrict__ x, const double2 *__restrict__ t1,
-                                                                 double2 *__restrict__ part, uint32_t nSpec, uint32_t dec,
-                                                                 uint32_t rowsPerChunk) {
+                                                                 double2 *__restrict__ part, uint32_t nSpec, FoldSpan sp) {
   const uint32_t r = blockIdx.x * FOLD_THREADS + threadIdx.x;
   if (r >= nSpec) return;
-  const uint32_t q0 = blockIdx.y * rowsPerChunk;
-  const uint32_t q1 = min(dec, q0 + rowsPerChunk);
+  uint32_t q0, q1, lo, hi;
+  fold_bands(sp, q0, q1, lo, hi);
   double2 acc = make_double2(0.0, 0.0);
-  const TIN *p = x + (size_t)q0 * nSpec + r;
-  uint32_t q = q0;
-  for (; q + FOLD_UNROLL <= q1; q += FOLD_UNROLL) {
+  auto masked = [&](uint32_t a, uint32_t b) {  // the slice's partial first / last row
+    for (uint32_t q = a; q < b; q++) {
+      const uint64_t g = (uint64_t)q * nSpec + r;
+      if (g >= sp.sample0 && g < sp.end) zfma(acc, widen(__ldg(x + (g - sp.sample0))), __ldg(t1 + q));
+    }
+  };
+  masked(q0, lo);
+  const TIN *p = x + ((uint64_t)lo * nSpec + r - sp.sample0);
+  uint32_t q = lo;
+  for (; q + FOLD_UNROLL <= hi; q += FOLD_UNROLL) {
     TIN v[FOLD_UNROLL];
 #pragma unroll
     for (int u = 0; u < FOLD_UNROLL; u++) v[u] = __ldg(p + (size_t)u * nSpec);
@@ -70,15 +103,16 @@ __global__ void __launch_bounds__(FOLD_THREADS) spec_fold_kernel(const TIN *__re
     for (int u = 0; u < FOLD_UNROLL; u++) zfma(acc, widen(v[u]), __ldg(t1 + q + u));
     p += (size_t)FOLD_UNROLL * nSpec;
   }
-  if (q < q1) {  // tail rows: still issued together
+  if (q < hi) {  // tail rows: still issued together
     TIN v[FOLD_UNROLL];
 #pragma unroll
     for (int u = 0; u < FOLD_UNROLL; u++)
-      if (q + u < q1) v[u] = __ldg(p + (size_t)u * nSpec);
+      if (q + u < hi) v[u] = __ldg(p + (size_t)u * nSpec);
 #pragma unroll
     for (int u = 0; u < FOLD_UNROLL; u++)
-      if (q + u < q1) zfma(acc, widen(v[u]), __ldg(t1 + q + u));
+      if (q + u < hi) zfma(acc, widen(v[u]), __ldg(t1 + q + u));
   }
+  masked(hi, q1);
   part[(size_t)blockIdx.y * nSpec + r] = acc;
 }
 
@@ -86,19 +120,39 @@ __global__ void __launch_bounds__(FOLD_THREADS) spec_fold_kernel(const TIN *__re
 // load is 512 contiguous bytes and FOLD_UNROLL x 16 bytes are in flight per thread -- what it takes to keep HBM busy
 // with 8 CTAs of 4 warps per SM (the 8-byte version stops at 60 % of the DRAM peak).
 // Same sums in the same order as the scalar kernel: results are bit-identical.
-template <int U, int MINB>
+// ODD (odd sample0): thread j pairs columns c = 2j + 1 and c + 1, so that its loads stay 16-byte aligned in the
+// local buffer; the last thread's second column is column 0 of the next row (phase t1[q + 1]).
+template <int U, int MINB, bool ODD>
 __global__ void __launch_bounds__(FOLD_THREADS, MINB) spec_fold2_kernel(const float2 *__restrict__ x, const double2 *__restrict__ t1,
-                                                                     double2 *__restrict__ part, uint32_t nSpec, uint32_t dec,
-                                                                     uint32_t rowsPerChunk) {
-  const uint32_t r = 2u * (blockIdx.x * FOLD_THREADS + threadIdx.x);
-  if (r >= nSpec) return;  // nSpec is even: r + 1 < nSpec as well
-  const uint32_t q0 = blockIdx.y * rowsPerChunk;
-  const uint32_t q1 = min(dec, q0 + rowsPerChunk);
+                                                                     double2 *__restrict__ part, uint32_t nSpec, FoldSpan sp) {
+  const uint32_t c = 2u * (blockIdx.x * FOLD_THREADS + threadIdx.x) + (ODD ? 1u : 0u);
+  if (c >= nSpec) return;  // nSpec is even: c + 1 <= nSpec
+  const bool wrap = ODD && c + 1 == nSpec;
+  uint32_t q0, q1, lo, hi;
+  fold_bands(sp, q0, q1, lo, hi);
   double2 acc0 = make_double2(0.0, 0.0), acc1 = make_double2(0.0, 0.0);
-  const float4 *p = reinterpret_cast<const float4 *>(x + (size_t)q0 * nSpec + r);
+  auto masked = [&](uint32_t a, uint32_t b) {  // the slice's partial first / last band
+    for (uint32_t q = a; q < b; q++) {
+      const uint64_t g = (uint64_t)q * nSpec + c;
+      const bool in0 = g >= sp.sample0 && g < sp.end, in1 = g + 1 >= sp.sample0 && g + 1 < sp.end;
+      if (!in0 && !in1) continue;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (in0 && in1) {
+        v = __ldg(reinterpret_cast<const float4 *>(x + (g - sp.sample0)));
+      } else {
+        const float2 e = __ldg(x + (g + (in0 ? 0 : 1) - sp.sample0));
+        if (in0) v.x = e.x, v.y = e.y;
+        else v.z = e.x, v.w = e.y;
+      }
+      if (in0) zfma(acc0, make_double2((double)v.x, (double)v.y), __ldg(t1 + q));
+      if (in1) zfma(acc1, make_double2((double)v.z, (double)v.w), __ldg(t1 + q + (wrap ? 1 : 0)));
+    }
+  };
+  masked(q0, lo);
+  const float4 *p = reinterpret_cast<const float4 *>(x + ((uint64_t)lo * nSpec + c - sp.sample0));
   const size_t rowStride = nSpec / 2;  // in float4
-  uint32_t q = q0;
-  for (; q + U <= q1; q += U) {
+  uint32_t q = lo;
+  for (; q + U <= hi; q += U) {
     float4 v[U];
 #pragma unroll
     for (int u = 0; u < U; u++) v[u] = __ldg(p + (size_t)u * rowStride);
@@ -106,31 +160,32 @@ __global__ void __launch_bounds__(FOLD_THREADS, MINB) spec_fold2_kernel(const fl
     for (int u = 0; u < U; u++) {
       const double2 w = __ldg(t1 + q + u);
       zfma(acc0, make_double2((double)v[u].x, (double)v[u].y), w);
-      zfma(acc1, make_double2((double)v[u].z, (double)v[u].w), w);
+      zfma(acc1, make_double2((double)v[u].z, (double)v[u].w), wrap ? __ldg(t1 + q + u + 1) : w);
     }
     p += (size_t)U * rowStride;
   }
-  if (q < q1) {
+  if (q < hi) {
     float4 v[U];
 #pragma unroll
     for (int u = 0; u < U; u++)
-      if (q + u < q1) v[u] = __ldg(p + (size_t)u * rowStride);
+      if (q + u < hi) v[u] = __ldg(p + (size_t)u * rowStride);
 #pragma unroll
     for (int u = 0; u < U; u++)
-      if (q + u < q1) {
+      if (q + u < hi) {
         const double2 w = __ldg(t1 + q + u);
         zfma(acc0, make_double2((double)v[u].x, (double)v[u].y), w);
-        zfma(acc1, make_double2((double)v[u].z, (double)v[u].w), w);
+        zfma(acc1, make_double2((double)v[u].z, (double)v[u].w), wrap ? __ldg(t1 + q + u + 1) : w);
       }
   }
-  double2 *dst = part + (size_t)blockIdx.y * nSpec + r;
-  dst[0] = acc0;
-  dst[1] = acc1;
+  masked(hi, q1);
+  double2 *dst = part + (size_t)blockIdx.y * nSpec;
+  dst[c] = acc0;
+  dst[wrap ? 0 : c + 1] = acc1;
 }
 
 // K_S2.  CTA = 32 columns x RED_WARPS warps; warp w adds chunks w, w + 32, ... (ascending), the 32 sums are then
 // added in warp order: a fixed tree, so the result does not depend on scheduling.  (Many warps, few loads each:
-// the kernel is one or two L2 round trips long.)
+// the kernel is one or two L2 round trips long.)  t2 == nullptr: the sums without the phase (a slice's part).
 __global__ void __launch_bounds__(32 * RED_WARPS) spec_reduce_kernel(const double2 *__restrict__ part, const double2 *__restrict__ t2,
                                                                      double2 *__restrict__ g, uint32_t nSpec, uint32_t nChunks) {
   __shared__ double2 s[RED_WARPS][32];
@@ -138,7 +193,7 @@ __global__ void __launch_bounds__(32 * RED_WARPS) spec_reduce_kernel(const doubl
   const uint32_t r = blockIdx.x * 32 + lane;
   double2 acc = make_double2(0.0, 0.0);
   double2 ph = make_double2(1.0, 0.0);
-  if (w == 0 && r < nSpec) ph = __ldg(t2 + r);  // issued with the partial sums: one memory round trip, not two
+  if (w == 0 && r < nSpec && t2) ph = __ldg(t2 + r);  // issued with the partial sums: one memory round trip, not two
   if (r < nSpec) {
     uint32_t c = w;
     for (; c + 3 * RED_WARPS < nChunks; c += 4 * RED_WARPS) {
@@ -162,7 +217,7 @@ __global__ void __launch_bounds__(32 * RED_WARPS) spec_reduce_kernel(const doubl
     double2 t = s[0][lane];
 #pragma unroll
     for (int k = 1; k < RED_WARPS; k++) { t.x += s[k][lane].x; t.y += s[k][lane].y; }
-    g[r] = make_double2(t.x * ph.x - t.y * ph.y, t.x * ph.y + t.y * ph.x);
+    g[r] = t2 ? make_double2(t.x * ph.x - t.y * ph.y, t.x * ph.y + t.y * ph.x) : t;
   }
 }
 
@@ -247,8 +302,8 @@ struct b200dd_spectrum {
   Stream stream;
   uint32_t n = 0, decimation = 0, nSpectrum = 0, nfft = 0;
   double bandwidth = 0.0;
-  uint32_t rowsPerChunk = 0, nChunks = 0;    // 8-byte-load fold (any nSpectrum / alignment, double2 input)
-  uint32_t rowsPerChunk2 = 0, nChunks2 = 0;  // two-columns-per-thread fold
+  uint32_t wantChunks = 0, rowsPerChunk = 0, nChunks = 0;     // 8-byte-load fold (any nSpectrum / alignment, double2 input)
+  uint32_t wantChunks2 = 0, rowsPerChunk2 = 0, nChunks2 = 0;  // two-columns-per-thread fold
   DevBuf<double2> d_t1, d_t2, d_w, d_part, d_g, d_out;
   DevBuf<double2> d_xd;  // host-path staging
   Event ev[3];
@@ -257,25 +312,55 @@ struct b200dd_spectrum {
 
 namespace {
 
-template <class TIN> int run_spectrum(b200dd_spectrum *h, const TIN *d_x, double2 *d_out, cudaStream_t st, bool timed) {
-  if (timed) B2_CUDA(cudaEventRecord(h->ev[0], st));
+// nRows rows in chunks of at least FOLD_UNROLL rows, at most `want` chunks
+void fold_chunking(uint32_t nRows, uint32_t want, uint32_t *rows, uint32_t *chunks) {
+  uint32_t r = (nRows + want - 1) / want;
+  if (r < (uint32_t)FOLD_UNROLL) r = FOLD_UNROLL;
+  *rows = r;
+  *chunks = (nRows + r - 1) / r;
+}
+
+// K_S1 over the samples [sample0, end) at x (x[0] = global sample sample0; end <= nfft, end > sample0) into per-chunk
+// column sums at h->d_part; *chunks = their number.  For sample0 = 0, end = nfft: the CPI's fold.
+template <class TIN>
+int fold_chunks(b200dd_spectrum *h, const TIN *x, uint32_t sample0, uint64_t end, cudaStream_t st, uint32_t *chunks) {
   bool vec2 = false;
   if constexpr (std::is_same<TIN, float2>::value)
-    vec2 = h->nSpectrum % 2 == 0 && (reinterpret_cast<uintptr_t>(d_x) & 15) == 0;
+    vec2 = h->nSpectrum % 2 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  const uint64_t ns = h->nSpectrum, shift = vec2 ? (sample0 & 1u) : 0u;
+  FoldSpan sp;
+  sp.sample0 = sample0;
+  sp.end = end;
+  sp.qa = (uint32_t)((sample0 - shift) / ns);
+  sp.qb = (uint32_t)((end - shift + ns - 1) / ns);
+  sp.fa = (uint32_t)((sample0 - shift + ns - 1) / ns);
+  sp.fb = (uint32_t)((end - shift) / ns);
+  fold_chunking(sp.qb - sp.qa, vec2 ? h->wantChunks2 : h->wantChunks, &sp.rowsPerChunk, chunks);
   if (vec2) {
-    const dim3 gridF((h->nSpectrum / 2 + FOLD_THREADS - 1) / FOLD_THREADS, h->nChunks2);
+    const dim3 gridF((h->nSpectrum / 2 + FOLD_THREADS - 1) / FOLD_THREADS, *chunks);
     // 8 rows in flight per thread, 6 CTAs per SM (faster than 16 x 4 and 4 x 10 rows x CTAs at 2e7)
-    spec_fold2_kernel<FOLD_UNROLL, 6><<<gridF, FOLD_THREADS, 0, st>>>((const float2 *)d_x, h->d_t1, h->d_part, h->nSpectrum,
-                                                                      h->decimation, h->rowsPerChunk2);
+    if (shift)
+      spec_fold2_kernel<FOLD_UNROLL, 6, true><<<gridF, FOLD_THREADS, 0, st>>>((const float2 *)x, h->d_t1, h->d_part, h->nSpectrum, sp);
+    else
+      spec_fold2_kernel<FOLD_UNROLL, 6, false><<<gridF, FOLD_THREADS, 0, st>>>((const float2 *)x, h->d_t1, h->d_part, h->nSpectrum, sp);
   } else {
-    const dim3 gridF((h->nSpectrum + FOLD_THREADS - 1) / FOLD_THREADS, h->nChunks);
-    spec_fold_kernel<TIN><<<gridF, FOLD_THREADS, 0, st>>>(d_x, h->d_t1, h->d_part, h->nSpectrum, h->decimation, h->rowsPerChunk);
+    const dim3 gridF((h->nSpectrum + FOLD_THREADS - 1) / FOLD_THREADS, *chunks);
+    spec_fold_kernel<TIN><<<gridF, FOLD_THREADS, 0, st>>>(x, h->d_t1, h->d_part, h->nSpectrum, sp);
   }
   B2_LAUNCH_CHECK();
-  const uint32_t nChunks = vec2 ? h->nChunks2 : h->nChunks;
-  if (timed) B2_CUDA(cudaEventRecord(h->ev[1], st));
-  spec_reduce_kernel<<<(h->nSpectrum + 31) / 32, 32 * RED_WARPS, 0, st>>>(h->d_part, h->d_t2, h->d_g, h->nSpectrum, nChunks);
+  return B200DD_OK;
+}
+
+// K_S2 over n_parts parts of column sums (t2 nullptr: without the phase, into a slice's part) into `g`
+int reduce_parts(b200dd_spectrum *h, const double2 *parts, uint32_t n_parts, const double2 *t2, double2 *g, cudaStream_t st) {
+  spec_reduce_kernel<<<(h->nSpectrum + 31) / 32, 32 * RED_WARPS, 0, st>>>(parts, t2, g, h->nSpectrum, n_parts);
   B2_LAUNCH_CHECK();
+  return B200DD_OK;
+}
+
+// K_S2 with t2 over the parts, then K_S3 into d_out
+int finish(b200dd_spectrum *h, const double2 *parts, uint32_t n_parts, double2 *d_out, cudaStream_t st) {
+  if (int rc = reduce_parts(h, parts, n_parts, h->d_t2, h->d_g, st)) return rc;
   const int gridD = (int)((h->nSpectrum + DFT_OUT - 1) / DFT_OUT);
   if (h->nSpectrum <= DFT_SMEM_BINS) {
     const size_t smem = sizeof(double2) * (size_t)h->nSpectrum;
@@ -284,6 +369,16 @@ template <class TIN> int run_spectrum(b200dd_spectrum *h, const TIN *d_x, double
     spec_dft_kernel<false><<<gridD, DFT_THREADS, 0, st>>>(h->d_g, h->d_w, d_out, h->nSpectrum);
   }
   B2_LAUNCH_CHECK();
+  return B200DD_OK;
+}
+
+// the CPI's spectrum: the fold of its first nfft samples, finished from its chunks
+template <class TIN> int run_spectrum(b200dd_spectrum *h, const TIN *d_x, double2 *d_out, cudaStream_t st, bool timed) {
+  if (timed) B2_CUDA(cudaEventRecord(h->ev[0], st));
+  uint32_t chunks = 0;
+  if (int rc = fold_chunks(h, d_x, 0, h->nfft, st, &chunks)) return rc;
+  if (timed) B2_CUDA(cudaEventRecord(h->ev[1], st));
+  if (int rc = finish(h, h->d_part, chunks, d_out, st)) return rc;
   if (timed) B2_CUDA(cudaEventRecord(h->ev[2], st));
   return B200DD_OK;
 }
@@ -325,19 +420,15 @@ static int spectrum_host_plan(uint32_t n, double bandwidth, b200dd_spectrum *h) 
   uint32_t wantChunks = (132u * 8u + colTiles - 1) / colTiles;
   if (wantChunks < 1) wantChunks = 1;
   if (wantChunks > 256) wantChunks = 256;
-  uint32_t rows = (decimation + wantChunks - 1) / wantChunks;
-  if (rows < (uint32_t)FOLD_UNROLL) rows = FOLD_UNROLL;
-  h->rowsPerChunk = rows;
-  h->nChunks = (decimation + rows - 1) / rows;
+  h->wantChunks = wantChunks;
+  fold_chunking(decimation, wantChunks, &h->rowsPerChunk, &h->nChunks);
   {
     const uint32_t perSm = 6u;  // resident CTAs per SM of spec_fold2_kernel (80 registers)
     const uint32_t colTiles2 = (nSpectrum / 2 + FOLD_THREADS - 1) / FOLD_THREADS;
     uint32_t want2 = (132u * perSm + (colTiles2 ? colTiles2 : 1) - 1) / (colTiles2 ? colTiles2 : 1);
     if (want2 > 256) want2 = 256;
-    uint32_t rows2 = (decimation + want2 - 1) / want2;
-    if (rows2 < 8u) rows2 = 8u;
-    h->rowsPerChunk2 = rows2;
-    h->nChunks2 = (decimation + rows2 - 1) / rows2;
+    h->wantChunks2 = want2;
+    fold_chunking(decimation, want2, &h->rowsPerChunk2, &h->nChunks2);
   }
   return B200DD_OK;
 }
@@ -382,7 +473,8 @@ int b200dd_spectrum_create(uint32_t n, double bandwidth, int32_t device, b200dd_
   B2_CUDA(h->d_t1.alloc(decimation));
   B2_CUDA(h->d_t2.alloc(nSpectrum));
   B2_CUDA(h->d_w.alloc(nSpectrum));
-  B2_CUDA(h->d_part.alloc((size_t)(h->nChunks > h->nChunks2 ? h->nChunks : h->nChunks2) * nSpectrum));
+  // a fold of any slice has at most wantChunks(2) chunks (fold_chunking), the whole CPI's among them
+  B2_CUDA(h->d_part.alloc((size_t)std::max(h->wantChunks, h->wantChunks2) * nSpectrum));
   B2_CUDA(h->d_g.alloc(nSpectrum));
   B2_CUDA(h->d_out.alloc(nSpectrum));
   B2_CUDA(cudaMemcpy(h->d_t1, t1.data(), sizeof(double2) * decimation, cudaMemcpyHostToDevice));
@@ -429,6 +521,30 @@ int b200dd_spectrum_process_device(b200dd_spectrum *h, const void *d_x, uint32_t
   DeviceGuard guard(h->device);
   cudaStream_t st = stream_or(stream, h->stream);
   return run_spectrum<float2>(h, (const float2 *)d_x, d_spectrum ? (double2 *)d_spectrum : h->d_out, st, false);
+}
+
+int b200dd_spectrum_fold_slice_device(b200dd_spectrum *h, const void *d_x, uint32_t sample0, uint32_t n, void *d_part,
+                                      void *stream) {
+  if (!h || !d_part || (!d_x && n)) return arg_fail("b200dd_spectrum_fold_slice_device: null argument");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream_or(stream, h->stream);
+  const uint64_t end = std::min<uint64_t>((uint64_t)sample0 + n, h->nfft);
+  if (end <= sample0) {  // nothing of [0, nfft): the part is zero
+    B2_CUDA(cudaMemsetAsync(d_part, 0, sizeof(double2) * h->nSpectrum, st));
+    return B200DD_OK;
+  }
+  uint32_t chunks = 0;
+  if (int rc = fold_chunks(h, (const float2 *)d_x, sample0, end, st, &chunks)) return rc;
+  return reduce_parts(h, h->d_part, chunks, nullptr, (double2 *)d_part, st);
+}
+
+int b200dd_spectrum_finish_device(b200dd_spectrum *h, const void *d_parts, uint32_t n_parts, void *d_spectrum,
+                                  void *stream) {
+  if (!h || !d_parts) return arg_fail("b200dd_spectrum_finish_device: null argument");
+  if (n_parts == 0) return arg_fail("b200dd_spectrum_finish_device: no parts");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream_or(stream, h->stream);
+  return finish(h, (const double2 *)d_parts, n_parts, d_spectrum ? (double2 *)d_spectrum : h->d_out, st);
 }
 
 int b200dd_spectrum_process_device_f64(b200dd_spectrum *h, const void *d_x, uint32_t n, void *d_spectrum, void *stream) {

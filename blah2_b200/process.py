@@ -294,6 +294,11 @@ class WienerHopfChunk(_Handle):
         rc = capi.check(self._lib.b200dd_wh_last_status(self._h), allow=(capi.FILTER_FAILED,))
         return rc == capi.OK
 
+    def device_status(self) -> int:
+        """Device pointer of the chunk's clutter-filter status word (0: the solve succeeded), written by filter_device.
+        The solve is replicated, so every chunk's word holds the CPI's verdict (Pipeline.submit_map takes it)."""
+        return int(self._lib.b200dd_wh_device_status(self._h))
+
     def debug_weights(self):
         """(w, a, b) of the last filter_device call (tests)."""
         w = np.empty(self.nBins, dtype=np.complex128)
@@ -336,6 +341,22 @@ class SpectrumAnalyser(_Handle):
         f64 = getattr(d_x, "element_size", lambda: 8)() == 16
         fn = self._lib.b200dd_spectrum_process_device_f64 if f64 else self._lib.b200dd_spectrum_process_device
         capi.check(fn(self._h, capi.ptr(d_x), int(n), capi.ptr(d_spectrum), self._st(stream)))
+
+    def fold_slice_device(self, d_x, sample0, d_part, stream=None):
+        """Folds the reference-channel samples [sample0, sample0 + len(d_x)) -- d_x a complex64 CUDA tensor whose first
+        element is global sample sample0 -- into d_part (complex128 CUDA tensor of nSpectrum): their share of the
+        CPI's spectrum before its last phase and transform.  Samples at or past nfft contribute nothing.
+        Asynchronous; finish_device turns the parts of slices covering [0, nfft) into the spectrum."""
+        n = int(d_x.numel())
+        capi.check(self._lib.b200dd_spectrum_fold_slice_device(self._h, capi.ptr(d_x) if n else None, int(sample0), n,
+                                                               capi.ptr(d_part), self._st(stream)))
+
+    def finish_device(self, d_parts, d_spectrum=None, stream=None):
+        """The spectrum from the parts of fold_slice_device (complex128 CUDA tensor [n_parts, nSpectrum]), summed in
+        index order, into d_spectrum or, when None, the handle's buffer (read with fetch()).  Asynchronous."""
+        n_parts = int(d_parts.numel()) // self.nSpectrum
+        capi.check(self._lib.b200dd_spectrum_finish_device(self._h, capi.ptr(d_parts), n_parts, capi.ptr(d_spectrum),
+                                                           self._st(stream)))
 
     def fetch(self, stream=None):
         out = np.empty(self.nSpectrum, dtype=np.complex128)
@@ -964,6 +985,24 @@ class Pipeline(_Handle):
         as after a submit; d_map must stay untouched until fetch().  Raises B200ddError (ERR_ARG) for a record of
         other parameters or stages."""
         capi.check(self._lib.b200dd_pipeline_submit_record(self._h, capi.ptr(d_record), capi.ptr(d_map)))
+
+    def submit_map(self, d_map, d_status=None, d_parts=None, stream=None):
+        """Takes a CPI whose complex64 map d_map (nDoppler x nDelay CUDA tensor) was computed elsewhere -- e.g. placed
+        from the tiles of shard.SingleCpiPlan -- and runs set_metrics, detection and every product after them on it
+        (b200dd_pipeline_submit_map).  d_status: device pointer (int) of the clutter-filter verdict, required iff the
+        clutter filter is enabled (WienerHopfChunk.device_status()); d_parts: the spectrum parts of
+        SpectrumAnalyser.fold_slice_device as a complex128 CUDA tensor [n_parts, nSpectrum], required iff the spectrum
+        stage is enabled.  Asynchronous on `stream`; then fetch() and every fetch_* behave as after a submit.  d_map
+        must stay untouched until fetch().  Raises B200ddError (ERR_ARG) for a missing or unexpected argument."""
+        n_parts = int(d_parts.numel()) // max(self.n_spectrum, 1) if d_parts is not None else 0
+        capi.check(self._lib.b200dd_pipeline_submit_map(self._h, capi.ptr(d_map), capi.ptr(d_status), capi.ptr(d_parts),
+                                                        n_parts, self._st(stream)))
+
+    def stamp(self, slot, stream=None):
+        """Timing stage: stamps the boundary ``slot`` (capi.STAMP_CHAIN, _SPECTRUM, _CLUTTER) of the CPI about to be
+        given to submit_map, on ``stream``; boundaries not stamped are stamped at submit_map's start.  Does nothing
+        when the timing stage is off."""
+        capi.check(self._lib.b200dd_pipeline_stamp(self._h, int(slot), self._st(stream)))
 
     def fetch_spectrum(self):
         """Spectrum of the reference channel of the last submitted CPI (complex128, nSpectrum bins)."""

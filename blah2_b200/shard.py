@@ -12,6 +12,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from .capi import STAMP_CHAIN, STAMP_CLUTTER, STAMP_SPECTRUM
 from .process import _Handle
 
 
@@ -334,10 +335,19 @@ class SingleCpiPlan:
       4. Doppler transform of the rank's tile of delay columns                         (Ambiguity.cpp:152-169);
       5. gather of the tiles to rank `dst`, placed into the row-major map.
     All buffers are allocated here, once; `run` only enqueues kernels and exchanges (`comm` is a blah2_b200.shard.Comm
-    on GPUs, a TorchComm in the CPU tests; `amb` / `whc_factory` are the process-layer classes or CPU stand-ins)."""
+    on GPUs, a TorchComm in the CPU tests; `amb` / `whc_factory` are the process-layer classes or CPU stand-ins).
 
-    def __init__(self, comm, amb, n_samples: int, device, clutter=None, whc_factory=None, dst: int = 0):
+    Every product of the CPI on `dst`: ``spectrum`` (every rank) is a SpectrumAnalyser(n_samples, bandwidth); each
+    rank folds its samples [s0, s0 + ns) below nfft into one part of the spectrum, and the parts are gathered to
+    `dst` in rank order.  ``pipeline`` (rank `dst` only) is the importing Pipeline, created with the full parameters:
+    `run` stamps its stage boundaries and ends with pipeline.submit_map of the placed map, the chunk's clutter-filter
+    verdict and the parts; the caller then fetches on `dst` as from any pipeline.  The plan reuses its map and part
+    buffers, so a run must follow the fetch of the previous CPI."""
+
+    def __init__(self, comm, amb, n_samples: int, device, clutter=None, whc_factory=None, dst: int = 0,
+                 spectrum=None, pipeline=None):
         self.comm, self.amb, self.dst = comm, amb, dst
+        self.spectrum, self.pipeline = spectrum, pipeline
         rank, world = comm.rank, comm.world
         g = amb.geometry
         self.n_dop, self.n_del, self.n_corr = g.n_doppler_bins, g.n_delay_bins, g.n_corr
@@ -373,6 +383,12 @@ class SingleCpiPlan:
         else:
             self.x_own = torch.zeros(self.ns, dtype=c64, device=device)
             self.y_own = torch.zeros(self.ns, dtype=c64, device=device)
+        if spectrum is not None:
+            # the rank's samples below nfft (none when the slice starts past it)
+            self.n_fold = max(0, min(self.ns, spectrum.nfft - self.s0))
+            self.part = torch.zeros(spectrum.nSpectrum, dtype=torch.complex128, device=device)
+            self.parts = torch.zeros((world, spectrum.nSpectrum), dtype=torch.complex128, device=device) \
+                if rank == dst else None
 
     def run(self, stream=None, marks=None):
         """Process the CPI whose samples are in x_own / y_own.  Returns the [nDop, nDel] map on `dst`, None elsewhere
@@ -387,6 +403,15 @@ class SingleCpiPlan:
                 e.record(stream)
                 marks.append((label, e))
         mark("start")
+        pipe = self.pipeline if rank == self.dst else None
+        if pipe is not None:
+            pipe.stamp(STAMP_CHAIN, sp)
+        if self.spectrum is not None:
+            self.spectrum.fold_slice_device(self.x_own[:self.n_fold], self.s0, self.part, sp)
+            comm.gather_async(self.part, self.parts, self.dst, after=stream)
+            mark("spectrum")
+        if pipe is not None:
+            pipe.stamp(STAMP_SPECTRUM, sp)
         x, y = self.x_own, self.y_own
         if self.whc is not None:
             nxt, prv = (rank + 1) % world, (rank - 1) % world
@@ -407,6 +432,8 @@ class SingleCpiPlan:
             self.whc.filter_device(self.ab, self.x_loc, self.y_loc, self.y_f, sp)
             mark("wh_solve_filter")
             y = self.y_f
+        if pipe is not None:
+            pipe.stamp(STAMP_CLUTTER, sp)
         n_own = self.nb * self.n_corr
         self.amb.range_device(x[:n_own], y[:n_own], self.b0, self.nb, self.R_local, sp)
         mark("range")
@@ -427,4 +454,8 @@ class SingleCpiPlan:
                 off = self.tile_offsets[r] // 8
                 self.amb.place_tile(self.tiles_all[off:off + self.n_dop * nc], c0, nc, self.map, sp)
         mark("place_tiles")
+        if pipe is not None:
+            pipe.submit_map(self.map, self.whc.device_status() if self.whc is not None else None,
+                            self.parts if self.spectrum is not None else None, sp)
+            mark("submit_map")
         return self.map

@@ -360,6 +360,20 @@ B200DD_API int b200dd_spectrum_process_device(b200dd_spectrum *h, const void *d_
                                               void *stream);
 B200DD_API int b200dd_spectrum_process_device_f64(b200dd_spectrum *h, const void *d_x, uint32_t n, void *d_spectrum,
                                                   void *stream);
+/* The spectrum of a CPI whose reference channel is spread over GPUs.  fold_slice: fold the reference-channel samples
+ * [sample0, sample0 + n) -- d_x[0] is global sample sample0, float2 -- into n_spectrum complex128 column sums at
+ * d_part (the fold's contribution of those samples, before the t2 phase).  Samples at or past nfft contribute
+ * nothing; a slice with none writes a zero part.  Parts of slices that cover [0, nfft) exactly once, handed to
+ * b200dd_spectrum_finish_device, give the CPI's spectrum.  finish: sum n_parts parts (n_parts x n_spectrum
+ * complex128, back to back) in index order, apply t2 and the n_spectrum-point DFT; d_spectrum nullable = the
+ * handle's own buffer, as b200dd_spectrum_process_device.  One slice [0, n >= nfft) and a one-part finish equal
+ * b200dd_spectrum_process_device bit for bit; parts summed in a fixed order give a spectrum that is deterministic for
+ * a given partition.  Both asynchronous on `stream` (NULL = the handle's stream).  B200DD_ERR_ARG: a null handle or
+ * d_part / d_parts, a null d_x with n > 0, n_parts == 0. */
+B200DD_API int b200dd_spectrum_fold_slice_device(b200dd_spectrum *h, const void *d_x, uint32_t sample0, uint32_t n,
+                                                 void *d_part, void *stream);
+B200DD_API int b200dd_spectrum_finish_device(b200dd_spectrum *h, const void *d_parts, uint32_t n_parts, void *d_spectrum,
+                                             void *stream);
 /* Copies the handle's buffer (result of the last process_device call with d_spectrum == NULL) to the host and
  * synchronises the stream. */
 B200DD_API int b200dd_spectrum_fetch(b200dd_spectrum *h, double *spectrum_out, void *stream);
@@ -812,7 +826,10 @@ B200DD_API int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out,
  *                         that conversion runs after the filter); device submits: 0
  *   spectrum              the spectrum kernels and the IQ-data render (when the spectrum stage is enabled)
  *   clutter_filter        the WienerHopf kernels (when the clutter filter is enabled)
- *   ambiguity_processing  CAF and set_metrics
+ *   ambiguity_processing  CAF and set_metrics (after b200dd_pipeline_submit_map: from the clutter boundary to the end
+ *                         of set_metrics -- whatever the caller enqueued after that stamp, for SingleCpiPlan the
+ *                         distributed CAF and the tile placement, then the spectrum finish, the IQ-data render and
+ *                         set_metrics)
  *   detector              CFAR -> Centroid -> Interpolate (when detection is enabled)
  *   tracker               the tracker run at the CPI's first track fetch (when the tracker is enabled; 0 when CFAR
  *                         overflowed and the tracker skipped the CPI)
@@ -911,6 +928,36 @@ B200DD_API int b200dd_pipeline_share_history(b200dd_pipeline *const *members, ui
 B200DD_API int b200dd_pipeline_enable_export(b200dd_pipeline *h, uint32_t max_detections, size_t *record_bytes);
 B200DD_API int b200dd_pipeline_export_record(b200dd_pipeline *h, const void **d_record);
 B200DD_API int b200dd_pipeline_submit_record(b200dd_pipeline *h, const void *d_record, const void *d_map);
+
+/* One CPI over GPUs with every product on one rank (blah2_b200.shard.SingleCpiPlan): no GPU holds the whole CPI, so
+ * no rank can export a record; the importing pipeline, created with the full parameters, takes the assembled map and
+ * runs everything after the CAF itself.
+ *
+ * submit_map: the pipeline takes a CPI whose float2 map d_map (nDoppler x nDelay) was computed elsewhere, e.g. placed
+ * from the tiles of SingleCpiPlan.  d_filter_status: a device int holding the clutter-filter verdict (required iff
+ * the clutter filter is enabled; b200dd_wh_device_status of a chunk handle holds the global one, the solve being
+ * replicated).  d_spectrum_parts / n_parts: the parts of b200dd_spectrum_fold_slice_device (required iff the spectrum
+ * stage is enabled).  On `stream` (NULL = the pipeline's stream), ordered after what is already there, without host
+ * synchronisation, it enqueues: the spectrum finish into the pipeline's spectrum buffer and the IQ-data render; a
+ * copy of the verdict into the pipeline's clutter-filter status word; set_metrics and the detection stages on d_map;
+ * the map document, the max-hold push (at fetch for a share-set member) and the detection document; the detector and
+ * output stamps.  d_map must stay untouched until b200dd_pipeline_fetch.  Afterwards every fetch, stash, the tracker
+ * and the share-set rules behave as after a submit (path: device); a verdict of B200DD_FILTER_FAILED imports as a
+ * failed solve: nothing is committed, nCpi does not step.  No record is packed, and no graph is recorded.
+ * B200DD_ERR_ARG, nothing enqueued: a null h or d_map; a status given without the clutter filter or missing with it;
+ * parts given without the spectrum stage, missing with it, or n_parts == 0; a share-set member whose last CPI is not
+ * fetched.
+ *
+ * stamp: timing stage, the boundary `slot` (B200DD_STAMP_*) of the CPI about to be submitted with submit_map, on
+ * `stream` (NULL = the pipeline's stream).  submit_map stamps at its start every one of the three not stamped since
+ * the last submit, so that stages whose work ran elsewhere read 0 ms.  Nothing is enqueued when the timing stage is
+ * off.  B200DD_ERR_ARG: a null handle, another slot. */
+#define B200DD_STAMP_CHAIN 0     /* the CPI's first stamp: before its spectrum */
+#define B200DD_STAMP_SPECTRUM 1  /* after the spectrum fold (the exchange of the parts runs on its own stream) */
+#define B200DD_STAMP_CLUTTER 2   /* after the clutter filter */
+B200DD_API int b200dd_pipeline_submit_map(b200dd_pipeline *h, const void *d_map, const int *d_filter_status,
+                                          const void *d_spectrum_parts, uint32_t n_parts, void *stream);
+B200DD_API int b200dd_pipeline_stamp(b200dd_pipeline *h, int slot, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Inter-GPU exchanges (one process per GPU, NCCL over NVLink / NVSwitch).  The reference has no
