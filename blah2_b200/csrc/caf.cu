@@ -860,11 +860,6 @@ int caf_run_device(b200dd_caf *h, const float2 *d_x, const float2 *d_y, float2 *
   return B200DD_OK;
 }
 
-inline int grid_for(uint32_t n) {
-  int b = (int)((n + 255u) / 256u);
-  return b > 132 * 8 ? 132 * 8 : (b < 1 ? 1 : b);
-}
-
 }  // namespace
 
 // ------------------------------------------------------------------ C ABI

@@ -142,6 +142,12 @@ inline int resolve_device(int requested, int *dev) {
 // the caller's stream, else the handle's own
 inline cudaStream_t stream_or(void *stream, cudaStream_t own) { return stream ? (cudaStream_t)stream : own; }
 
+// the grid of a grid-stride loop over n items in 256-thread blocks: one block per 256 items, at most 8 per SM of 132
+inline int grid_for(uint32_t n) {
+  int b = (int)((n + 255u) / 256u);
+  return b > 132 * 8 ? 132 * 8 : (b < 1 ? 1 : b);
+}
+
 // A handle under construction, released into *out on success; a failed create frees it with the handle's destroy.
 template <class H> using Owned = std::unique_ptr<H, void (*)(H *)>;
 

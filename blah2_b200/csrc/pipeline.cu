@@ -10,6 +10,8 @@
 #include <cstring>
 #include <new>
 #include <string>
+#include <type_traits>
+#include <variant>
 #include <vector>
 
 using namespace b2;
@@ -71,11 +73,6 @@ __global__ void pl_ingest_ci8_kernel(const int8_t *__restrict__ x8, const int8_t
   }
 }
 
-inline int grid_for(uint32_t n) {
-  int b = (int)((n + 255u) / 256u);
-  return b > 132 * 8 ? 132 * 8 : (b < 1 ? 1 : b);
-}
-
 // The timing stage's device stamps, one slot per stage boundary (timing.cu).  Each stage's time is its closing stamp
 // minus the stamp before it in the chain.
 enum TmSlot {
@@ -91,6 +88,8 @@ enum TmSlot {
   kTmTracker1,
   kTmSlots
 };
+// the slots of b200dd_pipeline_stamp's boundaries B200DD_STAMP_CHAIN, _SPECTRUM and _CLUTTER
+constexpr int kStampSlots[] = {kTmChain, kTmSpectrum, kTmClutter};
 // kTmIngest: the host submits of capture-driver samples (int16, int8, complex64), whose extract_buffer is the H2D copy
 // and any de-interleave before the device chain
 enum TmPath { kTmNone, kTmHost, kTmIngest, kTmDevice };
@@ -98,17 +97,16 @@ enum TmPath { kTmNone, kTmHost, kTmIngest, kTmDevice };
 // the sample format a host submit takes
 enum HostFormat { kC128, kInt16, kCi8, kCf32 };
 
-// The stages whose fetches read the last CPI: one bit each in LastCpi::stages.
-enum StageBit : unsigned {
-  kIqBit = 1u,
-  kMapBit = 2u,
-  kMaxholdBit = 4u,
-  kDetBit = 8u,
-  kTrackBit = 16u,
-  kTimingBit = 32u,
-  kAllBits = 63u,
-  kShareBits = kIqBit | kMaxholdBit | kDetBit | kTrackBit | kTimingBit,  // the stages a share set takes over
-};
+// The optional stages.  The fetches of all but the spectrum read the last CPI: one bit each in LastCpi::stages.
+enum Stage { kIq, kMap, kMaxhold, kDet, kTrack, kTiming, kSpectrum, kStages };
+constexpr unsigned stage_bit(Stage s) { return 1u << s; }
+constexpr unsigned kAllBits = stage_bit(kSpectrum) - 1;
+constexpr unsigned kShareBits = kAllBits & ~stage_bit(kMap);  // the stages a share set takes over
+// each stage as the fetches' messages name it, and what a CPI whose clutter-filter solve failed lacks there
+const char *const kStageName[kStages] = {"IQ-data JSON", "map JSON", "max-hold", "detection JSON",
+                                         "tracker", "timing JSON", "spectrum"};
+const char *const kStageSkipped[kStages] = {"it has no document", "it has no map", nullptr, "it has no detections",
+                                            "the tracker skips it", "it has no document", nullptr};
 
 // ---- CPI record (b200dd_pipeline_enable_export / _submit_record): one fixed-size device buffer per CPI holding
 // everything the fetches read besides the map.  Layout, each section 16-byte aligned, present as its stage is:
@@ -227,21 +225,37 @@ __global__ void __launch_bounds__(256) pl_unpack_kernel(RecordArgs a) {
 
 }  // namespace
 
-// The stateful stages of a share set (b200dd_pipeline_share_history): one max-hold window, one detection history,
-// one IQ-data history, one tracker and one timing history for all members, each null when the members do not enable
-// it.  Every device operation on them is enqueued on the stream of the member that makes it, after the set's event,
-// and records the event again: so they run in the order the host calls them, whatever streams the members use.  The
-// timing history lives on the host and changes in that order too.
-struct ShareSet {
-  int device = 0;
-  std::vector<b200dd_pipeline *> members;
-  int64_t next_cpi = 0;  // the number the next submit to any member gets
+// The stateful stages: the max-hold window, the detection and IQ-data histories, the tracker and the timing history,
+// each null when it is not enabled, and the share-set number of the CPI each stage took last (-1 outside a share
+// set).  A lone pipeline holds its own, whose detection and IQ-data histories are those of its renders (dj and ij of
+// the pipeline, null here); a share set holds the one its members share, into which their renders commit.
+struct Stateful {
   b200dd_maxhold *mh = nullptr;
   b200dd_detjson *dj = nullptr;
   b200dd_iqjson *ij = nullptr;
   b200dd_tracker *tr = nullptr;
-  TimingHistory *tm = nullptr;  // host state: its commits need no event
-  int64_t mh_last = -1, dj_last = -1, ij_last = -1, tr_last = -1, tm_last = -1;  // the CPI each one took last
+  TimingHistory *tm = nullptr;  // host state: a share set's commits need no event
+  int64_t last[kStages] = {-1, -1, -1, -1, -1, -1, -1};
+};
+
+static void stateful_free(Stateful &s) {
+  b200dd_maxhold_destroy(s.mh);
+  b200dd_detjson_destroy(s.dj);
+  b200dd_iqjson_destroy(s.ij);
+  b200dd_tracker_destroy(s.tr);
+  timing_history_destroy(s.tm);
+  s = Stateful{};
+}
+
+// A share set (b200dd_pipeline_share_history): one set of stateful stages for all members.  Every device operation
+// on them is enqueued on the stream of the member that makes it, after the set's event, and records the event again:
+// so they run in the order the host calls them, whatever streams the members use.  The timing history lives on the
+// host and changes in that order too.
+struct ShareSet {
+  int device = 0;
+  std::vector<b200dd_pipeline *> members;
+  int64_t next_cpi = 0;  // the number the next submit to any member gets
+  Stateful st;
   Event ev;
   bool ev_recorded = false;
 };
@@ -250,7 +264,7 @@ struct ShareSet {
 // how far they have got with it.
 struct LastCpi {
   void *stream = nullptr;  // the stream it was submitted on: its products are there, its fetches run there
-  // StageBit: set by every submit, cleared when the stage is enabled or the pipeline joins a share set.  A stage
+  // stage_bit: set by every submit, cleared when the stage is enabled or the pipeline joins a share set.  A stage
   // whose bit is clear has no CPI submitted since then to fetch.
   unsigned stages = 0;
   int path = kTmNone;      // how it came in
@@ -276,13 +290,12 @@ struct b200dd_pipeline {
   b200dd_spectrum *spec = nullptr;  // optional first stage (blah2.cpp:263-265)
   b200dd_iqjson *ij = nullptr;      // optional, after the spectrum: the IQ-data document (blah2.cpp:299-300) and its stash
   b200dd_mapjson *mj = nullptr;     // optional last stage: the map document (blah2.cpp:303-304)
-  b200dd_maxhold *mh = nullptr;     // optional: the API's max-hold window (api/stash/maxhold.js)
   b200dd_detjson *dj = nullptr;     // optional: the detection document (blah2.cpp:312-317) and its stash
-  b200dd_tracker *tr = nullptr;     // optional: the tracker (blah2.cpp:291-296), run at fetch time
-  // optional: the timing document (blah2.cpp:331-345) from device stamps at the chain's stage boundaries, and its
-  // /stash/timing history (null for a share-set member: the set's)
+  // optional: the API's max-hold window (api/stash/maxhold.js), the tracker (blah2.cpp:291-296, run at fetch time)
+  // and the /stash/timing history; empty for a share-set member, which uses the set's (see `stateful`)
+  Stateful own;
+  // optional: the timing document (blah2.cpp:331-345) from device stamps at the chain's stage boundaries
   bool tm_on = false;               // the submits enqueue stamps
-  TimingHistory *tm = nullptr;
   uint64_t tm_t_start = 0;
   DevBuf<uint64_t> d_tm;            // the last submit's stamps, TmSlot
   std::vector<const char *> tm_names;  // behind the last document written
@@ -316,7 +329,7 @@ struct b200dd_pipeline {
   uint32_t dj_max_held = 0;
   b200dd_tracker_params tr_params{};
   uint32_t tr_max_tracks = 0, tr_max_history = 0;
-  ShareSet *set = nullptr;  // share-set membership: the stateful stages above are null and the set's are used
+  ShareSet *set = nullptr;  // share-set membership: `own` is empty and the set's stateful stages are used
   // CPI export (b200dd_pipeline_enable_export): every submit packs its record into d_rec; exp_max == 0 is off
   uint32_t exp_max = 0;
   RecordLayout exp_layout;
@@ -330,6 +343,16 @@ static void pipeline_drop_graphs(b200dd_pipeline *h) {
     if (e.exec) cudaGraphExecDestroy(e.exec);
   h->graphs.clear();
 }
+
+// the stateful stages a pipeline uses: its share set's, else its own
+static Stateful &stateful(b200dd_pipeline *h) {
+  if (ShareSet *s = h->set) return s->st;
+  return h->own;
+}
+static const Stateful &stateful(const b200dd_pipeline *h) { return stateful(const_cast<b200dd_pipeline *>(h)); }
+
+// B200DD_ERR_ARG with the message "<entry>: <what>"
+static int entry_fail(const char *entry, const std::string &what) { return arg_fail((entry + (": " + what)).c_str()); }
 
 // the set's operations run after the previous one (see ShareSet)
 static int set_wait(ShareSet *s, void *st) {
@@ -358,14 +381,85 @@ template <class Op> static int set_ordered(ShareSet *s, void *st, Op op) {
 // old stage (when the stage is in the chain), the old handle destroyed, and no CPI for the stage's fetches until the
 // next submit.
 template <class T>
-static int stage_reset(b200dd_pipeline *h, T *&stage, void (*destroy)(T *), unsigned bit, bool in_chain = true) {
+static int stage_reset(b200dd_pipeline *h, T *&stage, void (*destroy)(T *), Stage s, bool in_chain = true) {
   B2_CUDA(cudaStreamSynchronize(h->stream));
   if (in_chain) pipeline_drop_graphs(h);
   destroy(stage);
   stage = nullptr;
-  h->last.stages &= ~bit;
+  h->last.stages &= ~stage_bit(s);
   return B200DD_OK;
 }
+
+// Visits the fields that shape a pipeline's products, in one order: its parameters (not the device: members compare
+// it as resolved at create), then its stages' settings.  v(x) for each integer or double field x.  The clutter
+// filter's and detection's parameters are visited when v.uses(on) returns true, each stage's settings when
+// v.stage(stage, on) does, `on` being whether the pipeline runs that stage.
+template <class V> static void visit_params(const b200dd_pipeline *h, V &v) {
+  const b200dd_pipeline_params &p = h->p;
+  const b200dd_caf_params &c = p.caf;
+  const b200dd_det_params &d = p.det;
+  v(c.delay_min); v(c.delay_max); v(c.doppler_min); v(c.doppler_max); v(c.fs); v(c.n_samples); v(c.round_hamming);
+  v(p.clutter_enable);
+  if (v.uses(p.clutter_enable)) { v(p.clutter_delay_min); v(p.clutter_delay_max); }
+  v(p.detection_enable);
+  if (v.uses(p.detection_enable)) {
+    v(d.pfa); v(d.n_guard); v(d.n_train); v(d.min_delay); v(d.min_doppler); v(d.n_centroid_delay);
+    v(d.n_centroid_doppler); v(d.resolution_doppler); v(d.interp_delay); v(d.interp_doppler);
+  }
+  if (v.stage(kSpectrum, h->spec)) v(h->spec_bandwidth);
+  if (v.stage(kIq, h->ij)) { v(h->ij_metrics[0]); v(h->ij_metrics[1]); v(h->ij_metrics[2]); }
+  v.stage(kMaxhold, h->own.mh);
+  if (v.stage(kDet, h->dj)) v(h->dj_max_held);
+  if (v.stage(kTiming, h->tm_on)) v(h->tm_t_start);
+  if (v.stage(kTrack, h->own.tr)) {
+    const b200dd_tracker_params &t = h->tr_params;
+    v(t.m); v(t.n); v(t.n_delete); v(t.cpi); v(t.max_acc_init); v(t.fs); v(t.fc);
+    v(h->tr_max_tracks); v(h->tr_max_history);
+  }
+}
+
+// A pipeline's fields as b200dd_pipeline_share_history compares them with ==: every parameter, whether its stage
+// runs or not, and whether each stage runs and, if it does, its settings.
+struct ParamValues {
+  using Value = std::variant<uint64_t, double>;
+  std::vector<Value> params, stages;
+  template <class T> void operator()(T x) {
+    std::vector<Value> &to = stages.empty() ? params : stages;  // the stages' settings follow the first stage's flag
+    if constexpr (std::is_floating_point<T>::value) to.push_back((double)x);
+    else to.push_back((uint64_t)x);
+  }
+  bool uses(bool) { return true; }
+  bool stage(Stage, bool on) {
+    stages.push_back(Value((uint64_t)on));
+    return on;
+  }
+};
+
+// FNV-1a over everything that shapes a record's products: the CAF parameters, the clutter filter's and detection's
+// when they run, the spectrum stage's size and bandwidth, the timing flag and the layout L.  Exporter and importer
+// must agree on it.
+struct RecordFingerprint {
+  const RecordLayout &L;
+  uint64_t f = 1469598103934665603ull;
+  void mix(uint64_t v) {
+    for (int i = 0; i < 8; i++) {
+      f ^= (v >> (8 * i)) & 0xFFu;
+      f *= 1099511628211ull;
+    }
+  }
+  template <class T> void operator()(T x) {  // an integer sign- or zero-extended to 64 bits, a double's bits
+    uint64_t v;
+    if constexpr (std::is_floating_point<T>::value) memcpy(&v, &x, sizeof v);
+    else v = (uint64_t)x;
+    mix(v);
+  }
+  bool uses(bool on) { return on; }
+  bool stage(Stage s, bool) {
+    if (s == kSpectrum) mix(L.n_spec);
+    if (s == kTiming) mix(L.timing ? 1 : 0);
+    return s == kSpectrum && L.n_spec;
+  }
+};
 
 extern "C" {
 
@@ -416,10 +510,8 @@ void b200dd_pipeline_destroy(b200dd_pipeline *h) {
   b200dd_spectrum_destroy(h->spec);
   b200dd_iqjson_destroy(h->ij);
   b200dd_mapjson_destroy(h->mj);
-  b200dd_maxhold_destroy(h->mh);
   b200dd_detjson_destroy(h->dj);
-  b200dd_tracker_destroy(h->tr);
-  timing_history_destroy(h->tm);
+  stateful_free(h->own);
   delete h;
 }
 
@@ -442,14 +534,15 @@ static int maxhold_push(const b200dd_pipeline *h, b200dd_maxhold *mh, const void
                                       (cudaStream_t)st);
 }
 
-// the optional stages after set_metrics, on the map `map` of the CPI just enqueued on `st`
+// the optional stages after set_metrics, on the map `map` of the CPI just enqueued on `st` (a share-set member's
+// window push runs at fetch instead, member_fetch)
 static int pipeline_enqueue_products(b200dd_pipeline *h, float2 *map, void *st) {
   if (h->mj) {
     const int rc = mapjson_enqueue_with_metrics(h->mj, map, det_device_metrics(h->det), (cudaStream_t)st);
     if (rc != B200DD_OK) return rc;
   }
-  if (h->mh) {
-    const int rc = maxhold_push(h, h->mh, map, st);
+  if (h->own.mh) {
+    const int rc = maxhold_push(h, h->own.mh, map, st);
     if (rc != B200DD_OK) return rc;
   }
   if (h->dj) {
@@ -481,41 +574,14 @@ static RecordLayout record_layout(const b200dd_pipeline *h, uint32_t max_det) {
   return L;
 }
 
-// FNV-1a over everything that shapes a record's products: the CAF, clutter-filter and detection parameters (not the
-// device), the spectrum stage, the timing stage and the layout.  Exporter and importer must agree on it.
+// the fingerprint of the records `h` packs or takes in layout L
 static uint64_t record_fingerprint(const b200dd_pipeline *h, const RecordLayout &L) {
-  uint64_t f = 1469598103934665603ull;
-  auto mix = [&f](uint64_t v) {
-    for (int i = 0; i < 8; i++) {
-      f ^= (v >> (8 * i)) & 0xFFu;
-      f *= 1099511628211ull;
-    }
-  };
-  auto mixd = [&mix](double d) {
-    uint64_t v;
-    memcpy(&v, &d, sizeof v);
-    mix(v);
-  };
-  const b200dd_caf_params &c = h->p.caf;
-  const b200dd_det_params &d = h->p.det;
-  mix(kRecVersion);
-  mix((uint64_t)(int64_t)c.delay_min); mix((uint64_t)(int64_t)c.delay_max);
-  mix((uint64_t)(int64_t)c.doppler_min); mix((uint64_t)(int64_t)c.doppler_max);
-  mix(c.fs); mix(c.n_samples); mix((uint64_t)c.round_hamming);
-  mix((uint64_t)h->p.clutter_enable);
-  if (h->p.clutter_enable) { mix((uint64_t)(int64_t)h->p.clutter_delay_min); mix((uint64_t)(int64_t)h->p.clutter_delay_max); }
-  mix((uint64_t)h->p.detection_enable);
-  if (h->p.detection_enable) {
-    mixd(d.pfa); mix((uint64_t)(int64_t)d.n_guard); mix((uint64_t)(int64_t)d.n_train); mix((uint64_t)(int64_t)d.min_delay);
-    mixd(d.min_doppler); mix((uint64_t)(int64_t)d.n_centroid_delay); mix((uint64_t)(int64_t)d.n_centroid_doppler);
-    mixd(d.resolution_doppler); mix((uint64_t)(int64_t)d.interp_delay); mix((uint64_t)(int64_t)d.interp_doppler);
-  }
-  mix(L.n_spec);
-  if (L.n_spec) mixd(h->spec_bandwidth);
-  mix(L.timing ? 1 : 0);
-  mix(L.max_det);
-  mix(L.bytes);
-  return f;
+  RecordFingerprint v{L};
+  v.mix(kRecVersion);
+  visit_params(h, v);
+  v.mix(L.max_det);
+  v.mix(L.bytes);
+  return v.f;
 }
 
 // The record `rec` of layout L and `h`'s words it travels between: the stages' device buffers, which the pack kernel
@@ -622,10 +688,11 @@ static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const vo
   return pipeline_enqueue_tail(h, d_x, y, n, d_map ? (float2 *)d_map : h->d_map, path, st);
 }
 
-// After a submit enqueued its CPI on `st`, eagerly or as a graph replay, with map `map` (null: the pipeline's own):
-// the record its fetches read.  Every entry point calls this once, on success, and nothing else that a submit runs
-// changes that record: stream capture records the enqueue functions, and a replay runs none of their host code.
-static void pipeline_submitted(b200dd_pipeline *h, int path, void *st, const void *map) {
+// After a submit enqueued its CPI on `st`, eagerly or as a graph replay, with map `map` (null: the pipeline's own)
+// and, when `packed`, its export record: the record its fetches read.  Every entry point calls this once, on
+// success, and nothing else that a submit runs changes that record: stream capture records the enqueue functions,
+// and a replay runs none of their host code.
+static void pipeline_submitted(b200dd_pipeline *h, int path, void *st, const void *map, bool packed) {
   LastCpi &c = h->last;
   c.stream = st;
   c.stages = kAllBits;
@@ -643,7 +710,7 @@ static void pipeline_submitted(b200dd_pipeline *h, int path, void *st, const voi
   // an eager render marks its document itself; a replayed one cannot
   if (h->dj) detjson_mark_rendered(h->dj, true);
   if (h->ij) iqjson_mark_rendered(h->ij, true);
-  h->exp_valid = h->exp_max != 0;
+  h->exp_valid = packed;
   h->tm_pre = 0;
 }
 
@@ -655,8 +722,17 @@ static const b200dd_pipeline::GraphEntry *pipeline_find_graph(const b200dd_pipel
 }
 
 // A share-set member takes one CPI at a time: B200DD_ERR_ARG while its last one is not fetched.
-static int member_may_submit(const b200dd_pipeline *h, const char *msg) {
-  return h->set && h->last.unfetched ? arg_fail(msg) : B200DD_OK;
+static int member_may_submit(const b200dd_pipeline *h, const char *entry) {
+  return h->set && h->last.unfetched ? entry_fail(entry, "the share-set member's last CPI is not fetched yet")
+                                     : B200DD_OK;
+}
+
+// The start of submit `entry`: B200DD_ERR_ARG for a null argument (`args` false) and from member_may_submit; *st the
+// caller's stream, else the pipeline's.
+static int submit_start(const b200dd_pipeline *h, const char *entry, bool args, void *stream, cudaStream_t *st) {
+  if (!args) return entry_fail(entry, "null argument");
+  *st = stream_or(stream, h->stream);
+  return member_may_submit(h, entry);
 }
 
 // A CPI is 12+ kernel launches on the single submitting thread.  The chain's arguments only depend on the caller's
@@ -676,30 +752,31 @@ static int pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const voi
 
 int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
                                   void *stream) {
-  if (!h || !d_x || !d_y) return arg_fail("b200dd_pipeline_submit_device: null argument");
-  if (h->wh && n != h->p.caf.n_samples) return arg_fail("b200dd_pipeline_submit_device: the clutter filter needs exactly n_samples");
-  int rc = member_may_submit(h, "b200dd_pipeline_submit_device: the share-set member's last CPI is not fetched yet");
+  const char *entry = "b200dd_pipeline_submit_device";
+  cudaStream_t st;
+  int rc = submit_start(h, entry, h && d_x && d_y, stream, &st);
   if (rc != B200DD_OK) return rc;
-  void *st = stream ? stream : (void *)h->stream;
+  if (h->wh && n != h->p.caf.n_samples) return entry_fail(entry, "the clutter filter needs exactly n_samples");
   rc = pipeline_submit_device(h, d_x, d_y, n, d_map, kTmDevice, st);
-  if (rc == B200DD_OK) pipeline_submitted(h, kTmDevice, st, d_map);
+  if (rc == B200DD_OK) pipeline_submitted(h, kTmDevice, st, d_map, h->exp_max != 0);
   return rc;
 }
 
 int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n, void *d_map,
                                    void *stream) {
-  if (!h || !d_x || !d_y) return arg_fail("b200dd_pipeline_prepare_device: null argument");
+  const char *entry = "b200dd_pipeline_prepare_device";
+  if (!h || !d_x || !d_y) return entry_fail(entry, "null argument");
   if (h->eager_only) return B200DD_OK;
-  if (h->wh && n != h->p.caf.n_samples) return arg_fail("b200dd_pipeline_prepare_device: the clutter filter needs exactly n_samples");
+  if (h->wh && n != h->p.caf.n_samples) return entry_fail(entry, "the clutter filter needs exactly n_samples");
   DeviceGuard guard(h->device);
-  void *st = stream ? stream : (void *)h->stream;
+  const cudaStream_t st = stream_or(stream, h->stream);
   if (!pipeline_find_graph(h, d_x, d_y, n, d_map)) {
     // the eager run sets up what a capture must not do (uploads the axes, sizes scratch buffers); it is a CPI
-    int rc = member_may_submit(h, "b200dd_pipeline_prepare_device: the share-set member's last CPI is not fetched yet");
+    int rc = member_may_submit(h, entry);
     if (rc != B200DD_OK) return rc;
     rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, kTmDevice, st);
     if (rc != B200DD_OK) return rc;
-    pipeline_submitted(h, kTmDevice, st, d_map);
+    pipeline_submitted(h, kTmDevice, st, d_map, h->exp_max != 0);
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     if (cudaStreamBeginCapture((cudaStream_t)st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -734,10 +811,73 @@ static int read_status(const b200dd_pipeline *h, cudaStream_t st, bool sync, int
 }
 
 // A CPI whose clutter-filter solve failed publishes nothing after the filter: the reference skips the rest of it,
-// `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273).
-static int filter_failed(const char *msg) {
-  set_last_error(msg);
+// `if (!filter->process(x, y)) continue;` (blah2.cpp:270-273).  Fetch `entry` of stage `s` says so.
+static int filter_failed(const char *entry, Stage s) {
+  set_last_error(std::string(entry) + ": the CPI's clutter-filter solve failed; " + kStageSkipped[s]);
   return B200DD_FILTER_FAILED;
+}
+
+static bool stage_on(const b200dd_pipeline *h, Stage s) {
+  const Stateful &st = stateful(h);
+  switch (s) {
+    case kIq: return h->ij;
+    case kMap: return h->mj;
+    case kMaxhold: return st.mh;
+    case kDet: return h->dj;
+    case kTrack: return st.tr;
+    case kTiming: return h->tm_on && st.tm;
+    default: return h->spec;
+  }
+}
+
+// The checks a fetch `entry` of stage `s` starts with: *n_bytes (nullable) zeroed, then B200DD_ERR_ARG for a null
+// argument, a stage not enabled and, given `st`, no CPI submitted since the stage was enabled; *st is that CPI's
+// stream.  The stashes and the spectrum pass no `st`: they do not need a CPI.
+static int fetch_check(const b200dd_pipeline *h, const char *entry, Stage s, const void *out, size_t *n_bytes,
+                       cudaStream_t *st = nullptr) {
+  if (n_bytes) *n_bytes = 0;
+  if (!h || !out) return entry_fail(entry, "null argument");
+  if (!stage_on(h, s)) return entry_fail(entry, std::string("the ") + kStageName[s] + " stage is not enabled");
+  if (!st) return B200DD_OK;
+  if (!(h->last.stages & stage_bit(s))) return entry_fail(entry, "no CPI submitted since the stage was enabled");
+  *st = (cudaStream_t)h->last.stream;
+  return B200DD_OK;
+}
+
+// A share set's stage `s` takes the members' CPIs in set order: B200DD_ERR_ARG when it has taken a later one than
+// the member's last.  Outside a share set both numbers are -1.
+static int taken_later(const b200dd_pipeline *h, const char *entry, Stage s) {
+  if (h->last.cpi >= stateful(h).last[s]) return B200DD_OK;
+  return entry_fail(entry, std::string("the share set's ") + (s == kTrack ? "tracker" : "history") +
+                               " has taken a later CPI");
+}
+
+// The last CPI's verdict for fetch `entry` of stage `s`, read on `st` with the host waiting: B200DD_FILTER_FAILED when
+// its clutter-filter solve failed and, given its detection list `l`, B200DD_ERR_CAPACITY when CFAR found more
+// detections than the list holds (every stage after CFAR worked on a truncated list, as b200dd_pipeline_fetch
+// reports).  Either verdict drops the CPI's detection or IQ-data document.
+static int cpi_verdict(b200dd_pipeline *h, const char *entry, Stage s, cudaStream_t st,
+                       const DetDeviceList *l = nullptr) {
+  int fs;
+  uint32_t cfar = 0;
+  int rc = read_status(h, st, true, &fs, l, &cfar);
+  if (rc != B200DD_OK) return rc;
+  if (fs != 0) {
+    rc = filter_failed(entry, s);
+  } else if (l && cfar > l->cap) {
+    set_last_error(std::string(entry) + ": more CFAR detections than the list capacity (2^18)");
+    rc = B200DD_ERR_CAPACITY;
+  }
+  if (rc != B200DD_OK && s == kDet) detjson_mark_rendered(h->dj, false);
+  if (rc != B200DD_OK && s == kIq) iqjson_mark_rendered(h->ij, false);
+  return rc;
+}
+
+// A stash fetch of stage `s` runs on the last CPI's stream when one was submitted since the stage was enabled, else
+// on the pipeline's; in a share set, after the set's previous operation.
+static int stash_stream(b200dd_pipeline *h, Stage s, cudaStream_t *st) {
+  *st = h->last.stages & stage_bit(s) ? (cudaStream_t)h->last.stream : (cudaStream_t)h->stream;
+  return h->set ? set_wait(h->set, *st) : B200DD_OK;
 }
 
 // b200dd_pipeline_fetch of a share-set member: its CPI must be the set's oldest unfetched one; it enters the
@@ -749,10 +889,10 @@ static int member_fetch(b200dd_pipeline *h) {
   for (const b200dd_pipeline *m : s->members)
     if (m != h && m->last.unfetched && m->last.cpi < c.cpi)
       return arg_fail("b200dd_pipeline_fetch: an older CPI of the share set is not fetched yet (fetch in submit order)");
-  if (s->mh) {
-    const int rc = set_ordered(s, c.stream, [&] { return maxhold_push(h, s->mh, c.map, c.stream); });
+  if (s->st.mh) {
+    const int rc = set_ordered(s, c.stream, [&] { return maxhold_push(h, s->st.mh, c.map, c.stream); });
     if (rc != B200DD_OK) return rc;
-    s->mh_last = c.cpi;
+    s->st.last[kMaxhold] = c.cpi;
   }
   c.unfetched = false;
   return B200DD_OK;
@@ -794,17 +934,19 @@ int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double 
   return rc;
 }
 
-// A host submit's sample counts, checked in this order: the clutter filter and the CAF read *need samples of x and
-// y, and the spectrum reads nfft <= n_samples samples of x (SpectrumAnalyser.cpp:36-39), so *need_x of x are copied.
-static int host_counts(const b200dd_pipeline *h, uint32_t n, uint32_t *need, uint32_t *need_x, const char *count_msg,
-                       const char *member_msg, const char *nfft_msg) {
+// The start of host submit `entry` (submit_start, on the pipeline's stream) and its sample counts, checked in this
+// order: the clutter filter and the CAF read *need samples of x and y, and the spectrum reads nfft <= n_samples
+// samples of x (SpectrumAnalyser.cpp:36-39), so *need_x of x are copied.
+static int host_start(const b200dd_pipeline *h, const char *entry, bool args, uint32_t n, uint32_t *need,
+                      uint32_t *need_x) {
+  cudaStream_t st;
+  const int rc = submit_start(h, entry, args, nullptr, &st);
+  if (rc != B200DD_OK) return rc;
   const uint32_t N = h->p.caf.n_samples;
   *need = *need_x = h->wh ? N : h->g.n_used;
-  if (h->wh ? (n != N) : (n < *need)) return arg_fail(count_msg);
-  const int rc = member_may_submit(h, member_msg);
-  if (rc != B200DD_OK) return rc;
+  if (h->wh ? (n != N) : (n < *need)) return entry_fail(entry, "wrong number of samples");
   if (h->spec && h->spec_nfft > *need) {
-    if (n < h->spec_nfft) return arg_fail(nfft_msg);
+    if (n < h->spec_nfft) return entry_fail(entry, "the spectrum stage needs nfft samples");
     *need_x = h->spec_nfft;
   }
   return B200DD_OK;
@@ -834,16 +976,13 @@ static int host_submitted(b200dd_pipeline *h, int path, double *map_out) {
     B2_LAUNCH_CHECK();
     B2_CUDA(cudaMemcpyAsync(map_out, h->d_mapd, sizeof(double2) * cells, cudaMemcpyDeviceToHost, h->stream));
   }
-  pipeline_submitted(h, path, h->stream, h->d_map);
+  pipeline_submitted(h, path, h->stream, h->d_map, h->exp_max != 0);
   return B200DD_OK;
 }
 
 int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const double *y, uint32_t n, double *map_out) {
-  if (!h || !x || !y) return arg_fail("b200dd_pipeline_submit_host: null argument");
   uint32_t need, need_x;
-  int rc = host_counts(h, n, &need, &need_x, "b200dd_pipeline_submit_host: wrong number of samples",
-                       "b200dd_pipeline_submit_host: the share-set member's last CPI is not fetched yet",
-                       "b200dd_pipeline_submit_host: the spectrum stage needs nfft samples");
+  int rc = host_start(h, "b200dd_pipeline_submit_host", h && x && y, n, &need, &need_x);
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
   cudaStream_t st = h->stream;
@@ -877,18 +1016,15 @@ int b200dd_pipeline_submit_host(b200dd_pipeline *h, const double *x, const doubl
 
 }  // extern "C"
 
-// A host submit of capture-driver samples (int16, int8 or complex64, all exact in float32): the counts, the staging
-// and the stamp that opens extract_buffer, then ingest(need_x) -- the H2D copy of need_x instants of x and y and any
-// conversion into the complex64 d_xf, d_yf2 -- and the device chain on those, whose first stamp closes extract_buffer.
-// The CAF consumes n_used of the need_x instants.
+// A host submit of capture-driver samples (int16, int8 or complex64, all exact in float32; `args`: none is null):
+// the start and counts, the staging and the stamp that opens extract_buffer, then ingest(need_x) -- the H2D copy of
+// need_x instants of x and y and any conversion into the complex64 d_xf, d_yf2 -- and the device chain on those,
+// whose first stamp closes extract_buffer.  The CAF consumes n_used of the need_x instants.
 template <class Ingest>
-static int host_ingest(b200dd_pipeline *h, const char *entry, HostFormat fmt, uint32_t n, double *map_out,
+static int host_ingest(b200dd_pipeline *h, const char *entry, bool args, HostFormat fmt, uint32_t n, double *map_out,
                        Ingest ingest) {
-  const std::string e = entry;
   uint32_t need, need_x;
-  int rc = host_counts(h, n, &need, &need_x, (e + ": wrong number of samples").c_str(),
-                       (e + ": the share-set member's last CPI is not fetched yet").c_str(),
-                       (e + ": the spectrum stage needs nfft samples").c_str());
+  int rc = host_start(h, entry, args, n, &need, &need_x);
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
   rc = host_staging(h, fmt, map_out != nullptr);
@@ -902,8 +1038,7 @@ static int host_ingest(b200dd_pipeline *h, const char *entry, HostFormat fmt, ui
 extern "C" {
 
 int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, uint32_t n, double *map_out) {
-  if (!h || !iq) return arg_fail("b200dd_pipeline_submit_host_rspduo: null argument");
-  return host_ingest(h, "b200dd_pipeline_submit_host_rspduo", kInt16, n, map_out, [&](uint32_t m) -> int {
+  return host_ingest(h, "b200dd_pipeline_submit_host_rspduo", h && iq, kInt16, n, map_out, [&](uint32_t m) -> int {
     B2_CUDA(cudaMemcpyAsync(h->d_iq16, iq, sizeof(short4) * m, cudaMemcpyHostToDevice, h->stream));
     pl_ingest_rspduo_kernel<<<grid_for(m), 256, 0, h->stream>>>(h->d_iq16, h->d_xf, h->d_yf2, m);
     B2_LAUNCH_CHECK();
@@ -913,8 +1048,8 @@ int b200dd_pipeline_submit_host_rspduo(b200dd_pipeline *h, const int16_t *iq, ui
 
 int b200dd_pipeline_submit_host_ci8(b200dd_pipeline *h, const int8_t *x_iq, const int8_t *y_iq, uint32_t n,
                                     double *map_out) {
-  if (!h || !x_iq || !y_iq) return arg_fail("b200dd_pipeline_submit_host_ci8: null argument");
-  return host_ingest(h, "b200dd_pipeline_submit_host_ci8", kCi8, n, map_out, [&](uint32_t m) -> int {
+  const bool args = h && x_iq && y_iq;
+  return host_ingest(h, "b200dd_pipeline_submit_host_ci8", args, kCi8, n, map_out, [&](uint32_t m) -> int {
     B2_CUDA(cudaMemcpyAsync(h->d_x8, x_iq, 2 * (size_t)m, cudaMemcpyHostToDevice, h->stream));
     B2_CUDA(cudaMemcpyAsync(h->d_y8, y_iq, 2 * (size_t)m, cudaMemcpyHostToDevice, h->stream));
     pl_ingest_ci8_kernel<<<grid_for(m / 4 + m % 4), 256, 0, h->stream>>>(h->d_x8, h->d_y8, h->d_xf, h->d_yf2, m);
@@ -925,9 +1060,9 @@ int b200dd_pipeline_submit_host_ci8(b200dd_pipeline *h, const int8_t *x_iq, cons
 
 int b200dd_pipeline_submit_host_cf32(b200dd_pipeline *h, const float *x_iq, const float *y_iq, uint32_t n,
                                      double *map_out) {
-  if (!h || !x_iq || !y_iq) return arg_fail("b200dd_pipeline_submit_host_cf32: null argument");
   // complex64 is the device chain's own format: the samples go straight into its buffers
-  return host_ingest(h, "b200dd_pipeline_submit_host_cf32", kCf32, n, map_out, [&](uint32_t m) -> int {
+  const bool args = h && x_iq && y_iq;
+  return host_ingest(h, "b200dd_pipeline_submit_host_cf32", args, kCf32, n, map_out, [&](uint32_t m) -> int {
     B2_CUDA(cudaMemcpyAsync(h->d_xf, x_iq, sizeof(float2) * m, cudaMemcpyHostToDevice, h->stream));
     B2_CUDA(cudaMemcpyAsync(h->d_yf2, y_iq, sizeof(float2) * m, cudaMemcpyHostToDevice, h->stream));
     return B200DD_OK;
@@ -955,11 +1090,11 @@ static int tracker_create(const b200dd_pipeline *h, b200dd_tracker **out) {
 
 int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32_t *n_spectrum) {
   if (!h) return arg_fail("b200dd_pipeline_enable_spectrum: null handle");
-  if (h->set && h->set->ij)
+  if (h->set && h->set->st.ij)
     return arg_fail("b200dd_pipeline_enable_spectrum: the member's share set keeps an IQ-data history of its spectra");
   DeviceGuard guard(h->device);
   // the IQ-data stage goes too: its bin count may change, it is enabled again after this
-  int rc = stage_reset(h, h->ij, b200dd_iqjson_destroy, kIqBit);
+  int rc = stage_reset(h, h->ij, b200dd_iqjson_destroy, kIq);
   if (rc != B200DD_OK) return rc;
   b200dd_spectrum_destroy(h->spec);
   h->spec = nullptr;
@@ -976,8 +1111,8 @@ int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32
 }
 
 int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectrum_out, uint32_t cap) {
-  if (!h || !spectrum_out) return arg_fail("b200dd_pipeline_fetch_spectrum: null argument");
-  if (!h->spec) return arg_fail("b200dd_pipeline_fetch_spectrum: the spectrum stage is not enabled");
+  const int rc = fetch_check(h, "b200dd_pipeline_fetch_spectrum", kSpectrum, spectrum_out, nullptr);
+  if (rc != B200DD_OK) return rc;
   if (cap < h->spec_bins) return arg_fail("b200dd_pipeline_fetch_spectrum: capacity too small");
   return b200dd_spectrum_fetch(h->spec, spectrum_out, h->stream);
 }
@@ -985,7 +1120,7 @@ int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectrum_out, uin
 int b200dd_pipeline_enable_map_json(b200dd_pipeline *h, size_t *max_bytes) {
   if (!h) return arg_fail("b200dd_pipeline_enable_map_json: null handle");
   DeviceGuard guard(h->device);
-  int rc = stage_reset(h, h->mj, b200dd_mapjson_destroy, kMapBit);
+  int rc = stage_reset(h, h->mj, b200dd_mapjson_destroy, kMap);
   if (rc == B200DD_OK)
     rc = b200dd_mapjson_create(h->g.n_doppler_bins, h->g.n_delay_bins, h->delay.data(), h->doppler.data(), h->p.caf.fs,
                                h->device, &h->mj);
@@ -995,48 +1130,43 @@ int b200dd_pipeline_enable_map_json(b200dd_pipeline *h, size_t *max_bytes) {
 }
 
 int b200dd_pipeline_fetch_map_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_map_json: null argument");
-  if (!h->mj) return arg_fail("b200dd_pipeline_fetch_map_json: the map JSON stage is not enabled");
-  if (!(h->last.stages & kMapBit)) return arg_fail("b200dd_pipeline_fetch_map_json: no CPI submitted since the stage was enabled");
-  DeviceGuard guard(h->device);
-  cudaStream_t st = (cudaStream_t)h->last.stream;
-  int fs;
-  const int rc = read_status(h, st, true, &fs);
+  const char *entry = "b200dd_pipeline_fetch_map_json";
+  cudaStream_t st;
+  int rc = fetch_check(h, entry, kMap, out, n_bytes, &st);
   if (rc != B200DD_OK) return rc;
-  if (fs != 0) return filter_failed("b200dd_pipeline_fetch_map_json: the CPI's clutter-filter solve failed; it has no map");
-  return b200dd_mapjson_fetch(h->mj, timestamp, out, cap, n_bytes, st);
+  DeviceGuard guard(h->device);
+  rc = cpi_verdict(h, entry, kMap, st);
+  return rc != B200DD_OK ? rc : b200dd_mapjson_fetch(h->mj, timestamp, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_enable_maxhold(b200dd_pipeline *h, size_t *max_bytes) {
   if (!h) return arg_fail("b200dd_pipeline_enable_maxhold: null handle");
   if (h->set) return arg_fail("b200dd_pipeline_enable_maxhold: a share-set member's stateful stages are the set's");
   DeviceGuard guard(h->device);
-  int rc = stage_reset(h, h->mh, b200dd_maxhold_destroy, kMaxholdBit);
-  if (rc == B200DD_OK) rc = maxhold_create(h, &h->mh);
+  int rc = stage_reset(h, h->own.mh, b200dd_maxhold_destroy, kMaxhold);
+  if (rc == B200DD_OK) rc = maxhold_create(h, &h->own.mh);
   if (rc != B200DD_OK) return rc;
-  if (max_bytes) *max_bytes = b200dd_maxhold_max_bytes(h->mh);
+  if (max_bytes) *max_bytes = b200dd_maxhold_max_bytes(h->own.mh);
   return B200DD_OK;
 }
 
 int b200dd_pipeline_fetch_maxhold(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_maxhold: null argument");
+  ShareSet *s = h ? h->set : nullptr;
+  cudaStream_t st = nullptr;
+  // a share-set member's CPI is checked against the set's window instead
+  int rc = fetch_check(h, "b200dd_pipeline_fetch_maxhold", kMaxhold, out, n_bytes, s ? nullptr : &st);
+  if (rc != B200DD_OK) return rc;
   const LastCpi &c = h->last;
-  ShareSet *s = h->set;
-  b200dd_maxhold *mh = s ? s->mh : h->mh;
-  if (!mh) return arg_fail("b200dd_pipeline_fetch_maxhold: the max-hold stage is not enabled");
-  if (s && (c.cpi < 0 || c.unfetched || c.cpi != s->mh_last))
+  if (s && (c.cpi < 0 || c.unfetched || c.cpi != s->st.last[kMaxhold]))
     return arg_fail("b200dd_pipeline_fetch_maxhold: the share-set member's CPI is not the last one the window took "
                     "(call after b200dd_pipeline_fetch, before the next CPI of the set is fetched)");
-  if (!s && !(c.stages & kMaxholdBit))
-    return arg_fail("b200dd_pipeline_fetch_maxhold: no CPI submitted since the stage was enabled");
   DeviceGuard guard(h->device);
   if (s) {
-    const int rc = set_wait(s, c.stream);
+    st = (cudaStream_t)c.stream;
+    rc = set_wait(s, st);
     if (rc != B200DD_OK) return rc;
   }
-  return b200dd_maxhold_fetch(mh, timestamp, out, cap, n_bytes, c.stream);
+  return b200dd_maxhold_fetch(stateful(h).mh, timestamp, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held, size_t *doc_bytes,
@@ -1047,7 +1177,7 @@ int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held,
   int rc = detjson_check_axes(h->delay.data(), h->g.n_delay_bins, h->doppler.data(), h->g.n_doppler_bins, h->p.caf.fs);
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  rc = stage_reset(h, h->dj, b200dd_detjson_destroy, kDetBit);
+  rc = stage_reset(h, h->dj, b200dd_detjson_destroy, kDet);
   if (rc != B200DD_OK) return rc;
   h->dj_max_held = max_held;
   rc = detjson_create(h, &h->dj);
@@ -1059,50 +1189,30 @@ int b200dd_pipeline_enable_detection_json(b200dd_pipeline *h, uint32_t max_held,
 
 int b200dd_pipeline_fetch_detection_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap,
                                          size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_detection_json: null argument");
-  if (!h->dj) return arg_fail("b200dd_pipeline_fetch_detection_json: the detection JSON stage is not enabled");
-  if (!(h->last.stages & kDetBit))
-    return arg_fail("b200dd_pipeline_fetch_detection_json: no CPI submitted since the stage was enabled");
-  DeviceGuard guard(h->device);
-  cudaStream_t st = (cudaStream_t)h->last.stream;
-  ShareSet *s = h->set;
-  if (s && h->last.cpi < s->dj_last)
-    return arg_fail("b200dd_pipeline_fetch_detection_json: the share set's history has taken a later CPI");
-  DetDeviceList l;
-  int rc = det_device_list(h->det, &l);
+  const char *entry = "b200dd_pipeline_fetch_detection_json";
+  cudaStream_t st;
+  int rc = fetch_check(h, entry, kDet, out, n_bytes, &st);
+  if (rc == B200DD_OK) rc = taken_later(h, entry, kDet);
   if (rc != B200DD_OK) return rc;
-  rc = set_ordered(s, st, [&]() -> int {
-    int fs;
-    uint32_t cfar;
-    const int rs = read_status(h, st, true, &fs, &l, &cfar);
-    if (rs != B200DD_OK) return rs;
-    if (fs != 0) {
-      detjson_mark_rendered(h->dj, false);
-      return filter_failed("b200dd_pipeline_fetch_detection_json: the CPI's clutter-filter solve failed; it has no detections");
-    }
-    if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
-      detjson_mark_rendered(h->dj, false);
-      set_last_error("b200dd_pipeline_fetch_detection_json: more CFAR detections than the list capacity (2^18)");
-      return B200DD_ERR_CAPACITY;
-    }
-    return b200dd_detjson_fetch(h->dj, timestamp, out, cap, n_bytes, st);
+  DeviceGuard guard(h->device);
+  DetDeviceList l;
+  rc = det_device_list(h->det, &l);
+  if (rc != B200DD_OK) return rc;
+  rc = set_ordered(h->set, st, [&]() -> int {
+    const int rv = cpi_verdict(h, entry, kDet, st, &l);
+    return rv != B200DD_OK ? rv : b200dd_detjson_fetch(h->dj, timestamp, out, cap, n_bytes, st);
   });
-  if (rc == B200DD_OK && s) s->dj_last = h->last.cpi;
+  if (rc == B200DD_OK) stateful(h).last[kDet] = h->last.cpi;
   return rc;
 }
 
 int b200dd_pipeline_fetch_detection_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_detection_stash: null argument");
-  if (!h->dj) return arg_fail("b200dd_pipeline_fetch_detection_stash: the detection JSON stage is not enabled");
+  int rc = fetch_check(h, "b200dd_pipeline_fetch_detection_stash", kDet, out, n_bytes);
+  if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  void *st = h->last.stages & kDetBit ? h->last.stream : (void *)h->stream;
-  if (h->set) {
-    const int rc = set_wait(h->set, st);
-    if (rc != B200DD_OK) return rc;
-  }
-  return b200dd_detjson_fetch_stash(h->dj, out, cap, n_bytes, st);
+  cudaStream_t st;
+  rc = stash_stream(h, kDet, &st);
+  return rc != B200DD_OK ? rc : b200dd_detjson_fetch_stash(h->dj, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_enable_tracker(b200dd_pipeline *h, const b200dd_tracker_params *params, uint32_t max_tracks,
@@ -1111,61 +1221,50 @@ int b200dd_pipeline_enable_tracker(b200dd_pipeline *h, const b200dd_tracker_para
   if (h->set) return arg_fail("b200dd_pipeline_enable_tracker: a share-set member's stateful stages are the set's");
   if (!h->p.detection_enable) return arg_fail("b200dd_pipeline_enable_tracker: detection is not enabled");
   DeviceGuard guard(h->device);
-  int rc = stage_reset(h, h->tr, b200dd_tracker_destroy, kTrackBit, false);  // it runs at fetch time, not in the chain
+  int rc = stage_reset(h, h->own.tr, b200dd_tracker_destroy, kTrack, false);  // it runs at fetch time, not in the chain
   if (rc != B200DD_OK) return rc;
   h->tr_params = *params;
   h->tr_params.cpi = h->g.cpi;  // ambiguity->get_cpi(), blah2.cpp:195
   h->tr_params.fs = h->p.caf.fs;
   h->tr_max_tracks = max_tracks;
   h->tr_max_history = max_history;
-  rc = tracker_create(h, &h->tr);
+  rc = tracker_create(h, &h->own.tr);
   if (rc != B200DD_OK) return rc;
-  if (max_bytes) *max_bytes = b200dd_tracker_max_bytes(h->tr);
+  if (max_bytes) *max_bytes = b200dd_tracker_max_bytes(h->own.tr);
   return B200DD_OK;
 }
 
 // the tracker update of the last CPI, once, then the document
-static int track_json(b200dd_pipeline *h, b200dd_tracker *tr, uint64_t timestamp, char *out, size_t cap,
+static int track_json(b200dd_pipeline *h, const char *entry, uint64_t timestamp, char *out, size_t cap,
                       size_t *n_bytes, cudaStream_t st) {
   LastCpi &c = h->last;
+  Stateful &sf = stateful(h);
   if (c.tr_pending) {
     DetDeviceList l;
     int rc = det_device_list(h->det, &l);
-    if (rc != B200DD_OK) return rc;
-    int fs;
-    uint32_t cfar;
-    rc = read_status(h, st, true, &fs, &l, &cfar);
-    if (rc != B200DD_OK) return rc;
-    if (fs != 0) return filter_failed("b200dd_pipeline_fetch_track_json: the CPI's clutter-filter solve failed; the tracker skips it");
-    if (cfar > l.cap) {  // as b200dd_pipeline_fetch: every stage after CFAR worked on a truncated list
-      c.tm_track = 2;  // the tracker did not run: its time is 0
-      set_last_error("b200dd_pipeline_fetch_track_json: more CFAR detections than the list capacity (2^18)");
-      return B200DD_ERR_CAPACITY;
-    }
-    rc = tm_stamp(h, kTmTracker0, st);
-    if (rc == B200DD_OK) rc = b200dd_tracker_process_device(tr, l.delay, l.doppler, l.snr, l.count, timestamp, st);
+    if (rc == B200DD_OK) rc = cpi_verdict(h, entry, kTrack, st, &l);
+    if (rc == B200DD_ERR_CAPACITY) c.tm_track = 2;  // the tracker did not run: its time is 0
+    if (rc == B200DD_OK) rc = tm_stamp(h, kTmTracker0, st);
+    if (rc == B200DD_OK) rc = b200dd_tracker_process_device(sf.tr, l.delay, l.doppler, l.snr, l.count, timestamp, st);
     if (rc == B200DD_OK) rc = tm_stamp(h, kTmTracker1, st);
     if (rc != B200DD_OK) return rc;
     c.tm_track = 1;
     c.tr_pending = false;
-    if (h->set) h->set->tr_last = c.cpi;
+    sf.last[kTrack] = c.cpi;
   }
-  return b200dd_tracker_fetch(tr, timestamp, out, cap, n_bytes, st);
+  return b200dd_tracker_fetch(sf.tr, timestamp, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_fetch_track_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_track_json: null argument");
-  ShareSet *s = h->set;
-  b200dd_tracker *tr = s ? s->tr : h->tr;
-  if (!tr) return arg_fail("b200dd_pipeline_fetch_track_json: the tracker stage is not enabled");
-  if (!(h->last.stages & kTrackBit))
-    return arg_fail("b200dd_pipeline_fetch_track_json: no CPI submitted since the stage was enabled");
-  if (s && h->last.unfetched) return arg_fail("b200dd_pipeline_fetch_track_json: the share-set member's CPI is not fetched yet");
-  if (s && h->last.cpi < s->tr_last) return arg_fail("b200dd_pipeline_fetch_track_json: the share set's tracker has taken a later CPI");
+  const char *entry = "b200dd_pipeline_fetch_track_json";
+  cudaStream_t st;
+  int rc = fetch_check(h, entry, kTrack, out, n_bytes, &st);
+  if (rc != B200DD_OK) return rc;
+  if (h->set && h->last.unfetched) return entry_fail(entry, "the share-set member's CPI is not fetched yet");
+  rc = taken_later(h, entry, kTrack);
+  if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  cudaStream_t st = (cudaStream_t)h->last.stream;
-  return set_ordered(s, st, [&] { return track_json(h, tr, timestamp, out, cap, n_bytes, st); });
+  return set_ordered(h->set, st, [&] { return track_json(h, entry, timestamp, out, cap, n_bytes, st); });
 }
 
 int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double max, double mean, size_t *doc_bytes,
@@ -1174,7 +1273,7 @@ int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double ma
   if (h->set) return arg_fail("b200dd_pipeline_enable_iqdata_json: a share-set member's stateful stages are the set's");
   if (!h->spec) return arg_fail("b200dd_pipeline_enable_iqdata_json: the spectrum stage is not enabled");
   DeviceGuard guard(h->device);
-  int rc = stage_reset(h, h->ij, b200dd_iqjson_destroy, kIqBit);
+  int rc = stage_reset(h, h->ij, b200dd_iqjson_destroy, kIq);
   if (rc != B200DD_OK) return rc;
   h->ij_metrics[0] = min;
   h->ij_metrics[1] = max;
@@ -1188,56 +1287,42 @@ int b200dd_pipeline_enable_iqdata_json(b200dd_pipeline *h, double min, double ma
 
 // the last CPI's IQ-data document, committed to the history
 int b200dd_pipeline_fetch_iqdata_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_iqdata_json: null argument");
-  if (!h->ij) return arg_fail("b200dd_pipeline_fetch_iqdata_json: the IQ-data JSON stage is not enabled");
-  if (!(h->last.stages & kIqBit))
-    return arg_fail("b200dd_pipeline_fetch_iqdata_json: no CPI submitted since the stage was enabled");
-  ShareSet *s = h->set;
-  if (s && h->last.cpi < s->ij_last)
-    return arg_fail("b200dd_pipeline_fetch_iqdata_json: the share set's history has taken a later CPI");
+  const char *entry = "b200dd_pipeline_fetch_iqdata_json";
+  cudaStream_t st;
+  int rc = fetch_check(h, entry, kIq, out, n_bytes, &st);
+  if (rc == B200DD_OK) rc = taken_later(h, entry, kIq);
+  if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  cudaStream_t st = (cudaStream_t)h->last.stream;
-  const int rc = set_ordered(s, st, [&]() -> int {
-    int fs;
-    const int rs = read_status(h, st, true, &fs);
-    if (rs != B200DD_OK) return rs;
-    if (fs != 0) {
-      iqjson_mark_rendered(h->ij, false);
-      return filter_failed("b200dd_pipeline_fetch_iqdata_json: the CPI's clutter-filter solve failed; it has no document");
-    }
-    return b200dd_iqjson_fetch(h->ij, timestamp, out, cap, n_bytes, st);
+  rc = set_ordered(h->set, st, [&]() -> int {
+    const int rv = cpi_verdict(h, entry, kIq, st);
+    return rv != B200DD_OK ? rv : b200dd_iqjson_fetch(h->ij, timestamp, out, cap, n_bytes, st);
   });
-  if (rc == B200DD_OK && s) s->ij_last = h->last.cpi;
+  if (rc == B200DD_OK) stateful(h).last[kIq] = h->last.cpi;
   return rc;
 }
 
 int b200dd_pipeline_fetch_iqdata_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_iqdata_stash: null argument");
-  if (!h->ij) return arg_fail("b200dd_pipeline_fetch_iqdata_stash: the IQ-data JSON stage is not enabled");
+  int rc = fetch_check(h, "b200dd_pipeline_fetch_iqdata_stash", kIq, out, n_bytes);
+  if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  void *st = h->last.stages & kIqBit ? h->last.stream : (void *)h->stream;
-  if (h->set) {
-    const int rc = set_wait(h->set, st);
-    if (rc != B200DD_OK) return rc;
-  }
-  return b200dd_iqjson_fetch_stash(h->ij, out, cap, n_bytes, st);
+  cudaStream_t st;
+  rc = stash_stream(h, kIq, &st);
+  return rc != B200DD_OK ? rc : b200dd_iqjson_fetch_stash(h->ij, out, cap, n_bytes, st);
 }
 
 int b200dd_pipeline_enable_timing_json(b200dd_pipeline *h, uint64_t t_start, size_t *doc_bytes, size_t *stash_bytes) {
   if (!h) return arg_fail("b200dd_pipeline_enable_timing_json: null handle");
   if (h->set) return arg_fail("b200dd_pipeline_enable_timing_json: a share-set member's stateful stages are the set's");
   DeviceGuard guard(h->device);
-  int rc = stage_reset(h, h->tm, timing_history_destroy, kTimingBit);
+  int rc = stage_reset(h, h->own.tm, timing_history_destroy, kTiming);
   if (rc != B200DD_OK) return rc;
   if (!h->d_tm) {
     B2_CUDA(h->d_tm.alloc(kTmSlots));
     B2_CUDA(cudaMemset(h->d_tm, 0, sizeof(uint64_t) * kTmSlots));
   }
   h->tm_t_start = t_start;
-  h->tm = timing_history_create(t_start);
-  if (!h->tm) return arg_fail("b200dd_pipeline_enable_timing_json: out of host memory");
+  h->own.tm = timing_history_create(t_start);
+  if (!h->own.tm) return arg_fail("b200dd_pipeline_enable_timing_json: out of host memory");
   h->tm_on = true;
   h->tm_names.clear();
   h->tm_values.clear();
@@ -1290,41 +1375,35 @@ static void timing_values(b200dd_pipeline *h, const uint64_t *t, bool tracker) {
 }
 
 int b200dd_pipeline_fetch_timing_json(b200dd_pipeline *h, uint64_t timestamp, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_timing_json: null argument");
-  ShareSet *s = h->set;
-  TimingHistory *tm = s ? s->tm : h->tm;
+  const char *entry = "b200dd_pipeline_fetch_timing_json";
+  cudaStream_t st;
+  int rc = fetch_check(h, entry, kTiming, out, n_bytes, &st);
+  if (rc != B200DD_OK) return rc;
   LastCpi &c = h->last;
-  if (!h->tm_on || !tm) return arg_fail("b200dd_pipeline_fetch_timing_json: the timing JSON stage is not enabled");
-  if (!(c.stages & kTimingBit)) return arg_fail("b200dd_pipeline_fetch_timing_json: no CPI submitted since the stage was enabled");
-  if (!c.tm_fetched) return arg_fail("b200dd_pipeline_fetch_timing_json: call after the CPI's b200dd_pipeline_fetch");
-  if (c.tm_done) return arg_fail("b200dd_pipeline_fetch_timing_json: the CPI's document was fetched already");
-  if (c.tm_fs != 0) return filter_failed("b200dd_pipeline_fetch_timing_json: the CPI's clutter-filter solve failed; it has no document");
-  const bool tracker = (s ? s->tr : h->tr) != nullptr;
-  if (tracker && c.tm_track == 0)
-    return arg_fail("b200dd_pipeline_fetch_timing_json: with the tracker enabled, call after the CPI's track fetch");
-  if (s && c.cpi < s->tm_last)
-    return arg_fail("b200dd_pipeline_fetch_timing_json: the share set's history has taken a later CPI");
+  Stateful &sf = stateful(h);
+  if (!c.tm_fetched) return entry_fail(entry, "call after the CPI's b200dd_pipeline_fetch");
+  if (c.tm_done) return entry_fail(entry, "the CPI's document was fetched already");
+  if (c.tm_fs != 0) return filter_failed(entry, kTiming);
+  if (sf.tr && c.tm_track == 0) return entry_fail(entry, "with the tracker enabled, call after the CPI's track fetch");
+  rc = taken_later(h, entry, kTiming);
+  if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
   uint64_t t[kTmSlots];
-  B2_CUDA(cudaMemcpyAsync(t, h->d_tm, sizeof(t), cudaMemcpyDeviceToHost, (cudaStream_t)c.stream));
-  B2_CUDA(cudaStreamSynchronize((cudaStream_t)c.stream));
-  timing_values(h, t, tracker);
-  const int rc = timing_history_fetch(tm, timestamp, h->tm_names.data(), h->tm_values.data(),
-                                      (uint32_t)h->tm_names.size(), out, cap, n_bytes);
+  B2_CUDA(cudaMemcpyAsync(t, h->d_tm, sizeof(t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  timing_values(h, t, sf.tr != nullptr);
+  rc = timing_history_fetch(sf.tm, timestamp, h->tm_names.data(), h->tm_values.data(), (uint32_t)h->tm_names.size(),
+                            out, cap, n_bytes);
   if (rc == B200DD_OK) {
     c.tm_done = true;
-    if (s) s->tm_last = c.cpi;
+    sf.last[kTiming] = c.cpi;
   }
   return rc;
 }
 
 int b200dd_pipeline_fetch_timing_stash(b200dd_pipeline *h, char *out, size_t cap, size_t *n_bytes) {
-  if (n_bytes) *n_bytes = 0;
-  if (!h || !out) return arg_fail("b200dd_pipeline_fetch_timing_stash: null argument");
-  const TimingHistory *tm = h->set ? h->set->tm : h->tm;
-  if (!h->tm_on || !tm) return arg_fail("b200dd_pipeline_fetch_timing_stash: the timing JSON stage is not enabled");
-  return timing_history_stash(tm, out, cap, n_bytes);
+  const int rc = fetch_check(h, "b200dd_pipeline_fetch_timing_stash", kTiming, out, n_bytes);
+  return rc != B200DD_OK ? rc : timing_history_stash(stateful(h).tm, out, cap, n_bytes);
 }
 
 int b200dd_pipeline_debug_timing_values(b200dd_pipeline *h, const char **names, double *values, uint32_t cap,
@@ -1381,20 +1460,20 @@ int b200dd_pipeline_export_record(b200dd_pipeline *h, const void **d_record) {
 }
 
 int b200dd_pipeline_submit_record(b200dd_pipeline *h, const void *d_record, const void *d_map) {
-  if (!h || !d_record || !d_map) return arg_fail("b200dd_pipeline_submit_record: null argument");
-  int rc = member_may_submit(h, "b200dd_pipeline_submit_record: the share-set member's last CPI is not fetched yet");
+  const char *entry = "b200dd_pipeline_submit_record";
+  cudaStream_t st;
+  int rc = submit_start(h, entry, h && d_record && d_map, nullptr, &st);
   if (rc != B200DD_OK) return rc;
   DeviceGuard guard(h->device);
-  cudaStream_t st = h->stream;
   RecHeader hd;
   B2_CUDA(cudaMemcpyAsync(&hd, d_record, sizeof(hd), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
-  if (hd.version != kRecVersion) return arg_fail("b200dd_pipeline_submit_record: not a CPI record of this version");
+  if (hd.version != kRecVersion) return entry_fail(entry, "not a CPI record of this version");
   if (hd.max_detections == 0 || hd.max_detections > kRecMaxDetections || hd.path < kTmHost || hd.path > kTmDevice)
-    return arg_fail("b200dd_pipeline_submit_record: not a CPI record");
+    return entry_fail(entry, "not a CPI record");
   const RecordLayout L = record_layout(h, hd.max_detections);
   if (hd.bytes != L.bytes || hd.fingerprint != record_fingerprint(h, L))
-    return arg_fail("b200dd_pipeline_submit_record: the record comes from a pipeline of other parameters or stages");
+    return entry_fail(entry, "the record comes from a pipeline of other parameters or stages");
   det_adopt_chain(h->det, h->p.detection_enable ? B200DD_DET_INTERPOLATE : 0);
   RecordArgs a;
   rc = record_args(h, d_record, L, hd.fingerprint, (int)hd.path, &a);
@@ -1405,36 +1484,33 @@ int b200dd_pipeline_submit_record(b200dd_pipeline *h, const void *d_record, cons
   if (h->ij) rc = b200dd_iqjson_render_device(h->ij, spectrum_device_output(h->spec), st);
   if (rc == B200DD_OK) rc = pipeline_enqueue_products(h, (float2 *)const_cast<void *>(d_map), st);
   if (rc != B200DD_OK) return rc;
-  pipeline_submitted(h, (int)hd.path, st, d_map);
-  h->exp_valid = false;  // the import packed nothing
+  pipeline_submitted(h, (int)hd.path, st, d_map, false);
   return B200DD_OK;
 }
 
 int b200dd_pipeline_stamp(b200dd_pipeline *h, int slot, void *stream) {
   if (!h) return arg_fail("b200dd_pipeline_stamp: null handle");
-  static const int slots[] = {kTmChain, kTmSpectrum, kTmClutter};  // B200DD_STAMP_CHAIN, _SPECTRUM, _CLUTTER
   if (slot < B200DD_STAMP_CHAIN || slot > B200DD_STAMP_CLUTTER) return arg_fail("b200dd_pipeline_stamp: not a boundary slot");
   if (!h->tm_on) return B200DD_OK;
   DeviceGuard guard(h->device);
-  const int rc = tm_stamp(h, slots[slot], stream ? stream : (void *)h->stream);
+  const int rc = tm_stamp(h, kStampSlots[slot], stream_or(stream, h->stream));
   if (rc == B200DD_OK) h->tm_pre |= 1u << slot;
   return rc;
 }
 
 int b200dd_pipeline_submit_map(b200dd_pipeline *h, const void *d_map, const int *d_filter_status,
                                const void *d_spectrum_parts, uint32_t n_parts, void *stream) {
-  if (!h || !d_map) return arg_fail("b200dd_pipeline_submit_map: null argument");
-  if (!h->wh != !d_filter_status)
-    return arg_fail("b200dd_pipeline_submit_map: a clutter-filter status is required iff the clutter filter is enabled");
-  if (h->spec ? (!d_spectrum_parts || n_parts == 0) : (d_spectrum_parts || n_parts))
-    return arg_fail("b200dd_pipeline_submit_map: spectrum parts are required iff the spectrum stage is enabled");
-  int rc = member_may_submit(h, "b200dd_pipeline_submit_map: the share-set member's last CPI is not fetched yet");
+  const char *entry = "b200dd_pipeline_submit_map";
+  cudaStream_t st;
+  int rc = submit_start(h, entry, h && d_map, stream, &st);
   if (rc != B200DD_OK) return rc;
+  if (!h->wh != !d_filter_status)
+    return entry_fail(entry, "a clutter-filter status is required iff the clutter filter is enabled");
+  if (h->spec ? (!d_spectrum_parts || n_parts == 0) : (d_spectrum_parts || n_parts))
+    return entry_fail(entry, "spectrum parts are required iff the spectrum stage is enabled");
   DeviceGuard guard(h->device);
-  void *st = stream ? stream : (void *)h->stream;
-  static const int slots[] = {kTmChain, kTmSpectrum, kTmClutter};
-  for (int i = 0; i < 3 && rc == B200DD_OK; i++)
-    if (!(h->tm_pre & (1u << i))) rc = tm_stamp(h, slots[i], st);
+  for (int i = B200DD_STAMP_CHAIN; i <= B200DD_STAMP_CLUTTER && rc == B200DD_OK; i++)
+    if (!(h->tm_pre & (1u << i))) rc = tm_stamp(h, kStampSlots[i], st);
   if (rc == B200DD_OK && h->spec) {
     rc = b200dd_spectrum_finish_device(h->spec, d_spectrum_parts, n_parts, nullptr, st);
     if (rc == B200DD_OK && h->ij) rc = b200dd_iqjson_render_device(h->ij, spectrum_device_output(h->spec), st);
@@ -1442,54 +1518,16 @@ int b200dd_pipeline_submit_map(b200dd_pipeline *h, const void *d_map, const int 
   if (rc != B200DD_OK) return rc;
   if (h->wh)
     B2_CUDA(cudaMemcpyAsync(const_cast<int *>(b200dd_wh_device_status(h->wh)), d_filter_status, sizeof(int),
-                            cudaMemcpyDeviceToDevice, (cudaStream_t)st));
+                            cudaMemcpyDeviceToDevice, st));
   rc = pipeline_enqueue_after_map(h, (float2 *)const_cast<void *>(d_map), st);
   if (rc != B200DD_OK) return rc;
-  pipeline_submitted(h, kTmDevice, st, d_map);
-  h->exp_valid = false;  // nothing was packed
+  pipeline_submitted(h, kTmDevice, st, d_map, false);
   return B200DD_OK;
-}
-
-
-static bool same_params(const b200dd_pipeline *a, const b200dd_pipeline *b) {
-  const b200dd_caf_params &c = a->p.caf, &e = b->p.caf;  // devices compared as resolved at create
-  const b200dd_det_params &d = a->p.det, &f = b->p.det;
-  return c.delay_min == e.delay_min && c.delay_max == e.delay_max && c.doppler_min == e.doppler_min &&
-         c.doppler_max == e.doppler_max && c.fs == e.fs && c.n_samples == e.n_samples &&
-         c.round_hamming == e.round_hamming && a->p.clutter_enable == b->p.clutter_enable &&
-         a->p.clutter_delay_min == b->p.clutter_delay_min && a->p.clutter_delay_max == b->p.clutter_delay_max &&
-         a->p.detection_enable == b->p.detection_enable && d.pfa == f.pfa && d.n_guard == f.n_guard &&
-         d.n_train == f.n_train && d.min_delay == f.min_delay && d.min_doppler == f.min_doppler &&
-         d.n_centroid_delay == f.n_centroid_delay && d.n_centroid_doppler == f.n_centroid_doppler &&
-         d.resolution_doppler == f.resolution_doppler && d.interp_delay == f.interp_delay &&
-         d.interp_doppler == f.interp_doppler;
-}
-
-// the spectrum and the four stateful stages are enabled alike, with the same parameters
-static bool same_stages(const b200dd_pipeline *a, const b200dd_pipeline *b) {
-  if (!a->spec != !b->spec || !a->ij != !b->ij || !a->mh != !b->mh || !a->dj != !b->dj || !a->tr != !b->tr) return false;
-  if (a->spec && a->spec_bandwidth != b->spec_bandwidth) return false;
-  if (a->ij && (a->ij_metrics[0] != b->ij_metrics[0] || a->ij_metrics[1] != b->ij_metrics[1] ||
-                a->ij_metrics[2] != b->ij_metrics[2]))
-    return false;
-  if (a->dj && a->dj_max_held != b->dj_max_held) return false;
-  if (a->tm_on != b->tm_on || (a->tm_on && a->tm_t_start != b->tm_t_start)) return false;
-  if (a->tr) {
-    const b200dd_tracker_params &t = a->tr_params, &u = b->tr_params;
-    if (t.m != u.m || t.n != u.n || t.n_delete != u.n_delete || t.cpi != u.cpi || t.max_acc_init != u.max_acc_init ||
-        t.fs != u.fs || t.fc != u.fc || a->tr_max_tracks != b->tr_max_tracks || a->tr_max_history != b->tr_max_history)
-      return false;
-  }
-  return true;
 }
 
 static void set_free(ShareSet *s) {
   DeviceGuard guard(s->device);
-  b200dd_maxhold_destroy(s->mh);
-  b200dd_detjson_destroy(s->dj);
-  b200dd_iqjson_destroy(s->ij);
-  b200dd_tracker_destroy(s->tr);
-  timing_history_destroy(s->tm);
+  stateful_free(s->st);
   delete s;  // under the guard: the event goes with it
 }
 
@@ -1511,8 +1549,11 @@ int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
       if (members[j] == m) return arg_fail("b200dd_pipeline_share_history: a pipeline is given twice");
     if (m->set) return arg_fail("b200dd_pipeline_share_history: a pipeline is in a share set already");
     if (m->device != members[0]->device) return arg_fail("b200dd_pipeline_share_history: members on different devices");
-    if (!same_params(m, members[0])) return arg_fail("b200dd_pipeline_share_history: the members' parameters differ");
-    if (!same_stages(m, members[0]))
+    ParamValues a, b;
+    visit_params(m, a);
+    visit_params(members[0], b);
+    if (a.params != b.params) return arg_fail("b200dd_pipeline_share_history: the members' parameters differ");
+    if (a.stages != b.stages)
       return arg_fail("b200dd_pipeline_share_history: the members' spectrum or stateful stages differ");
   }
   b200dd_pipeline *h0 = members[0];
@@ -1522,11 +1563,12 @@ int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
   set->device = h0->device;
   for (uint32_t i = 0; i < n; i++) B2_CUDA(cudaStreamSynchronize(members[i]->stream));
   B2_CUDA(set->ev.create(cudaEventDisableTiming));
-  int rc = h0->mh ? maxhold_create(h0, &set->mh) : B200DD_OK;
-  if (rc == B200DD_OK && h0->dj) rc = detjson_create(h0, &set->dj);
-  if (rc == B200DD_OK && h0->ij) rc = iqjson_create(h0, &set->ij);
-  if (rc == B200DD_OK && h0->tr) rc = tracker_create(h0, &set->tr);
-  if (rc == B200DD_OK && h0->tm_on && !(set->tm = timing_history_create(h0->tm_t_start)))
+  Stateful &st = set->st;
+  int rc = h0->own.mh ? maxhold_create(h0, &st.mh) : B200DD_OK;
+  if (rc == B200DD_OK && h0->dj) rc = detjson_create(h0, &st.dj);
+  if (rc == B200DD_OK && h0->ij) rc = iqjson_create(h0, &st.ij);
+  if (rc == B200DD_OK && h0->own.tr) rc = tracker_create(h0, &st.tr);
+  if (rc == B200DD_OK && h0->tm_on && !(st.tm = timing_history_create(h0->tm_t_start)))
     rc = arg_fail("b200dd_pipeline_share_history: out of host memory");
   if (rc != B200DD_OK) return rc;
   ShareSet *s = set.release();
@@ -1534,16 +1576,11 @@ int b200dd_pipeline_share_history(b200dd_pipeline *const *members, uint32_t n) {
   int first = B200DD_OK;  // only a CUDA error can fail here; every member joins all the same
   for (uint32_t i = 0; i < n; i++) {
     b200dd_pipeline *m = members[i];
-    int r = m->dj ? detjson_share(m->dj, s->dj) : B200DD_OK;
-    if (r == B200DD_OK && m->ij) r = iqjson_share(m->ij, s->ij);
+    int r = m->dj ? detjson_share(m->dj, s->st.dj) : B200DD_OK;
+    if (r == B200DD_OK && m->ij) r = iqjson_share(m->ij, s->st.ij);
     if (first == B200DD_OK) first = r;
     pipeline_drop_graphs(m);  // they record the window's push
-    b200dd_maxhold_destroy(m->mh);
-    m->mh = nullptr;
-    b200dd_tracker_destroy(m->tr);
-    m->tr = nullptr;
-    timing_history_destroy(m->tm);
-    m->tm = nullptr;
+    stateful_free(m->own);
     m->last.stages &= ~kShareBits;
     m->last.cpi = -1;
     m->last.unfetched = false;

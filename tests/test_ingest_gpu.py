@@ -5,7 +5,6 @@ are read as int8 as blah2's Kraken source reads them; b200dd_pipeline_submit_hos
 same complex64 samples bit for bit and the complex128 entry to FP32 accuracy.  Odd lengths, misaligned and pinned host
 buffers, a wrong count, a failed clutter-filter solve and a share set behave as on the other entries."""
 import json
-import struct
 
 import numpy as np
 import pytest
@@ -14,6 +13,7 @@ import bench
 from blah2_b200 import capi
 from blah2_b200.process import Pipeline
 from blah2_b200.scene import Target, make_scene
+from cpi_products import code, cpi_products
 
 pytestmark = pytest.mark.gpu
 
@@ -61,13 +61,6 @@ def _int16(x, y):
     return iq
 
 
-def _code(f):
-    try:
-        return f()
-    except capi.B200ddError as e:
-        return e.code
-
-
 def _timing_shape(doc):
     """A timing document without its stage times, which come from the clock: its keys in order and the values
     that do not (timestamp, nCpi, uptime)."""
@@ -85,23 +78,11 @@ def _stash_shape(doc):
 
 
 def _products(pipe, ts):
-    """fetch() of the CPI, then every product of it in the order blah2's process thread sends them."""
-    r = pipe.fetch()
-    d = r["detections"]
-    rec = {"fetch": (r["skipped"], struct.pack("<2d", r["noisePower"], r["maxPower"]), d.delay.tobytes(),
-                     d.doppler.tobytes(), d.snr.tobytes()),
-           "n_detections": d.get_nDetections()}
-    for name, f in (("map", lambda: pipe.fetch_map_json(ts)),
-                    ("spectrum", lambda: pipe.fetch_spectrum().tobytes()),
-                    ("maxhold", lambda: pipe.fetch_maxhold(ts)),
-                    ("detection", lambda: pipe.fetch_detection_json(ts)),
-                    ("detection_stash", pipe.fetch_detection_stash),
-                    ("iqdata", lambda: pipe.fetch_iqdata_json(ts)),
-                    ("iqdata_stash", pipe.fetch_iqdata_stash),
-                    ("track", lambda: pipe.fetch_track_json(ts))):
-        rec[name] = _code(f)
-    rec["timing"] = _timing_shape(_code(lambda: pipe.fetch_timing_json(ts)))
-    rec["timing_stash"] = _stash_shape(_code(pipe.fetch_timing_stash))
+    """cpi_products as a dict, with the detection count, then the timing document's and stash's shapes."""
+    rec = dict(cpi_products(pipe, ts))
+    rec["n_detections"] = len(rec["fetch"][2]) // 8
+    rec["timing"] = _timing_shape(code(lambda: pipe.fetch_timing_json(ts)))
+    rec["timing_stash"] = _stash_shape(code(pipe.fetch_timing_stash))
     return rec
 
 

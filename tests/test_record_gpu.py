@@ -12,6 +12,7 @@ import pytest
 
 from blah2_b200 import capi
 from blah2_b200.process import Pipeline, record_bytes, timing_render_host
+from cpi_products import code, cpi_products
 
 pytestmark = pytest.mark.gpu
 
@@ -93,13 +94,6 @@ def _map_buf(p):
     return torch.empty((g.n_doppler_bins, g.n_delay_bins), dtype=torch.complex64, device="cuda")
 
 
-def _code(f):
-    try:
-        return f()
-    except capi.B200ddError as e:
-        return e.code
-
-
 def _raw_fetch(p):
     """b200dd_pipeline_fetch's return code and results (Pipeline.fetch accepts ERR_CAPACITY silently)."""
     res = capi.CpiResult()
@@ -114,19 +108,10 @@ def _products(p, i, timing=True):
     """CPI i's fetch and then every product, in blah2's order; the timing document is checked against the stand-alone
     render of its names and values and returned as (names, values) instead of bytes."""
     ts = _ts(i)
-    out = [("fetch", _raw_fetch(p))]
-    for name, f in (("map", lambda: p.fetch_map_json(ts)),
-                    ("spectrum", lambda: p.fetch_spectrum().tobytes()),
-                    ("maxhold", lambda: p.fetch_maxhold(ts)),
-                    ("detection", lambda: p.fetch_detection_json(ts)),
-                    ("detection_stash", p.fetch_detection_stash),
-                    ("iqdata", lambda: p.fetch_iqdata_json(ts)),
-                    ("iqdata_stash", p.fetch_iqdata_stash),
-                    ("track", lambda: p.fetch_track_json(ts))):
-        out.append((name, _code(f)))
+    out = cpi_products(p, ts, fetch=_raw_fetch)
     tm = None
     if timing:
-        doc = _code(lambda: p.fetch_timing_json(ts))
+        doc = code(lambda: p.fetch_timing_json(ts))
         if isinstance(doc, bytes):
             names, values = p.timing_values()
             n_cpi = json.loads(doc)["nCpi"]
@@ -173,7 +158,7 @@ def _export_all(geom, k):
         maps.append(m.clone())
         torch.cuda.synchronize()
         e.fetch()
-        doc = _code(lambda: e.fetch_timing_json(_ts(i)))
+        doc = code(lambda: e.fetch_timing_json(_ts(i)))
         tms.append(dict(zip(*e.timing_values())) if isinstance(doc, bytes) else doc)
     for j, e in enumerate(exps):
         x, y = scenes[j]
@@ -400,7 +385,7 @@ def test_mismatched_records_are_refused():
             q.submit_record(e.export_record(), m)
         assert ei.value.code == capi.ERR_ARG
     # nothing was taken: the importer has no CPI to fetch
-    assert _code(lambda: q.fetch_map_json(0)) == capi.ERR_ARG
+    assert code(lambda: q.fetch_map_json(0)) == capi.ERR_ARG
     # a buffer that is not a record
     junk = torch.zeros(4096, dtype=torch.uint8, device="cuda")
     with pytest.raises(capi.B200ddError):

@@ -3,7 +3,6 @@ and one tracker.  After every fetch, with P members taking CPIs round-robin, eve
 every per-CPI product -- equals that of one unshared pipeline given the same CPIs one after another, on every submit
 path; the same alternation without sharing does not; misuse is refused without consuming or committing anything."""
 import ctypes as C
-import struct
 
 import numpy as np
 import pytest
@@ -11,6 +10,7 @@ import pytest
 from blah2_b200 import capi
 from blah2_b200.process import Pipeline
 from blah2_b200.scene import Target, make_scene
+from cpi_products import cpi_products
 
 pytestmark = pytest.mark.gpu
 
@@ -100,32 +100,6 @@ class Feeder:
                 pipe.submit_device(dx, dy, dm)
 
 
-def _code(f):
-    try:
-        return f()
-    except capi.B200ddError as e:
-        return e.code
-
-
-def _products(pipe, i):
-    """fetch() of CPI i and then every product of it, as one pipeline of the blah2 process thread would send them."""
-    ts = _ts(i)
-    r = pipe.fetch()
-    d = r["detections"]
-    rec = [("fetch", r["skipped"], struct.pack("<2d", r["noisePower"], r["maxPower"]), d.delay.tobytes(),
-            d.doppler.tobytes(), d.snr.tobytes())]
-    for name, f in (("map", lambda: pipe.fetch_map_json(ts)),
-                    ("spectrum", lambda: pipe.fetch_spectrum().tobytes()),
-                    ("maxhold", lambda: pipe.fetch_maxhold(ts)),
-                    ("detection", lambda: pipe.fetch_detection_json(ts)),
-                    ("detection_stash", pipe.fetch_detection_stash),
-                    ("iqdata", lambda: pipe.fetch_iqdata_json(ts)),
-                    ("iqdata_stash", pipe.fetch_iqdata_stash),
-                    ("track", lambda: pipe.fetch_track_json(ts))):
-        rec.append((name, _code(f)))
-    return rec
-
-
 _REFS = {}
 
 
@@ -138,7 +112,7 @@ def _reference(config, path):
         out = []
         for k in range(N_CPI):
             feed.submit(pipe, k)
-            out.append(_products(pipe, k))
+            out.append(cpi_products(pipe, _ts(k)))
         pipe.close()
         _REFS[key] = out
     return _REFS[key]
@@ -153,9 +127,9 @@ def _alternate(pipes, feed, ks, out, between=None):
             between(n, k)
         if n - P + 1 >= 0:
             j = n - P + 1
-            out[ks[j]] = _products(pipes[j % P], ks[j])
+            out[ks[j]] = cpi_products(pipes[j % P], _ts(ks[j]))
     for j in range(max(len(ks) - P + 1, 0), len(ks)):
-        out[ks[j]] = _products(pipes[j % P], ks[j])
+        out[ks[j]] = cpi_products(pipes[j % P], _ts(ks[j]))
 
 
 def _assert_same(got, ref):
@@ -168,7 +142,7 @@ def test_sequence_exercises_every_case():
     for config in ("filtered", "direct"):
         ref = _reference(config, "submit_host")
         rec = dict((name, v) for name, v, *_ in ref[BAD])
-        assert ref[BAD][0][1] == (config == "filtered")  # the failed solve skips the CPI
+        assert ref[BAD][0][1][0] == (config == "filtered")  # the failed solve skips the CPI
         assert rec["maxhold"] == (capi.FILTER_FAILED if config == "filtered" else capi.ERR_NONFINITE)
         held = [dict((n, v) for n, v, *_ in r)["iqdata_stash"].count(b",[]") + 1 for r in ref[1:]]
         assert max(held) == 20 and held[-1] == 20  # the IQ-data window fills and evicts

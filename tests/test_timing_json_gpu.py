@@ -15,8 +15,8 @@ from blah2_b200 import capi
 from blah2_b200.process import Pipeline, timing_render_host
 from blah2_b200.scene import Target, make_scene
 from oracle.stash_timing import Stash
-from test_shared_history_gpu import (BAD, DET, DET_DIRECT, FS, METRICS, N, N_CPI, PATHS, TRK, Feeder, _products,
-                                     _scenes, _ts)
+from cpi_products import cpi_products
+from test_shared_history_gpu import BAD, DET, DET_DIRECT, FS, METRICS, N, N_CPI, PATHS, TRK, Feeder, _scenes, _ts
 
 pytestmark = pytest.mark.gpu
 
@@ -100,7 +100,7 @@ def test_stage_off_and_on_give_identical_outputs_on_every_path():
                 out = []
                 for k in range(14):
                     feed.submit(pipe, k)
-                    out.append(_products(pipe, k))
+                    out.append(cpi_products(pipe, _ts(k)))
                     if on:
                         code = _code(lambda: pipe.fetch_timing_json(_ts(k)))
                         assert code == (capi.FILTER_FAILED if (config, k) == ("filtered", BAD) else capi.OK)
