@@ -241,6 +241,8 @@ SIGNATURES = [
     ("b200dd_tracker_destroy", None, [_VP]),
     ("b200dd_tracker_reset", C.c_int, [_VP]),
     ("b200dd_tracker_max_bytes", C.c_size_t, [_VP]),
+    ("b200dd_tracker_reserve", C.c_int, [_VP, C.c_uint32, C.c_uint32, _VP]),
+    ("b200dd_tracker_usage", C.c_int, [_VP, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _VP]),
     ("b200dd_tracker_process_device", C.c_int, [_VP, _VP, _VP, _VP, _VP, C.c_uint64, _VP]),
     ("b200dd_tracker_process_host", C.c_int, [_VP, _VP, _VP, _VP, C.c_uint32, C.c_uint64, _VP]),
     ("b200dd_tracker_fetch", C.c_int, [_VP, C.c_uint64, _VP, C.c_size_t, C.POINTER(C.c_size_t), _VP]),

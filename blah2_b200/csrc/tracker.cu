@@ -228,6 +228,48 @@ __global__ void __launch_bounds__(kThreads) tr_append_kernel(TrArgs a, const dou
   }
 }
 
+// b200dd_tracker_reserve: every old slot's values and history rows moved to the new stride (o = the old arrays, a =
+// the new, every slot index kept), the position arrays copied, the new slots pushed above the free stack's top, and
+// the state copied with the larger free count.  Old and new never alias, so no thread reads what another writes.
+__global__ void tr_repack_kernel(TrArgs o, TrArgs a) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x, g0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  for (size_t g = g0; g < (size_t)o.slots * o.H; g += stride) {
+    const uint32_t slot = (uint32_t)(g / o.H), k = (uint32_t)(g - (size_t)slot * o.H);
+    a.hd[(size_t)slot * a.H + k] = o.hd[g];
+    a.hf[(size_t)slot * a.H + k] = o.hf[g];
+    if (k < o.W) a.st[(size_t)slot * a.W + k] = o.st[(size_t)slot * o.W + k];
+    if (k == 0) {
+      a.cur_delay[slot] = o.cur_delay[slot];
+      a.cur_doppler[slot] = o.cur_doppler[slot];
+      a.acc[slot] = o.acc[slot];
+      a.id[slot] = o.id[slot];
+      a.len[slot] = o.len[slot];
+    }
+  }
+  const uint32_t ft = o.s->free_top, added = a.slots - o.slots;
+  for (size_t i = g0; i < a.slots; i += stride) {
+    a.order[i] = i < o.slots ? o.order[i] : 0u;
+    a.counter[i] = i < o.slots ? o.counter[i] : 0u;  // positions never reached count from 0
+    if (i < ft) a.free_list[i] = o.free_list[i];
+    else if (i < (size_t)ft + added) a.free_list[i] = a.slots - 1 - (uint32_t)(i - ft);
+  }
+  if (g0 == 0) {
+    TrState z = *o.s;  // an overflowed handle stays overflowed
+    z.free_top = ft + added;
+    *a.s = z;
+  }
+}
+
+// b200dd_tracker_usage: the longest history among the live tracks
+__global__ void tr_usage_kernel(TrArgs a, uint32_t *longest) {
+  const uint32_t n = a.s->n;
+  uint32_t m = 0;
+  for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x)
+    m = max(m, a.len[a.order[p]]);
+  m = __reduce_max_sync(0xFFFFFFFFu, m);
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(longest, m);
+}
+
 __global__ void tr_reset_kernel(TrArgs a) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.slots; i += gridDim.x * blockDim.x) {
     a.free_list[i] = a.slots - 1 - i;  // slots are taken from the top: 0, 1, 2, ...
@@ -407,21 +449,48 @@ int check_params(const b200dd_tracker_params *p, uint32_t max_tracks, uint32_t m
 
 size_t slot_bytes(uint32_t H) { return 16 * (size_t)H + 4 * (size_t)((H + 15) / 16) + 52; }
 
+// The arrays sized by the limits: create allocates them, reserve allocates larger ones and repacks into them.
+struct TrStore {
+  DevBuf<TrState> s;
+  DevBuf<uint32_t> order, order_tmp, free_list, counter, id, len, st;
+  DevBuf<double> cur_delay, cur_doppler, acc, hd, hf;
+  DevBuf<uint32_t> item_len, tile_len, tile_off;
+
+  cudaError_t alloc(size_t S, uint32_t H) {
+    const size_t W = (H + 15) / 16, tiles = (S + kThreads - 1) / kThreads;
+    for (cudaError_t e : {s.alloc(1), order.alloc(S), order_tmp.alloc(S), free_list.alloc(S), counter.alloc(S),
+                          cur_delay.alloc(S), cur_doppler.alloc(S), acc.alloc(S), id.alloc(S), len.alloc(S),
+                          hd.alloc(S * H), hf.alloc(S * H), st.alloc(S * W), item_len.alloc(S),
+                          tile_len.alloc(tiles), tile_off.alloc(tiles + 1)})
+      if (e != cudaSuccess) return e;
+    return cudaSuccess;
+  }
+  // the kernels' view of the arrays at `slots` x H
+  void bind(TrArgs &a, RenderArgs &r, uint32_t slots, uint32_t H) const {
+    a.s = s; a.order = order; a.order_tmp = order_tmp; a.free_list = free_list; a.counter = counter;
+    a.cur_delay = cur_delay; a.cur_doppler = cur_doppler; a.acc = acc; a.id = id; a.len = len; a.hd = hd;
+    a.hf = hf; a.st = st;
+    a.slots = slots;
+    a.H = H;
+    a.W = (H + 15) / 16;
+    r.item_len = item_len; r.tile_len = tile_len; r.tile_off = tile_off;
+  }
+};
+
 }  // namespace
 
 struct b200dd_tracker {
   int device = 0;
   Stream stream;
   b200dd_tracker_params p{};
-  uint32_t slots = 0, H = 0, W = 0, tiles = 0, nh = 0;
+  uint32_t slots = 0, H = 0, tiles = 0, nh = 0;
   size_t max_bytes = 0;
   TrArgs a{};      // the kernels' view of the arrays below
   RenderArgs r{};
-  DevBuf<TrState> d_s;
-  DevBuf<uint32_t> d_order, d_order_tmp, d_free_list, d_counter, d_id, d_len, d_st;
-  DevBuf<double> d_cur_delay, d_cur_doppler, d_acc, d_hd, d_hf, d_acc_init;
+  TrStore store;
+  DevBuf<double> d_acc_init;
   DevBuf<TrInfo> d_info;
-  DevBuf<uint32_t> d_item_len, d_tile_len, d_tile_off;
+  DevBuf<uint32_t> d_longest;  // b200dd_tracker_usage
   DevBuf<char> d_body;
   size_t body_alloc = 0;
   DevBuf<double> d_in;  // process_host staging: delay, doppler
@@ -456,7 +525,6 @@ int b200dd_tracker_create(const b200dd_tracker_params *params, uint32_t max_trac
   h->p = *params;
   h->slots = max_tracks;
   h->H = max_history;
-  h->W = (max_history + 15) / 16;
   h->tiles = (max_tracks + kThreads - 1) / kThreads;
   h->nh = (uint32_t)acc.size();
   h->max_bytes = kHeadBound + (size_t)max_tracks * item_bound(max_history);
@@ -465,36 +533,17 @@ int b200dd_tracker_create(const b200dd_tracker_params *params, uint32_t max_trac
   if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
   TrArgs &a = h->a;
   RenderArgs &r = h->r;
-  const size_t S = max_tracks;
   B2_CUDA(h->stream.create());
-  B2_CUDA(h->d_s.alloc(1));
-  B2_CUDA(h->d_order.alloc(S));
-  B2_CUDA(h->d_order_tmp.alloc(S));
-  B2_CUDA(h->d_free_list.alloc(S));
-  B2_CUDA(h->d_counter.alloc(S));
-  B2_CUDA(h->d_cur_delay.alloc(S));
-  B2_CUDA(h->d_cur_doppler.alloc(S));
-  B2_CUDA(h->d_acc.alloc(S));
-  B2_CUDA(h->d_id.alloc(S));
-  B2_CUDA(h->d_len.alloc(S));
-  B2_CUDA(h->d_hd.alloc(S * h->H));
-  B2_CUDA(h->d_hf.alloc(S * h->H));
-  B2_CUDA(h->d_st.alloc(S * h->W));
+  B2_CUDA(h->store.alloc(max_tracks, max_history));
   B2_CUDA(h->d_acc_init.alloc(acc.size()));
   B2_CUDA(cudaMemcpy(h->d_acc_init, acc.data(), sizeof(double) * acc.size(), cudaMemcpyHostToDevice));
   B2_CUDA(h->d_info.alloc(1));
-  B2_CUDA(h->d_item_len.alloc(S));
-  B2_CUDA(h->d_tile_len.alloc(h->tiles));
-  B2_CUDA(h->d_tile_off.alloc(h->tiles + 1));
-  a.s = h->d_s; a.order = h->d_order; a.order_tmp = h->d_order_tmp; a.free_list = h->d_free_list;
-  a.counter = h->d_counter; a.cur_delay = h->d_cur_delay; a.cur_doppler = h->d_cur_doppler; a.acc = h->d_acc;
-  a.id = h->d_id; a.len = h->d_len; a.hd = h->d_hd; a.hf = h->d_hf; a.st = h->d_st; a.acc_init = h->d_acc_init;
-  r.info = h->d_info; r.item_len = h->d_item_len; r.tile_len = h->d_tile_len; r.tile_off = h->d_tile_off;
+  B2_CUDA(h->d_longest.alloc(1));
+  h->store.bind(a, r, max_tracks, max_history);
+  a.acc_init = h->d_acc_init;
+  r.info = h->d_info;
   const double c = (double)299792458u;  // Constants::c, blah2.cpp:193-194
   a.nh = h->nh;
-  a.slots = max_tracks;
-  a.H = h->H;
-  a.W = h->W;
   a.m = params->m;
   a.n = params->n;
   a.n_delete = params->n_delete;
@@ -525,6 +574,48 @@ int b200dd_tracker_reset(b200dd_tracker *h) {
 }
 
 size_t b200dd_tracker_max_bytes(const b200dd_tracker *h) { return h ? h->max_bytes : 0; }
+
+int b200dd_tracker_reserve(b200dd_tracker *h, uint32_t max_tracks, uint32_t max_history, void *stream) {
+  if (!h) return arg_fail("b200dd_tracker_reserve: null handle");
+  const uint32_t S = std::max(max_tracks, h->slots), H = std::max(max_history, h->H);
+  if (S == h->slots && H == h->H) return B200DD_OK;
+  int rc = check_params(&h->p, S, H, "b200dd_tracker_reserve");
+  if (rc != B200DD_OK) return rc;
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream_or(stream, h->stream);
+  TrStore next;
+  B2_CUDA(next.alloc(S, H));
+  TrArgs a = h->a;
+  RenderArgs r = h->r;
+  next.bind(a, r, S, H);
+  tr_repack_kernel<<<kAppendBlocks, kThreads, 0, st>>>(h->a, a);
+  B2_LAUNCH_CHECK();
+  h->store = std::move(next);  // cudaFree waits for the device, the repack included, before it frees the old arrays
+  h->a = a;
+  h->r = r;
+  h->slots = S;
+  h->H = H;
+  h->tiles = (S + kThreads - 1) / kThreads;
+  h->max_bytes = kHeadBound + (size_t)S * item_bound(H);
+  return B200DD_OK;
+}
+
+int b200dd_tracker_usage(b200dd_tracker *h, uint32_t *live_tracks, uint32_t *longest_history, void *stream) {
+  if (!h || !live_tracks || !longest_history) return arg_fail("b200dd_tracker_usage: null argument");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = stream_or(stream, h->stream);
+  B2_CUDA(cudaMemsetAsync(h->d_longest, 0, sizeof(uint32_t), st));
+  tr_usage_kernel<<<std::min<uint32_t>(h->tiles, kAppendBlocks), kThreads, 0, st>>>(h->a, h->d_longest);
+  B2_LAUNCH_CHECK();
+  TrState s;
+  uint32_t longest;
+  B2_CUDA(cudaMemcpyAsync(&s, h->a.s, sizeof(s), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(&longest, h->d_longest, sizeof(longest), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  *live_tracks = s.n;
+  *longest_history = longest;
+  return B200DD_OK;
+}
 
 int b200dd_tracker_process_device(b200dd_tracker *h, const double *d_delay, const double *d_doppler,
                                   const double *d_snr, const uint32_t *d_count, uint64_t timestamp, void *stream) {
@@ -572,7 +663,7 @@ int b200dd_tracker_fetch(b200dd_tracker *h, uint64_t timestamp, char *out, size_
   B2_CUDA(cudaMemsetAsync(h->r.info, 0, sizeof(TrInfo), st));
   tr_len_kernel<<<h->tiles, kThreads, 0, st>>>(h->a, h->r);
   B2_LAUNCH_CHECK();
-  scan_kernel<<<1, 1024, 0, st>>>(h->d_tile_len, h->d_tile_off, (int)h->tiles, &h->d_info->body);
+  scan_kernel<<<1, 1024, 0, st>>>(h->store.tile_len, h->store.tile_off, (int)h->tiles, &h->d_info->body);
   B2_LAUNCH_CHECK();
   TrState s;
   TrInfo info;

@@ -762,6 +762,17 @@ class Tracker(_Handle):
     def reset(self):
         capi.check(self._lib.b200dd_tracker_reset(self._h))
 
+    def reserve(self, max_tracks, max_history, stream=None):
+        """Raise the limits to at least max_tracks x max_history, keeping every track (b200dd_tracker_reserve)."""
+        capi.check(self._lib.b200dd_tracker_reserve(self._h, int(max_tracks), int(max_history), self._st(stream)))
+        self.max_bytes = int(self._lib.b200dd_tracker_max_bytes(self._h))
+
+    def usage(self, stream=None):
+        """(live tracks, longest history among them) after the work enqueued so far (synchronous)."""
+        live, longest = C.c_uint32(), C.c_uint32()
+        capi.check(self._lib.b200dd_tracker_usage(self._h, C.byref(live), C.byref(longest), self._st(stream)))
+        return live.value, longest.value
+
 
 def record_bytes(max_detections, n_spectrum=0, timing=False, detection=True) -> int:
     """The size of a pipeline's CPI record (b200dd_pipeline_enable_export): a 64-byte header, 80 bytes of stage stamps

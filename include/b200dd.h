@@ -603,9 +603,9 @@ B200DD_API size_t b200dd_timing_max_bytes(void);
  * The document is {"timestamp":T,"n":..,"nTentative":..,"nAssociated":..,"nActive":..,"nCoasting":..,"data":[..]},
  * every double written once at two decimals (delays stay in bins).
  *
- * Limits: the reference has none.  max_tracks live tracks and max_history entries per track are create-time limits;
- * a CPI that would exceed either puts the handle in an overflowed state in which process does nothing and fetch
- * returns B200DD_ERR_CAPACITY with *n_bytes = 0, until b200dd_tracker_reset.  Inactivity counters are 32-bit.
+ * Limits: the reference has none.  max_tracks live tracks and max_history entries per track are set at creation and
+ * raised by b200dd_tracker_reserve; a CPI that would exceed either puts the handle in an overflowed state in which
+ * process does nothing and fetch returns B200DD_ERR_CAPACITY with *n_bytes = 0, until b200dd_tracker_reset.  Inactivity counters are 32-bit.
  * Device memory: 16 max_history + 4 ceil(max_history / 16) + 52 bytes per track slot, plus the document body
  * (grown to the largest document fetched so far).
  */
@@ -633,6 +633,20 @@ B200DD_API void b200dd_tracker_destroy(b200dd_tracker *h);
 B200DD_API int b200dd_tracker_reset(b200dd_tracker *h);
 /* The document size bound of the handle's limits. */
 B200DD_API size_t b200dd_tracker_max_bytes(const b200dd_tracker *h);
+/* Raises the limits of a live handle to max(max_tracks, current) x max(max_history, current) without changing its
+ * state: every track, its history, the order of the tracks, the inactivity counters, the id counter and the timestamp
+ * carry over, and every later document is the one a handle created at the larger limits gives.  The new limits'
+ * arrays are allocated, a kernel on `stream` (NULL = the handle's stream) moves the state into them, and the old
+ * arrays are freed (cudaFree waits for the device).  A request that raises neither limit does nothing.
+ * B200DD_ERR_ARG, with the handle unchanged, where b200dd_tracker_plan refuses the new limits.  An overflowed handle
+ * stays overflowed.  The growth rule belongs to the caller: before a CPI of n detections, live + n * n_hypotheses
+ * tracks and longest + 2 history entries cannot overflow (every unassociated detection starts n_hypotheses tracks,
+ * and a CPI adds at most the association and the prediction to a history). */
+B200DD_API int b200dd_tracker_reserve(b200dd_tracker *h, uint32_t max_tracks, uint32_t max_history, void *stream);
+/* The live track count and the longest history among the live tracks, after the work enqueued on `stream`
+ * (NULL = the handle's stream).  Synchronises `stream`. */
+B200DD_API int b200dd_tracker_usage(b200dd_tracker *h, uint32_t *live_tracks, uint32_t *longest_history,
+                                    void *stream);
 /* Tracker::process(detection, timestamp) on a device detection list: d_delay (bins), d_doppler (Hz) doubles whose
  * length is the device word *d_count (d_snr is accepted for the Detection's shape; the tracker never reads it).
  * Asynchronous on `stream` (NULL = the handle's stream): no host synchronisation and no count read on the host. */
