@@ -264,6 +264,7 @@ struct ShareSet {
 // how far they have got with it.
 struct LastCpi {
   void *stream = nullptr;  // the stream it was submitted on: its products are there, its fetches run there
+  bool in_flight = false;  // no b200dd_pipeline_fetch or prepare has synchronised it yet (see order_after_last)
   // stage_bit: set by every submit, cleared when the stage is enabled or the pipeline joins a share set.  A stage
   // whose bit is clear has no CPI submitted since then to fetch.
   unsigned stages = 0;
@@ -313,6 +314,7 @@ struct b200dd_pipeline {
   DevBuf<short4> d_iq16;       // int16 ingest staging
   DevBuf<int8_t> d_x8, d_y8;   // int8 ingest staging, 2 N bytes per channel
   LastCpi last;
+  Event last_ev;  // recorded on last.stream when another stream must wait for the last CPI
   // CUDA-graph replay of the device chain (b200dd_pipeline_submit_device): one instantiated graph per
   // (d_x, d_y, d_map) triple given to b200dd_pipeline_prepare_device
   struct GraphEntry {
@@ -490,6 +492,7 @@ int b200dd_pipeline_create(const b200dd_pipeline_params *params, b200dd_pipeline
   rc = b200dd_det_create(&dp, h->g.n_doppler_bins, h->g.n_delay_bins, &h->det);  // also serves set_metrics
   if (rc != B200DD_OK) return rc;
   B2_CUDA(h->stream.create());
+  B2_CUDA(h->last_ev.create(cudaEventDisableTiming));
   B2_CUDA(h->d_map.alloc((size_t)h->g.n_doppler_bins * h->g.n_delay_bins));
   if (h->wh) B2_CUDA(h->d_yf.alloc(params->caf.n_samples));
   *out = h.release();
@@ -695,6 +698,7 @@ static int pipeline_enqueue_device(b200dd_pipeline *h, const void *d_x, const vo
 static void pipeline_submitted(b200dd_pipeline *h, int path, void *st, const void *map, bool packed) {
   LastCpi &c = h->last;
   c.stream = st;
+  c.in_flight = true;
   c.stages = kAllBits;
   c.path = path;
   c.filter = h->wh != nullptr;
@@ -721,6 +725,19 @@ static const b200dd_pipeline::GraphEntry *pipeline_find_graph(const b200dd_pipel
   return nullptr;
 }
 
+// Every CPI shares the pipeline's buffers (the filtered channel, the CAF scratch, the detection list, the status
+// word), so a submit or fetch on `st` must run after the last CPI.  On that CPI's own stream, stream order does it and
+// nothing is enqueued; on another stream, while no fetch or prepare has synchronised the CPI, `st` waits for an event
+// recorded on the CPI's stream.  The host never waits here.  So the stream a CPI was submitted on must stay alive
+// until the CPI is fetched, which its fetches need anyway.
+static int order_after_last(b200dd_pipeline *h, void *st) {
+  if (!h->last.in_flight || st == h->last.stream) return B200DD_OK;
+  DeviceGuard guard(h->device);
+  B2_CUDA(cudaEventRecord(h->last_ev, (cudaStream_t)h->last.stream));
+  B2_CUDA(cudaStreamWaitEvent((cudaStream_t)st, h->last_ev, 0));
+  return B200DD_OK;
+}
+
 // A share-set member takes one CPI at a time: B200DD_ERR_ARG while its last one is not fetched.
 static int member_may_submit(const b200dd_pipeline *h, const char *entry) {
   return h->set && h->last.unfetched ? entry_fail(entry, "the share-set member's last CPI is not fetched yet")
@@ -728,11 +745,12 @@ static int member_may_submit(const b200dd_pipeline *h, const char *entry) {
 }
 
 // The start of submit `entry`: B200DD_ERR_ARG for a null argument (`args` false) and from member_may_submit; *st the
-// caller's stream, else the pipeline's.
-static int submit_start(const b200dd_pipeline *h, const char *entry, bool args, void *stream, cudaStream_t *st) {
+// caller's stream, else the pipeline's, ordered after the last CPI.
+static int submit_start(b200dd_pipeline *h, const char *entry, bool args, void *stream, cudaStream_t *st) {
   if (!args) return entry_fail(entry, "null argument");
   *st = stream_or(stream, h->stream);
-  return member_may_submit(h, entry);
+  const int rc = member_may_submit(h, entry);
+  return rc != B200DD_OK ? rc : order_after_last(h, *st);
 }
 
 // A CPI is 12+ kernel launches on the single submitting thread.  The chain's arguments only depend on the caller's
@@ -773,6 +791,7 @@ int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const vo
   if (!pipeline_find_graph(h, d_x, d_y, n, d_map)) {
     // the eager run sets up what a capture must not do (uploads the axes, sizes scratch buffers); it is a CPI
     int rc = member_may_submit(h, entry);
+    if (rc == B200DD_OK) rc = order_after_last(h, st);  // before the capture, which must not wait on outside work
     if (rc != B200DD_OK) return rc;
     rc = pipeline_enqueue_device(h, d_x, d_y, n, d_map, kTmDevice, st);
     if (rc != B200DD_OK) return rc;
@@ -795,6 +814,7 @@ int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const vo
     }
   }
   B2_CUDA(cudaStreamSynchronize((cudaStream_t)st));
+  if (h->last.stream == st) h->last.in_flight = false;
   return B200DD_OK;
 }
 
@@ -911,13 +931,16 @@ int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double 
   result->n_detections = 0;
   result->noise_power = 0.0;
   result->max_power = 0.0;
+  int rc = order_after_last(h, st);  // after the share set's max-hold push, which runs on the CPI's stream
+  if (rc != B200DD_OK) return rc;
   int fs;
-  int rc = read_status(h, (cudaStream_t)st, false, &fs);
+  rc = read_status(h, (cudaStream_t)st, false, &fs);
   if (rc != B200DD_OK) return rc;
   double metrics[2] = {0.0, 0.0};
   uint32_t n = 0;
   rc = b200dd_det_chain_fetch(h->det, metrics, o_delay, o_doppler, o_snr, cap, &n, st);  // synchronises st
   if (rc == B200DD_OK || rc == B200DD_ERR_CAPACITY) {
+    h->last.in_flight = false;
     h->last.tm_fetched = true;
     h->last.tm_fs = fs;
   }
@@ -937,7 +960,7 @@ int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double 
 // The start of host submit `entry` (submit_start, on the pipeline's stream) and its sample counts, checked in this
 // order: the clutter filter and the CAF read *need samples of x and y, and the spectrum reads nfft <= n_samples
 // samples of x (SpectrumAnalyser.cpp:36-39), so *need_x of x are copied.
-static int host_start(const b200dd_pipeline *h, const char *entry, bool args, uint32_t n, uint32_t *need,
+static int host_start(b200dd_pipeline *h, const char *entry, bool args, uint32_t n, uint32_t *need,
                       uint32_t *need_x) {
   cudaStream_t st;
   const int rc = submit_start(h, entry, args, nullptr, &st);
@@ -1111,10 +1134,11 @@ int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32
 }
 
 int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectrum_out, uint32_t cap) {
-  const int rc = fetch_check(h, "b200dd_pipeline_fetch_spectrum", kSpectrum, spectrum_out, nullptr);
+  int rc = fetch_check(h, "b200dd_pipeline_fetch_spectrum", kSpectrum, spectrum_out, nullptr);
   if (rc != B200DD_OK) return rc;
   if (cap < h->spec_bins) return arg_fail("b200dd_pipeline_fetch_spectrum: capacity too small");
-  return b200dd_spectrum_fetch(h->spec, spectrum_out, h->stream);
+  rc = order_after_last(h, h->stream);
+  return rc != B200DD_OK ? rc : b200dd_spectrum_fetch(h->spec, spectrum_out, h->stream);
 }
 
 int b200dd_pipeline_enable_map_json(b200dd_pipeline *h, size_t *max_bytes) {
@@ -1493,7 +1517,9 @@ int b200dd_pipeline_stamp(b200dd_pipeline *h, int slot, void *stream) {
   if (slot < B200DD_STAMP_CHAIN || slot > B200DD_STAMP_CLUTTER) return arg_fail("b200dd_pipeline_stamp: not a boundary slot");
   if (!h->tm_on) return B200DD_OK;
   DeviceGuard guard(h->device);
-  const int rc = tm_stamp(h, kStampSlots[slot], stream_or(stream, h->stream));
+  const cudaStream_t st = stream_or(stream, h->stream);
+  int rc = order_after_last(h, st);  // the stamps are the last CPI's until the next submit
+  if (rc == B200DD_OK) rc = tm_stamp(h, kStampSlots[slot], st);
   if (rc == B200DD_OK) h->tm_pre |= 1u << slot;
   return rc;
 }

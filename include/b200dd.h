@@ -740,7 +740,11 @@ B200DD_API int b200dd_pipeline_submit_host_cf32(b200dd_pipeline *h, const float 
                                                 double *map_out);
 
 /* DEVICE buffers (float2), asynchronous on `stream` (NULL = the pipeline's stream).  d_map
- * (nullable) receives the float2 map.  Results stay on the device until b200dd_pipeline_fetch. */
+ * (nullable) receives the float2 map.  Results stay on the device until b200dd_pipeline_fetch.
+ * Ordering: every submit entry (this one, prepare_device, submit_host*, submit_map, submit_record) runs after the
+ * pipeline's last CPI, whatever stream either uses: when the last CPI went on another stream and has not been fetched,
+ * the new stream waits for it on the device (the host never waits).  On the last CPI's own stream nothing extra is
+ * enqueued.  The stream a CPI was submitted on must stay alive until the CPI is fetched. */
 B200DD_API int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n,
                                              void *d_map, void *stream);
 /* Plan creation for the device path (optional): records the whole chain for this (d_x, d_y, d_map) triple as a CUDA
@@ -751,6 +755,8 @@ B200DD_API int b200dd_pipeline_submit_device(b200dd_pipeline *h, const void *d_x
  * enqueued eagerly.  Where the chain cannot be captured, the pipeline stays eager and this call does nothing. */
 B200DD_API int b200dd_pipeline_prepare_device(b200dd_pipeline *h, const void *d_x, const void *d_y, uint32_t n,
                                               void *d_map, void *stream);
+/* The last CPI's clutter-filter status, set_metrics and detection list into host memory, read on `stream` (NULL =
+ * the pipeline's stream) after that CPI, whichever stream it was submitted on; returns when they are there. */
 B200DD_API int b200dd_pipeline_fetch(b200dd_pipeline *h, b200dd_cpi_result *result, double *o_delay,
                                      double *o_doppler, double *o_snr, uint32_t cap, void *stream);
 B200DD_API void *b200dd_pipeline_stream(b200dd_pipeline *h);
@@ -759,7 +765,7 @@ B200DD_API void *b200dd_pipeline_stream(b200dd_pipeline *h);
  * the reference channel of every CPI submitted afterwards, evaluated on the samples already resident on the
  * device (no extra transfer).  *n_spectrum (nullable) receives the number of bins.  The spectrum of the last
  * submitted CPI is read with b200dd_pipeline_fetch_spectrum (call it after b200dd_pipeline_fetch, or it
- * synchronises the pipeline's stream itself). */
+ * waits for that CPI itself). */
 B200DD_API int b200dd_pipeline_enable_spectrum(b200dd_pipeline *h, double bandwidth, uint32_t *n_spectrum);
 B200DD_API int b200dd_pipeline_fetch_spectrum(b200dd_pipeline *h, double *spectrum_out, uint32_t cap);
 
